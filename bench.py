@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""clips/sec forward+backward of the ClipBERT hot path on N B200s (one process per GPU).
+"""clips/sec forward+backward of the ClipBERT hot path on N H100s (one process per GPU).
 
-  python bench.py --gpus 1 --steps 20 --warmup 5                      # this repo's sm_100a path
+  python bench.py --gpus 1 --steps 20 --warmup 5                      # this repo's sm_90a path
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
   python bench.py --impl reference ...                                # the reference's CPU path (oracle port)
 
@@ -20,11 +20,18 @@ JSON keys beyond the base contract:
   value     clips/s with the batch already resident in HBM (device-timed, CUDA events, max over ranks)
   e2e       same metric through the public API (ClipBert.forward on a batch dict) with HOST (pinned)
             uint8 frames / ids / masks / labels copied H2D and the loss copied D2H every step
-  roofline  the tcgen05 GEMM kernel (all convs + linears, fwd/dgrad/wgrad): algorithmic FLOPs per step
+  roofline  the wgmma GEMM kernel (all convs + linears, fwd/dgrad/wgrad): algorithmic FLOPs per step
             / device time of its launches (the step's cb_gemm calls replayed back to back from a CUDA
             graph on one stream right after the timed region, CUDA events around the replay), against
             MEASURED_PEAKS.json
   cpu_baseline  the CPU oracle (oracle/clipbert_ref.py, a port: kind "port") on this host's cores
+
+--dump-outputs DIR writes, after the timed steps, what the timed path computed in its last step as DIR/<name>.npy: the loss
+(training) and the logits of every (clip, text row), and for training a fixed sample of the parameter gradients
+(grad_sample.npy: up to 4096 seeded positions of every trainable parameter, in named_parameters order) with the norm of every
+parameter gradient (grad_norms.npy, float64). The inputs, weights and dropout streams are seeded, so two builds run with the
+same arguments can be compared output for output (the weight gradients are summed with fp32 atomics, so they agree to
+rounding, not bit for bit).
 """
 import argparse
 import json
@@ -61,8 +68,8 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(tflops=d.get("bf16_tflops_sustained", 1464.0), hbm=d.get("hbm_gbs", 6489.9), src="measured")
-    return dict(tflops=1400.0, hbm=6650.0, src="fallback")
+        return dict(tflops=d.get("bf16_tflops_sustained", 989.0), hbm=d.get("hbm_gbs", 3350.0), src="measured")
+    return dict(tflops=989.0, hbm=3350.0, src="H100 SXM data sheet (dense bf16, HBM3)")
 
 
 def _device(local_rank):
@@ -134,11 +141,6 @@ def gemm_algorithmic_bytes(kw):
     return b
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch from the committed `ncu --set full` capture
-# (profiles/r02z_ncu_full_gemm_summary.txt, profiled launch 4: the committed round-2 kernel), keyed by the launch's shape
-NCU_TRAFFIC_BYTES = {(401408, 256, 64, 1, True): 257.406208e6 + 162.649600e6}
-
-
 def hbm_bound_launch(ops, rec, stream, peaks, reps=20):
     cand = [kw for kw in rec if "group" not in kw and kw.get("mode", 0) != 1 and kw.get("ntaps", 1) == 1 and kw["k"] <= 128 and kw["m"] >= 4096]
     if not cand:
@@ -156,13 +158,11 @@ def hbm_bound_launch(ops, rec, stream, peaks, reps=20):
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / reps
     gbs = nbytes / us / 1e3
-    key = (kw["m"], kw["n"], kw["k"], kw.get("ntaps", 1), kw.get("residual") is not None)
     return dict(bound="hbm", kernel="cb::gemm_kernel 1x1 conv + FrozenBN shift%s + ReLU, m=%d n=%d k=%d" % (
                     " + shortcut" if kw.get("residual") is not None else "", kw["m"], kw["n"], kw["k"]),
                 achieved=round(gbs, 1), peak=peaks["hbm"], unit="GB/s", frac=round(gbs / peaks["hbm"], 4),
-                peak_source="%s hbm_gbs (copy bandwidth)" % peaks["src"], algorithmic_bytes=int(nbytes), us_per_launch=round(us, 2),
-                traffic=NCU_TRAFFIC_BYTES.get(key), traffic_source="profiles/r02z_ncu_full_gemm_summary.txt (ncu --set full, one launch)",
-                note="%d back-to-back launches of the same problem, CUDA events on the launch stream; working set %.0f MB > 126 MB L2"
+                peak_source="%s hbm_gbs (copy bandwidth)" % peaks["src"], algorithmic_bytes=int(nbytes), us_per_launch=round(us, 2), traffic=None,
+                note="%d back-to-back launches of the same problem, CUDA events on the launch stream; working set %.0f MB > 50 MB L2"
                      % (reps, nbytes / 1e6))
 
 
@@ -265,8 +265,8 @@ def run_b200(args):
     model.zero_grad_in_forward = bool(args.zero_grad_in_forward) and not args.inference
     exchange = args.exchange
     if world > 1:
-        if exchange == "auto":       # this library's NVLS all-reduce where the box has a multicast mapping (N = 8: 0.956 of linear against
-            exchange = "nvls" if cb.ClipBert.nvls_available(device=dev) else "nccl"          # 0.920 with NCCL, profiles/r02_multi_gpu.txt)
+        if exchange == "auto":       # this library's NVLS all-reduce where the node has a multicast mapping
+            exchange = "nvls" if cb.ClipBert.nvls_available(device=dev) else "nccl"
         model.enable_overlapped_allreduce(cnn_buckets=bool(args.cnn_buckets), exchange=exchange, max_ctas=args.nvls_ctas, wire=args.wire, tail_ctas=args.nvls_tail_ctas)
 
     opt = None
@@ -289,6 +289,10 @@ def run_b200(args):
         for k in host:
             dbuf[k].copy_(host[k], non_blocking=True)
 
+    # outputs of the latest fwd_bwd (under graph replay: the graph's own buffers, rewritten by every replay), detached: holding
+    # their autograd history would keep the pass's backward state alive into the next pass
+    last = {}
+
     def fwd_bwd():
         if args.inference:         # inference_retrieval (run_video_retrieval.py:629-734): CNN once per video, then the captions
             with torch.no_grad():
@@ -296,6 +300,7 @@ def run_b200(args):
                 mb = dict(text_input_ids=dbuf["text_input_ids"], text_input_mask=dbuf["text_input_mask"], n_examples_list=[n_ex] * B)
                 logits = model.forward_clips(mb, n_clips, grid=grid)["logits"]
                 loss_dev.copy_(logits.float().mean().reshape(1))          # the per-step result read back by the e2e leg
+            last["logits"] = logits.detach()
             return
         if args.clip_batching:     # SURVEY §8 f1: the n_clips passes of the reference loop as ONE pass over B*n_clips units
             mb = dict(visual_inputs=dbuf["visual_inputs"], text_input_ids=dbuf["text_input_ids"], text_input_mask=dbuf["text_input_mask"],
@@ -312,6 +317,7 @@ def run_b200(args):
                           labels=dbuf["labels"] if args.head == "retrieval" else None, n_examples_list=[n_ex] * B)
                 logits.append(model(mb)["logits"])
         loss = cb.clip_lse_loss(logits, dbuf["labels"]) if args.fused_loss else lse_loss(logits, dbuf["labels"])
+        last["logits"] = logits.detach() if torch.is_tensor(logits) else [l.detach() for l in logits]   # clip loop: stacked only when dumped
         loss.backward()
         if world > 1:
             model.allreduce_grads()       # transformer buffer already in flight since its last backward (overlaps the CNN backward)
@@ -438,6 +444,8 @@ def run_b200(args):
         return float(t.item()), launches, clocks
 
     ms_dev, launches, clocks = timed(step_device, args.steps, args.warmup, sample_clocks=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["logits"], None if args.inference else loss_dev, None if args.inference else model)
     e2e_mode = "serialized"
     ms_e2e = None
     if args.prefetch:
@@ -462,12 +470,12 @@ def run_b200(args):
     value = clips_per_step / (ms_dev / args.steps / 1e3)
     e2e_value = clips_per_step / (ms_e2e / args.steps / 1e3)
 
-    # ---- instrumented pass: device time of the step's tcgen05 GEMM launches ----
+    # ---- instrumented pass: device time of the step's GEMM launches ----
     roof = None
     cpu = None
     try:          # every rank runs the instrumented pass (it contains the collectives); rank 0 reports. Guarded: the primary
                   # metric above must reach the JSON line even if the secondary figures cannot be produced
-        # Device time of the tcgen05 GEMM launches of one step: the cb_gemm descriptors of one eager step are recorded (their
+        # Device time of the GEMM launches of one step: the cb_gemm descriptors of one eager step are recorded (their
         # operand tensors stay referenced), then exactly those launches are replayed back to back from a CUDA graph on ONE
         # stream (no wgrad overlap, no PDL) and timed with CUDA events around the replay. Bracketing every launch with its own
         # event pair instead made the figure depend on the host: the GPU idles between "event recorded" and "kernel enqueued".
@@ -504,7 +512,7 @@ def run_b200(args):
         g1.record()
         torch.cuda.synchronize()
         gemm_ms = g0.elapsed_time(g1) / 5
-        # ---- the largest HBM-bound launch of the step on its own (a 1x1 conv: K <= 128, far below the ~225 FLOP/B ridge) ----
+        # ---- the largest HBM-bound launch of the step on its own (a 1x1 conv: K <= 128, far below the ~295 FLOP/B ridge of an H100 SXM) ----
         try:
             hbm_roof = hbm_bound_launch(ops, rec, gs, peaks)
         except Exception as e:          # never lose the bench line over the secondary figure
@@ -522,7 +530,7 @@ def run_b200(args):
         eager_ms = e0.elapsed_time(e1)
         algo_tf = fl_clip * B * n_clips / 1e12
         achieved = algo_tf / (gemm_ms / 1e3)
-        roof = dict(bound="tensor", kernel="cb::gemm_kernel<BN,MODE> (tcgen05, all convs + linears fwd/dgrad/wgrad)",
+        roof = dict(bound="tensor", kernel="cb::gemm_kernel<BN,MODE,OCC> (wgmma, all convs + linears fwd/dgrad/wgrad)",
                     achieved=round(achieved, 2), peak=peaks["tflops"], unit="TFLOP/s", frac=round(achieved / peaks["tflops"], 4),
                     peak_source="%s bf16_tflops_sustained" % peaks["src"], traffic=None, launches_per_step=n_gemm,
                     gemm_ms_per_step=round(gemm_ms, 3), eager_step_ms=round(eager_ms, 3),
@@ -590,7 +598,7 @@ def run_b200(args):
                    scaling="weak", vs_baseline=None, dtype="bf16", data="synthetic",
                    config=dict(workload=workload_name(args), name=args.config,
                                clips_per_step_per_gpu=B * n_clips, seq_len=L, parallelism="dp%d" % world,
-                               l2="per-step working set (activations + 149 M-parameter operands, > 2 GB) >> 126 MB L2; no explicit flush",
+                               l2="per-step working set (activations + 149 M-parameter operands, > 2 GB) >> 50 MB L2; no explicit flush",
                                cuda_graph=graph is not None, clip_batching=bool(args.clip_batching), pdl=int(args.pdl), mn3d=bool(args.mn3d), group_wgrad=int(args.group_wgrad), occ2=[args.occ2, args.occ2_gflop], overlap_wgrad=bool(args.overlap_wgrad), stem=args.stem,
                                fused_loss=bool(args.fused_loss), zero_grad_in_forward=bool(model.zero_grad_in_forward), attn_rows48=bool(args.attn_rows48), attn_flash_pipe=bool(args.attn_flash_pipe), cnn_buckets=bool(args.cnn_buckets), exchange=exchange, wire=args.wire, sm_limit=args.sm_limit, nccl_ctas=args.nccl_ctas,
                                weight_recast="in the optimizer step (FusedAdamW attached before the loop emits the bf16 operands)" if recast_attached else "inside every step (no optimizer attached)",
@@ -606,6 +614,34 @@ def run_b200(args):
         sys.stdout.flush()
         sys.stderr.flush()
         os._exit(0)
+
+
+GRAD_SAMPLE = 4096      # gradient positions per parameter written by --dump-outputs
+
+
+def dump_outputs(out_dir, logits, loss, model):
+    """--dump-outputs: the last timed step's results as float32 / float64 .npy files (a few MB in all)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    logits = logits if torch.is_tensor(logits) else torch.stack(logits)
+    np.save(os.path.join(out_dir, "logits.npy"), logits.detach().float().cpu().numpy())
+    if loss is not None:
+        np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().cpu().numpy())
+    if model is None:
+        return
+    samples, norms = [], []
+    for i, (_, p) in enumerate(model.named_parameters()):
+        if not p.requires_grad:
+            continue
+        g = p.grad.detach().float().flatten() if p.grad is not None else torch.zeros(p.numel(), device=p.device)
+        norms.append(float(g.double().norm()))
+        if g.numel() > GRAD_SAMPLE:
+            idx = torch.randperm(g.numel(), generator=torch.Generator().manual_seed(i))[:GRAD_SAMPLE].sort().values
+            g = g[idx.to(g.device)]
+        samples.append(g.cpu())
+    np.save(os.path.join(out_dir, "grad_sample.npy"), torch.cat(samples).numpy())
+    np.save(os.path.join(out_dir, "grad_norms.npy"), np.array(norms, dtype=np.float64))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -671,9 +707,9 @@ def run_reference(args):
         return
     b = args.cpu_batch
     sd, batch = _cpu_setup(args, b)
-    for _ in range(max(1, min(args.warmup, 1))):
+    for _ in range(args.warmup):
         _cpu_step(sd, batch, args.n_clips, args.n_frm, args.size)
-    steps = max(1, min(args.steps, 3))
+    steps = max(1, args.steps)
     t0 = time.time()
     for _ in range(steps):
         _cpu_step(sd, batch, args.n_clips, args.n_frm, args.size)
@@ -681,7 +717,7 @@ def run_reference(args):
     val = round(b * args.n_clips / dt, 3)
     L = args.txt_len + (args.size // 32 // 2) ** 2
     out = dict(impl="reference", metric=METRIC_TRAIN, value=val, unit="clips/s", n_gpus=args.gpus,
-               steps=steps, warmup=1, ms_per_step=round(dt * 1e3, 2), higher_is_better=True, scaling="weak", vs_baseline=None, dtype="f32",
+               steps=steps, warmup=args.warmup, ms_per_step=round(dt * 1e3, 2), higher_is_better=True, scaling="weak", vs_baseline=None, dtype="f32",
                data="synthetic",
                config=dict(workload="MSRVTT retrieval train step (bounded CPU sample): %d videos x %d clips x %d frames %dx%d, %d-token text, n_ex=%d"
                            % (b, args.n_clips, args.n_frm, args.size, args.size, args.txt_len, args.n_ex), seq_len=L,
@@ -697,6 +733,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's outputs (logits, loss, sampled gradients) as DIR/<name>.npy")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="headline", choices=sorted(CONFIGS), help="BASELINE.json workload (default: the configuration the metric names)")
@@ -721,22 +759,23 @@ def main():
     ap.add_argument("--fused_loss", type=int, default=1, help="1 (default): clip aggregation + LSE loss fwd+bwd as one kernel (cb_clip_lse_loss); 0: ~45 ATen launches")
     ap.add_argument("--recast_in_step", type=int, default=0, help="1: no optimizer attached before the loop -> fp32 -> bf16 weight re-cast inside every step (round-1 behaviour)")
     ap.add_argument("--exchange", default="auto", choices=["auto", "nccl", "nvls"], help="N>1 gradient exchange: NCCL all-reduce, this library's NVLS all-reduce (csrc/nvls.cu), or auto = nvls where a multicast mapping exists")
-    ap.add_argument("--nvls_ctas", type=int, default=0, help="CTAs of the NVLS all-reduce kernel while it overlaps the backward; 0 (default) = by world size: 64 at N <= 4, "
-                    "32 above (N = 8: 32 -> 0.966 of linear, 64 -> 0.953, 96 -> 0.942; N = 2: 64 -> 10.28 ms/step, 32 -> 11.2, 96 -> 10.37)")
-    ap.add_argument("--nvls_tail_ctas", type=int, default=148, help="CTAs of the NVLS all-reduce of the last, exposed slices (0 = --nvls_ctas)")
+    ap.add_argument("--nvls_ctas", type=int, default=0, help="CTAs of the NVLS all-reduce kernel while it overlaps the backward; 0 (default) = by world size: 64 at N <= 4, 32 above")
+    ap.add_argument("--nvls_tail_ctas", type=int, default=132, help="CTAs of the NVLS all-reduce of the last, exposed slices (0 = --nvls_ctas)")
     ap.add_argument("--wire", default="fp32", choices=["fp32", "bf16"], help="N>1: gradients travel as fp32 (the flat buffers as they are) or as bf16 (cast, all-reduce, cast back: half the payload, the reference's fp16 wire precision)")
     ap.add_argument("--cnn_buckets", type=int, default=1, help="N>1: exchange res5 + grid_encoder gradients mid-backward (default; 0: one CNN exchange at the end)")
     ap.add_argument("--sm_limit", type=int, default=0, help="cap the persistent GEMM grid (0 = all SMs); leaves SMs to the overlapped NCCL kernels")
     ap.add_argument("--nccl_ctas", type=int, default=0, help="N>1: NCCL_MAX_CTAS for the process group (0 = NCCL default)")
     ap.add_argument("--mn3d", type=int, default=1, help="dgrad / wgrad GEMMs: MN-major operands as one 3-D TMA box per k-chunk (default) or BN/64 2-D boxes")
-    ap.add_argument("--group_wgrad", type=int, default=3, help="grouped weight-gradient launches (cb_gemm_wgrad_group): 0 none, 1 BertLayer + bottleneck block, 2 blocks only, 3 BertLayer only (default: measured best), 4 BertLayer as two pairs + blocks")
-    ap.add_argument("--occ2", type=int, default=1, help="two GEMM CTAs per SM: 0 never, 1 only launches the tuning table marks, 2 every eligible launch up to --occ2_gflop")
+    ap.add_argument("--group_wgrad", type=int, default=3, help="grouped weight-gradient launches (cb_gemm_wgrad_group): 0 none, 1 BertLayer + bottleneck block, 2 blocks only, 3 BertLayer only (default), 4 BertLayer as two pairs + blocks")
+    ap.add_argument("--occ2", type=int, default=1, help="two GEMM CTAs per SM: 0 never, 1 only launches that ask for it (cb_gemm_desc.reserved bit 5), 2 every eligible launch up to --occ2_gflop")
     ap.add_argument("--occ2_gflop", type=float, default=0.0, help="with --occ2 2: largest launch (GFLOP) that runs two CTAs per SM (0 = no limit)")
     ap.add_argument("--cpu_batch", type=int, default=4)
     ap.add_argument("--optimizer", type=int, default=1, help="also time the fused AdamW step (informational key fused_optimizer)")
     ap.add_argument("--opt_steps", type=int, default=10, help="timed iterations of the informational fused-optimizer leg")
     ap.add_argument("--no_cpu", type=int, default=0, help="skip the CPU baseline leg (profiling runs)")
     args = apply_config(ap.parse_args())
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs writes the outputs of this repo's GPU path; --impl reference has none to write")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-"""clipbert_b200 — the ClipBERT forward/backward hot path as hand-written sm_100a kernels.
+"""clipbert_b200 — the ClipBERT forward/backward hot path as hand-written sm_90a kernels.
 
 Only what the path needs: ``csrc/`` (CUDA kernels + C ABI), ``_lib``/``ops`` (ctypes binding) and the
 host-side mirrors of the reference module interface (``ClipBert``, ``GridFeatBackbone``,

@@ -1,4 +1,4 @@
-"""ctypes binding of libclipbert_sm100.so (the C ABI declared in include/clipbert_b200.h).
+"""ctypes binding of libclipbert_sm90.so (the C ABI declared in include/clipbert_b200.h).
 
 The product path has no CPU or eager-PyTorch fallback: if the library is missing or fails to load,
 every op raises. torch is used only for device memory, streams and torch.distributed.
@@ -9,7 +9,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "libclipbert_sm100.so")
+LIB_PATH = os.path.join(_HERE, "lib", "libclipbert_sm90.so")
 
 CB_GEMM_TN, CB_GEMM_WGRAD = 0, 1
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_TANH, ACT_GELU_STASH_GRAD = 0, 1, 2, 3, 4

@@ -1,7 +1,7 @@
-"""Build libclipbert_sm100.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libclipbert_sm90.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
 The library is compiled ahead of time into ``clipbert_b200/lib/`` so that it travels with the
-repository snapshot to the GPU box; there is no JIT cache and no torch extension machinery.
+repository tree to the machine that runs it; there is no JIT cache and no torch extension machinery.
 """
 import os
 import subprocess
@@ -12,11 +12,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
-LIB = os.path.join(LIBDIR, "libclipbert_sm100.so")
+LIB = os.path.join(LIBDIR, "libclipbert_sm90.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--use_fast_math", "-Xptxas", "-v",
     "-I", os.path.join(HERE, "..", "include"),
 ]
@@ -48,7 +48,7 @@ def _compile(src, verbose):
 
 
 def build(verbose=False, force=False):
-    """Compile every .cu under csrc/ for sm_100a and link the shared library. Returns its path."""
+    """Compile every .cu under csrc/ for sm_90a and link the shared library. Returns its path."""
     os.makedirs(OBJDIR, exist_ok=True)
     if force:
         for f in os.listdir(OBJDIR):

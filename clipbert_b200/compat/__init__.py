@@ -1,5 +1,5 @@
 """Import-time stand-ins for the two third-party packages the reference task scripts import around the hot path and
-that a B200 installation does not need (SURVEY.md §8b): ``horovod.torch`` (-> torch.distributed / NCCL) and ``apex``
+that an H100 installation does not need (SURVEY.md §8b): ``horovod.torch`` (-> torch.distributed / NCCL) and ``apex``
 (``amp`` is a no-op here: parameters stay fp32 masters and the kernels consume their own bf16 copy; ``FusedLayerNorm``
 is only a parameter container on this path).
 
@@ -18,7 +18,7 @@ from . import amp, horovod_torch
 def alias_reference_modules():
     """Make the reference's own import lines resolve to this package (src/tasks/run_*.py:7-11, src/pretrain/run_pretrain.py:7-8):
     ``from src.modeling.e2e_model import ClipBert``, ``from src.modeling.modeling import ClipBertFor...`` and
-    ``from src.modeling.grid_feat import GridFeatBackbone`` then import the B200 modules - the scripts stay byte-identical.
+    ``from src.modeling.grid_feat import GridFeatBackbone`` then import the H100 modules - the scripts stay byte-identical.
     Call it before the script's imports run, with the reference root on ``sys.path`` (its ``src`` package must be importable)."""
     import clipbert_b200.e2e_model as e2e
     import clipbert_b200.grid_feat as gf

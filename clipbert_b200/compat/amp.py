@@ -1,5 +1,5 @@
 """``apex.amp`` as the reference uses it (src/tasks/run_video_retrieval.py:307-309,428-431,477-480; src/utils/load_save.py:
-initialize / scale_loss / master_params / state_dict / load_state_dict). On the B200 path mixed precision is internal to the
+initialize / scale_loss / master_params / state_dict / load_state_dict). On the H100 path mixed precision is internal to the
 kernels (fp32 master parameters, bf16 operand copies, fp32 accumulation, bf16 has fp32's exponent range: no loss scaling),
 so every call is the identity."""
 import contextlib

@@ -119,7 +119,7 @@ bool get_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t ro
 
 // The same [rows, cols] row-major bf16 matrix seen as 3-D {64 columns, rows, cols / 64 column blocks}: ONE box of
 // {64, box_rows, nblk} lands as nblk consecutive 128B-swizzled [box_rows x 64] slabs - exactly what nblk separate 2-D boxes of an
-// MN-major UMMA operand produce - so the producer issues one cp.async.bulk.tensor instead of nblk. cols must be a multiple of 64.
+// MN-major wgmma operand produce - so the producer issues one cp.async.bulk.tensor instead of nblk. cols must be a multiple of 64.
 bool get_tmap_3d_mn(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t ld, uint32_t box_rows, uint32_t nblk) {
   static std::mutex mu;
   static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
@@ -165,7 +165,7 @@ bool get_tmap_3d_mn(CUtensorMap* out, const void* base, uint64_t cols, uint64_t 
 extern "C" {
 const char* cb_last_error(void) { return cb::t_err; }
 int cb_version(void) { return 100; }
-int cb_sm_arch(void) { return 100; }
+int cb_sm_arch(void) { return 90; }
 int64_t cb_launch_count(void) { return cb::g_launches.load(std::memory_order_relaxed); }
 int cb_set_pdl(int enable) { return cb::g_pdl.exchange(enable == 2 ? 2 : (enable ? 1 : 0), std::memory_order_relaxed); }
 int cb_dropout_offset_bind(const uint64_t* device_word) {

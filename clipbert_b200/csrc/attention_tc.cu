@@ -5,9 +5,9 @@
 // layout is reused as the A operand of the next product). Same math, masks, dropout stream and lse convention as
 // csrc/attention.cu, which remains the path for L > 64 (448 px frames, 512-token inference).
 //
-// Why mma.sync and not tcgen05 here: a (sequence, head) problem is 41x41x64 - 0.9 % of the layer FLOPs; it is
-// latency-bound, and a tcgen05 pipeline (TMEM allocation, 128-row UMMA tiles, mbarrier hand-offs) costs more than
-// the whole product. All GEMM-shaped work of the path runs on tcgen05 (csrc/gemm.cu).
+// Why mma.sync and not wgmma here: a (sequence, head) problem is 41x41x64 - 0.9 % of the layer FLOPs; it is
+// latency-bound, and a wgmma pipeline (warpgroup-wide 64-row tiles, TMA staging, mbarrier hand-offs) costs more than
+// the whole product. All GEMM-shaped work of the path runs on wgmma (csrc/gemm.cu).
 #include "common.cuh"
 #include "host_util.h"
 
@@ -223,10 +223,7 @@ __global__ void __launch_bounds__(RT * 32) attn_tc_fwd_kernel(const __nv_bfloat1
 // recurrence (running row max m, running sum, accumulator rescaled by exp(m_old - m_new)). Mask, dropout stream
 // (index = ((b*H + h)*L + query)*L + key) and the saved log-sum-exp follow attn_fwd_kernel (attention.cu), so the general
 // backward kernels consume its output unchanged. At L = 521 the CUDA-core kernel spends 0.83 GFLOP per (sequence, layer)
-// on fp32 FMAs - more than the whole layer's tcgen05 GEMM time; this path puts those products on mma.sync.
-// (A variant with 32 query rows per warp - every K / V fragment feeding two row tiles, two warps per CTA - passed the same tests and
-// measured level with this kernel on config 5 (735 against 723-747 clips/s, profiles/r02_ab_runs.txt call 27): 255 registers leave
-// 8 warps per SM, which costs what the saved ldmatrix traffic gains. Not kept.)
+// on fp32 FMAs - more than the whole layer's GEMM time; this path puts those products on mma.sync.
 // PIPE = true (default): the K / V / mask tiles are double-buffered and the next key tile travels global -> shared with cp.async
 // (zero-filled beyond L) while the current one is multiplied; PIPE = false: the synchronous loads of the first version (A/B).
 __device__ __forceinline__ void cp_async16_zfill(__nv_bfloat16* dst, const __nv_bfloat16* src, int src_bytes) {

@@ -670,7 +670,7 @@ int cb_layernorm_bwd(const void* dy, const void* x, const float* stats, const fl
   CB_REQUIRE(hidden == HID, "cb_layernorm_bwd: hidden size %d unsupported", hidden);
   CB_REQUIRE(dy && x && stats && gamma && dx && m > 0, "cb_layernorm_bwd: bad arguments");
   // the dgamma / dbeta / dbias atomics contend once per block and column: a few rows per warp, not one
-  const int blocks = max(1, min(ceil_div(m, ROWS_PER_BLOCK), 148 * 2));
+  const int blocks = max(1, min(ceil_div(m, ROWS_PER_BLOCK), 132 * 2));   // two CTAs per H100 SM
   launch_k(ln_bwd_kernel, blocks, 128, 0, static_cast<cudaStream_t>(stream), 
       static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x), stats, gamma,
       static_cast<__nv_bfloat16*>(dx), static_cast<__nv_bfloat16*>(dx_drop), dgamma, dbeta, dbias_drop, m,

@@ -1,7 +1,7 @@
 // Memory-bound CNN-side kernels for the GridFeat ResNet-50 path (reference call sites:
 // src/modeling/grid_feat.py:89-105 -> detectron2 BasicStem / BottleneckBlock / MaxPool, and the
 // grid_encoder MaxPool2d+ReLU at grid_feat.py:43-48). Activations are NHWC bf16; every thread moves
-// 8 channels with one 128-bit access. All convolution FLOPs run in gemm.cu (tcgen05).
+// 8 channels with one 128-bit access. All convolution FLOPs run in gemm.cu (wgmma).
 #include "common.cuh"
 #include "host_util.h"
 

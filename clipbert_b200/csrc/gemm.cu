@@ -1,4 +1,4 @@
-// tcgen05 tensor-core contraction for every dense op on the ClipBERT path (see cb_gemm in
+// wgmma tensor-core contraction for every dense op on the ClipBERT path (see cb_gemm in
 // include/clipbert_b200.h). One persistent, warp-specialised kernel, three operand modes:
 //   MODE 0 (TN)    : A [rows, K] and B [N, K] both K-major; optional 9-tap row-shifted K loop
 //                    (3x3 conv over a zero-bordered NHWC activation); fused epilogue.
@@ -7,17 +7,16 @@
 //                    split over the pixel/token dimension, fp32 red.global accumulation.
 //
 // Structure (persistent CTAs, grid = min(#tiles, #SMs x CTAs per SM), static round-robin tile schedule):
-//   warp 0      TMA producer   : smem ring of STAGES x (A 128x64 | B BNx64) bf16 tiles, 128B swizzle
-//   warp 1      MMA issuer     : tcgen05.mma into one of TWO TMEM accumulator stages (2 x BN columns)
-//   warps 2..   epilogue       : TMEM -> registers -> fused epilogue, overlapping the next tile's TMA + MMA through the
-//                                tmem_full / tmem_empty barrier pair. Two I/O paths:
-//       EPI 1 (bf16 out): BN/16 WARP-PRIVATE pipelines. Warp (q, c) owns the 32-row x 64-column slab (TMEM lane quarter q,
-//             64-column chunk c) of every tile: its lane 0 TMA-loads the slab of the residual / aux tensor and the chunk's 64
-//             shift values into the warp's own shared-memory slab one main loop ahead, the warp converts its accumulator
-//             columns in four passes of 16, writes the result IN PLACE and lane 0 TMA-stores the slab. No barrier between
-//             warps, no loader warp: one tile costs a warp ~250 instructions (the chunk-cooperative version with named
-//             barriers cost ~1000 and was bound by their issue rate, profiles/r02e_gemm_cta_timeline_lean_epilogue.txt).
-//       EPI 0 (row re-map with stash / fp32 / wgrad red.add): per-warp smem staging -> coalesced 128-byte accesses, 8 warps.
+//   warp 8      TMA producer   : smem ring of STAGES x (A 128x64 | B BNx64) bf16 tiles, 128B swizzle
+//   warps 0..7  two consumer warpgroups: warpgroup g multiplies rows 64g .. 64g+63 of the tile with wgmma m64nBNk16 into
+//               registers, hands every smem stage back as soon as the products that read it have retired (one stage of
+//               wgmma stays in flight), then runs the epilogue of its rows while the producer already fills the ring
+//               with the next tile's operands.
+//   Epilogue (TN / NN): each warp owns 16 rows of the tile. Per 32-column slice it moves its accumulator fragment through a
+//               small per-warp fp32 staging tile so that every lane holds 16 consecutive columns of one row, applies the
+//               fused epilogue (bias / FrozenBN shift, residual, dropout, activation, stashes) and writes 16-byte vectors,
+//               re-mapping the output row (zero-bordered <-> compact pixel rows) where asked.
+//   Epilogue (WGRAD): red.global.add.v2.f32 straight from the fragment (four lanes cover 32 contiguous bytes of a row).
 #include "common.cuh"
 #include "host_util.h"
 
@@ -25,13 +24,16 @@ namespace cb {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-__host__ __device__ constexpr int gemm_threads(int ew) { return 64 + ew * 32; }   // TMA producer, MMA issuer, EW epilogue warps
-__host__ __device__ constexpr int epi_warps(int bn, int epi) { return epi == 1 ? bn / 16 : 8; }   // TMA epilogue: one warp per 32 x 64 output slab of a tile
+constexpr int CONSUMER_WARPS = 8;                          // two warpgroups of 64 tile rows each
+constexpr int GEMM_THREADS = (CONSUMER_WARPS + 1) * 32;    // + the TMA producer warp
+// (Nine warps put three on each SM sub-partition, which caps a thread at 168 registers: the 128 x 256 tiles of the TN / NN
+// epilogue spill at that budget, so the launch model only picks them for the weight gradients, whose epilogue is lean.)
 constexpr int MAX_STAGES = 8;
-constexpr int SLAB_BYTES = 32 * 128;            // one 32-row x 64-column bf16 slab (TMA epilogue: one warp's share of a tile)
 constexpr int SMEM_LIMIT = 232448;              // 227 KB opt-in limit per CTA
-constexpr int STG_ROW = 144;                    // staging row pitch in bytes (128 + 16: conflict-free 16 B accesses)
-constexpr int STG_BYTES = 32 * STG_ROW;         // per epilogue warp
+constexpr int SMEM_LIMIT_OCC2 = 113 * 1024;     // two CTAs per SM: (228 KB - 2 x 1 KB reserved) / 2
+constexpr int STG_PITCH = 36;                   // fp32 staging row pitch in floats (32 + 4: conflict-free 16-byte row reads)
+constexpr int STG_WARP_FLOATS = 16 * STG_PITCH; // one warp: 16 rows x 32 columns
+constexpr int EPI_BYTES = CONSUMER_WARPS * STG_WARP_FLOATS * 4;
 
 struct GemmEpi {
   const float* scale;
@@ -52,12 +54,9 @@ struct GemmEpi {
   float drop_inv_keep;
   uint64_t seed;
   const uint64_t* seed_off;   // device word folded into the seed at run time (cb_dropout_offset_bind), or nullptr
-  int shift_smem;   // TMA epilogue: the 64 shift values of every output chunk travel through shared memory (1-D bulk copy by the
-                    // loader warp, 256 B per residual-ring slot) instead of four __ldg per 16 columns: those loads sat on the
-                    // critical path of every chunk at full L2 latency (~700 cycles, profiles/r02e_gemm_cta_timeline_lean_epilogue.txt)
   int mn3d;         // MN-major operands (B of NN mode, A and B of WGRAD mode) arrive as ONE 3-D TMA box per k-chunk instead of
-                    // BN/64 (BM/64) 2-D boxes: tmA / tmB are then the {64, rows, cols/64} maps of get_tmap_3d_mn (CG = 1 only)
-  long long* dbg;   // optional in-kernel clock64 timeline, 16 slots per CTA (bring-up / tuning only; NULL in production)
+                    // BN/64 (BM/64) 2-D boxes: tmA / tmB are then the {64, rows, cols/64} maps of get_tmap_3d_mn
+  long long* dbg;   // optional in-kernel clock64 timeline, 32 slots per CTA (bring-up / tuning only; NULL in production)
 };
 
 // bring-up / tuning only: clock64 stamps of EVERY CTA (32 slots per CTA; slots 12 / 13 = %globaltimer at entry / exit so that
@@ -78,8 +77,7 @@ struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_BYTES = 512;
-  static constexpr int TMEM_COLS = 2 * BN;      // two accumulator stages
+  static constexpr int BAR_BYTES = 256;
 };
 
 // ---- epilogue arithmetic on NC consecutive columns [nb, nb+NC) of one output row ------------------------------------------------
@@ -288,27 +286,80 @@ __device__ __forceinline__ TileInfo decode_tile(int tile, int tiles_m, int tiles
   return t;
 }
 
-template <int BN, int MODE, int EPI, int OCC>
-__global__ void __launch_bounds__(gemm_threads(epi_warps(BN, EPI)), OCC)
-    gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
-                const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmC2, int M, int N, int K, int ntaps,
-                int tap_w, int tap_sign,
-                int iters_per_split, int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, int epi_bytes, GemmEpi epi) {
+// ---- consumer side of the operand ring ------------------------------------------------------------------------------------------
+// One tile's main loop of a consumer warpgroup: n_iters 64-deep k-chunks, KCH per ring stage. The wgmma of a stage are committed
+// as one group; once the NEXT stage's group is issued, the previous group is waited for and its stage handed back to the producer
+// (every consumer warp arrives on the stage's empty barrier). On return every product of the tile has landed in acc.
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], uint32_t smem0, int stage_bytes, int KCH, int STAGES, int n_iters, int wg,
+                                         int lane, int& s, uint32_t& ph, uint64_t* full_bar, uint64_t* empty_bar) {
   using Cfg = GemmCfg<BN>;
-  constexpr int EW = epi_warps(BN, EPI);
-  constexpr int EPI_WARPS = EW;
-  static_assert(OCC == 1 || (OCC == 2 && BN <= 128), "two CTAs per SM: 2 x BN <= 256 TMEM columns each");
+  int prev = -1;
+  for (int i = 0; i < n_iters; i += KCH) {
+    const int nch = min(KCH, n_iters - i);
+    mbar_wait(&full_bar[s], ph);
+    __syncwarp();
+    wgmma_fence();
+    wgmma_fence_acc(acc);
+    for (int ch = 0; ch < nch; ++ch) {
+      // this warpgroup's 64 A rows: K-major, 64 rows x 128 B further on; MN-major, the second 64-row box (8 KB) - the same offset
+      const uint32_t a_addr = smem0 + s * stage_bytes + ch * Cfg::STAGE_BYTES + wg * (64 * 128);
+      const uint32_t b_addr = smem0 + s * stage_bytes + ch * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t ad = TA ? gmma_desc(a_addr + k * 2048, BK * 128, 1024) : gmma_desc(a_addr + k * 32, 16, 1024);
+        const uint64_t bd = TB ? gmma_desc(b_addr + k * 2048, BK * 128, 1024) : gmma_desc(b_addr + k * 32, 16, 1024);
+        wgmma_bf16<BN, TA, TB>(acc, ad, bd, (i > 0 || ch > 0 || k > 0) ? 1u : 0u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_fence_acc(acc);
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    prev = s;
+    if (++s == STAGES) { s = 0; ph ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+  if (prev >= 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+  }
+}
+
+// ---- weight-gradient epilogue: out[tap * N + n] of rows m += acc * scale[m], straight from the wgmma fragment ----------------------
+// Fragment layout of m64nNk16 (f32): warp w of the warpgroup holds rows 16w + lane/4 (d[4j], d[4j+1]) and 16w + lane/4 + 8
+// (d[4j+2], d[4j+3]) at columns 8j + 2 (lane % 4) + {0, 1}.
+template <int BN>
+__device__ __forceinline__ void wgrad_epilogue(const float (&acc)[BN / 2], float* obase, int64_t out_ld, const float* scale, int M, int N, int r0,
+                                               int n0, int lane) {
+  const int r1 = r0 + 8;
+  const float rs0 = (r0 < M && scale) ? scale[r0] : 1.0f;
+  const float rs1 = (r1 < M && scale) ? scale[r1] : 1.0f;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = n0 + j * 8 + 2 * (lane & 3);
+    if (n < N) {     // N % 8 == 0: the pair n, n + 1 is inside
+      if (r0 < M) red_add_f32x2(obase + static_cast<int64_t>(r0) * out_ld + n, acc[4 * j] * rs0, acc[4 * j + 1] * rs0);
+      if (r1 < M) red_add_f32x2(obase + static_cast<int64_t>(r1) * out_ld + n, acc[4 * j + 2] * rs1, acc[4 * j + 3] * rs1);
+    }
+  }
+}
+
+template <int BN, int MODE, int OCC>
+__global__ void __launch_bounds__(GEMM_THREADS, OCC)
+    gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K, int ntaps, int tap_w,
+                int tap_sign, int iters_per_split, int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, int epi_bytes, GemmEpi epi) {
+  using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int stage_bytes = KCH * Cfg::STAGE_BYTES;           // a stage holds KCH consecutive 64-deep k-chunks (one barrier round trip)
-  uint8_t* stg_base = smem + STAGES * stage_bytes;          // epilogue region (1024-byte aligned: chunk sizes are multiples of 8 KB)
+  uint8_t* stg_base = smem + STAGES * stage_bytes;          // epilogue staging (TN / NN)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + epi_bytes);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* tfull_bar = empty_bar + MAX_STAGES;  // [2] accumulator stage ready for the epilogue
-  uint64_t* tempty_bar = tfull_bar + 2;          // [2] accumulator stage drained by the epilogue
-  uint64_t* win_bar = tempty_bar + 2;            // [16][2] per epilogue warp: inputs (residual / aux slab, shift values) of a tile landed (EPI 1)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(win_bar + 32);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -319,42 +370,23 @@ __global__ void __launch_bounds__(gemm_threads(epi_warps(BN, EPI)), OCC)
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (EPI == 1) {
-      if (epi.rowmap == CB_ROWMAP_NONE) tma_prefetch_desc(&tmC);
-      if (epi.out2) tma_prefetch_desc(&tmC2);
-      if (epi.residual) tma_prefetch_desc(&tmR);
-      if (epi.aux) tma_prefetch_desc(&tmX);
-    }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], CONSUMER_WARPS);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], EPI_WARPS);
-    }
-    for (int s = 0; s < 32; ++s) mbar_init(&win_bar[s], 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int kc_per_tap = (K + BK - 1) / BK;
-  // PDL: barrier init, TMEM allocation and descriptor prefetch above overlapped the previous kernel's tail; from here on
-  // this kernel touches global memory (TMA loads, epilogue loads/stores), so its producers must have completed.
+  // PDL: barrier init and descriptor prefetch above overlapped the previous kernel's tail; from here on this kernel touches
+  // global memory (TMA loads, epilogue loads/stores), so its producers must have completed.
   pdl_wait();
   if (threadIdx.x == 0) dbg_stamp(epi, 1);
 
-  if (warp == 0) {
+  if (warp >= CONSUMER_WARPS) {
     // ===================== TMA producer =====================
     // One elected lane owns the barriers and issues the TMA boxes of a stage (KCH chunks x {A boxes, B boxes}).
-    // (Issuing the boxes from several lanes of one instruction was measured 2x SLOWER: UTMALDG takes uniform
-    // operands, so divergent per-lane operands are serialised through a per-lane uniform-register loop.)
-    if (lane == 0) {
+    if (warp == CONSUMER_WARPS && lane == 0) {
       constexpr int A_BOXES = (MODE == 1) ? BM / 64 : 1;
       constexpr int B_BOXES = (MODE == 0) ? 1 : BN / 64;
       int s = 0;        // smem ring position / phase, carried across tiles
@@ -408,479 +440,168 @@ __global__ void __launch_bounds__(gemm_threads(epi_warps(BN, EPI)), OCC)
       }
       dbg_stamp(epi, 3);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN, MODE == 1, MODE != 0);
-      int s = 0;
-      uint32_t ph = 0;
-      int local = 0;
-      for (int tile = unit; tile < total_tiles; tile += n_units, ++local) {
-        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-        const int acc = local & 1;
-        const uint32_t acc_ph = (local >> 1) & 1;
-        mbar_wait(&tempty_bar[acc], acc_ph ^ 1);  // epilogue has drained this accumulator stage
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int i = 0; i < t.n_iters; i += KCH) {
-          const int nch = min(KCH, t.n_iters - i);
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          if (i == 0 && local == 0) dbg_stamp(epi, 4);
-          for (int ch = 0; ch < nch; ++ch) {
-            const uint32_t a_addr = smem_u32(smem + s * stage_bytes + ch * Cfg::STAGE_BYTES);
-            const uint32_t b_addr = a_addr + Cfg::A_BYTES;
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              uint64_t ad, bd;
-              if (MODE == 1) ad = umma_smem_desc(a_addr + k * 2048, BK * 128, 1024);
-              else ad = umma_smem_desc(a_addr + k * 32, 16, 1024);
-              if (MODE == 0) bd = umma_smem_desc(b_addr + k * 32, 16, 1024);
-              else bd = umma_smem_desc(b_addr + k * 2048, BK * 128, 1024);
-              const uint32_t accum = (i > 0 || ch > 0 || k > 0) ? 1u : 0u;
-              umma_bf16(d_tmem, ad, bd, idesc, accum);
-            }
-          }
-          umma_commit(&empty_bar[s]);           // frees this smem stage once the MMAs have read it
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);         // accumulator complete
-        if (local == 0) dbg_stamp(epi, 5);
-      }
-      dbg_stamp(epi, 6);
-    }
-  } else {
-    // ===================== epilogue warps =====================
-    auto release_acc = [&](uint64_t* bar) { mbar_arrive(bar); };   // hand the accumulator stage back to the MMA warp
-    const uint64_t dseed = epi.drop_thresh ? drop_seed(epi.seed, epi.seed_off) : 0ull;   // after pdl_wait: the word is device data
-    const int ew = warp - 2;          // 0 .. EW-1
-    const int q = warp & 3;           // TMEM lane quarter this warp may access (any four consecutive warps cover all four)
-    const int grp = ew >> 2;          // EPI 1: the 64-column chunk of the tile this warp owns; EPI 0: which half of the chunks
-    int local = 0;
-
-    if (EPI == 1) {
-      // ---------- TMA epilogue: bf16 output, warp-private pipelines ----------
-      // This warp owns rows q*32 .. q*32+31, columns grp*64 .. grp*64+63 of every tile. Shared memory of the warp:
-      //   S0  [32 x 128 B, 128B-swizzled]  residual slab in (TMA load), output slab out (written in place, TMA store)
-      //   S1  [32 x 128 B]                 aux slab in, or second output (pre-activation stash / gelu') out
-      //   SH  [2][64 floats]               shift values of the chunk, double-buffered
-      // Lane 0 requests the inputs of the warp's NEXT tile right after the store of the current one has read the slab, i.e.
-      // one main loop before they are needed. All shared-memory traffic uses explicit 32-bit shared addresses whose per-thread
-      // swizzled offsets are computed once.
-      constexpr int NC = 16;                            // columns per pass (one tcgen05.ld.x16)
-      constexpr int NPASS = 64 / NC;
-      const bool has_out2 = epi.out2 != nullptr;        // pre-activation stash: a second output slab
-      const bool has_res = epi.residual != nullptr, has_aux = epi.aux != nullptr;
-      const bool has_shift = epi.shift != nullptr, sh_smem = epi.shift_smem != 0;
-      const bool has_in = has_res || has_aux || sh_smem;
-      const bool second = (has_res && has_aux) || has_out2;     // aux alone lives in S0 (read, then overwritten in place by the output)
-      const bool remap = epi.rowmap != CB_ROWMAP_NONE;  // output rows are re-mapped: coalesced stores by the warp instead of TMA
-      const uint32_t s0 = smem_u32(stg_base) + ew * SLAB_BYTES;
-      const uint32_t s1 = second ? smem_u32(stg_base) + (EW + ew) * SLAB_BYTES : s0;
-      const uint32_t sh = smem_u32(stg_base) + EW * SLAB_BYTES * (second ? 2 : 1) + ew * 512;
-      uint64_t* my_bar = win_bar + ew * 2;              // [2]: inputs of this warp's even / odd tiles
-      const int swz = lane & 7;                         // 128B-swizzle XOR of this thread's slab row (row = lane)
-      const uint32_t rowb = lane * 128;                 // this thread's 128-byte slab row; its 16-byte unit u sits at rowb + ((u ^ swz) << 4)
-      // epilogue kind, fixed for the launch (see the EK_* functions)
-      const bool full = (N & 63) == 0 && epi.scale == nullptr;
-      const bool drop = epi.drop_thresh != 0;
-      int kind = EK_GENERIC;
-      if (full) {
-        if (!drop && !has_out2 && !has_aux && (epi.act == CB_ACT_NONE || epi.act == CB_ACT_RELU)) kind = EK_SHIFT_ACT;
-        else if (!drop && !has_out2 && !has_shift && has_aux && epi.aux_mode == CB_AUX_RELU_MASK && epi.act == CB_ACT_NONE) kind = EK_RELU_MASK;
-        else if (drop && !has_out2 && !has_aux && epi.act == CB_ACT_NONE) kind = EK_DROP_RES;
-        else if (!drop && has_out2 && !has_aux && !has_res && epi.act == CB_ACT_GELU_STASH_GRAD) kind = EK_GELU_STASH;
-        else if (!drop && !has_out2 && !has_shift && has_aux && epi.aux_mode == CB_AUX_MUL && epi.act == CB_ACT_NONE) kind = EK_AUX_MUL;
-      }
-      const bool kind_relu = epi.act == CB_ACT_RELU;
-      const bool guard = (N & 63) != 0;                 // ragged last chunk: per-float4 column checks in the generic epilogue
-
-      // lane 0: request the inputs of this warp's i-th tile (slab rows / columns outside the tensor are zero-filled by TMA)
-      auto request_inputs = [&](int i, int tile) {
-        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-        const int col = t.n0 + grp * 64, rw = t.m0 + q * 32;
-        const int ncols = min(64, N - col);                                // N % 8 == 0: a multiple of 8 floats = 32 bytes
-        const uint32_t sbytes = (sh_smem && ncols > 0) ? static_cast<uint32_t>(ncols) * 4u : 0u;
-        const uint32_t bytes = (has_res ? SLAB_BYTES : 0) + (has_aux ? SLAB_BYTES : 0) + sbytes;
-        uint64_t* bar = my_bar + (i & 1);
-        if (bytes) mbar_expect_tx(bar, bytes);
-        else mbar_arrive(bar);
-        if (has_res) tma_load_2d_s32(s0, &tmR, bar, col, rw);
-        if (has_aux) tma_load_2d_s32(s1, &tmX, bar, col, rw);     // s1 == s0 when there is no residual
-        if (sbytes) bulk_load_1d(sh + (i & 1) * 256, epi.shift + col, sbytes, bar);
-      };
-      if (has_in && lane == 0 && unit < total_tiles) request_inputs(0, unit);
-      for (int tile = unit; tile < total_tiles; tile += n_units, ++local) {
-        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-        const int acc = local & 1;
-        const uint32_t acc_ph = (local >> 1) & 1;
-        const int col0 = t.n0 + grp * 64;               // first column of this warp's slab
-        const int row0 = t.m0 + q * 32;                 // first row of this warp's slab
-        const int64_t orow = row0 + lane;
-        mbar_wait(&tfull_bar[acc], acc_ph);
-        tc_fence_after();
-        const bool stamp = epi.dbg != nullptr && ew == 0 && lane == 0 && local == 0;
-        if (stamp) dbg_stamp(epi, 7);
-        if (has_in) mbar_wait(my_bar + (local & 1), (local >> 1) & 1);
-        if (!has_res && !has_aux) {      // nothing was loaded into the slabs: the previous tile's store may still be reading them
-          if (lane == 0) tma_store_wait_read<0>();
-          __syncwarp();
-        }
-        const uint32_t trow = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16) + grp * 64;
-        const uint32_t shb = sh + (local & 1) * 256;
-        // 128 x 256 tiles (576 threads, 96 registers): not unrolled, the four passes share one copy of every epilogue kind in the
-        // i-cache. Narrower tiles have 8 / 4 epilogue warps and registers to spare: two passes in flight per warp give the
-        // schedulers the independent instructions that two warps per scheduler cannot (GELU / dropout passes are latency-bound).
-#pragma unroll(BN <= 128 ? 2 : 1)
-        for (int ps = 0; ps < NPASS; ++ps) {
-          const int nb = col0 + ps * NC;                // global column of f[0]
-          const uint32_t off0 = rowb + (((2 * ps) ^ swz) << 4), off1 = rowb + (((2 * ps + 1) ^ swz) << 4);
-          uint32_t v[NC];
-          __syncwarp();
-          tmem_ld16(trow + ps * NC, v);
-          tmem_ld_wait();
-          if (stamp && ps == 0) dbg_stamp(epi, 16);
-          if (ps == NPASS - 1) {                        // last TMEM read of this tile
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-          }
-          uint32_t res16[NC / 2], aux16[NC / 2];
-          if (has_res) {
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              const uint4 u = lds128(s0 + (j ? off1 : off0));
-              res16[4 * j] = u.x; res16[4 * j + 1] = u.y; res16[4 * j + 2] = u.z; res16[4 * j + 3] = u.w;
-            }
-          }
-          if (has_aux) {
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              const uint4 u = lds128(s1 + (j ? off1 : off0));
-              aux16[4 * j] = u.x; aux16[4 * j + 1] = u.y; aux16[4 * j + 2] = u.z; aux16[4 * j + 3] = u.w;
-            }
-          }
-          float shv[NC];                                // shift (bias / FrozenBN shift) of these columns
-          if (sh_smem) {
-#pragma unroll
-            for (int j = 0; j < NC / 4; ++j) {          // every lane reads the same 16 bytes: a shared-memory broadcast
-              const uint4 u = lds128(shb + ps * (NC * 4) + j * 16);
-              shv[4 * j] = __uint_as_float(u.x); shv[4 * j + 1] = __uint_as_float(u.y);
-              shv[4 * j + 2] = __uint_as_float(u.z); shv[4 * j + 3] = __uint_as_float(u.w);
-            }
-          } else if (has_shift) {
-#pragma unroll
-            for (int j = 0; j < NC; j += 4) {
-              float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (!guard || nb + j + 4 <= N) s4 = __ldg(reinterpret_cast<const float4*>(epi.shift + nb + j));
-              shv[j] = s4.x; shv[j + 1] = s4.y; shv[j + 2] = s4.z; shv[j + 3] = s4.w;
-            }
-          }
-          float f[NC];
-#pragma unroll
-          for (int j = 0; j < NC; ++j) f[j] = __uint_as_float(v[j]);
-          uint32_t o2_16[NC / 2];
-          switch (kind) {
-            case EK_SHIFT_ACT: epilogue_shift_act<NC>(f, shv, has_shift, res16, has_res, kind_relu); break;
-            case EK_RELU_MASK: epilogue_relu_mask<NC>(f, res16, has_res, aux16); break;
-            case EK_DROP_RES:
-              epilogue_drop_res<NC>(f, shv, has_shift, res16, has_res, dseed, static_cast<uint64_t>(orow) * static_cast<uint64_t>(N) + nb, epi.drop_thresh,
-                                    epi.drop_inv_keep);
-              break;
-            case EK_GELU_STASH: epilogue_gelu_stash<NC>(f, shv, has_shift, o2_16); break;
-            case EK_AUX_MUL: epilogue_aux_mul<NC>(f, res16, has_res, aux16); break;
-            default:
-              if (guard) epilogue_math<NC, true>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
-              else epilogue_math<NC, false>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
-          }
-          if (stamp && ps == 0) dbg_stamp(epi, 17);
-          if (has_out2) {
-#pragma unroll
-            for (int j = 0; j < 2; ++j)
-              sts128(s1 + (j ? off1 : off0), make_uint4(o2_16[4 * j], o2_16[4 * j + 1], o2_16[4 * j + 2], o2_16[4 * j + 3]));
-          }
-#pragma unroll
-          for (int j = 0; j < 2; ++j)
-            sts128(s0 + (j ? off1 : off0), make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                                                    pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7])));
-        }
-        if (stamp) dbg_stamp(epi, 18);
-        const bool in_range = row0 < M && col0 < N;     // (a slab entirely outside the tensor is not stored)
-        if (!remap) {
-          fence_proxy_async_smem();                     // generic-proxy smem writes -> visible to the TMA store
-          __syncwarp();
-          if (lane == 0) {
-            if (in_range) {
-              tma_store_2d_s32(&tmC, s0, col0, row0);
-              if (has_out2) tma_store_2d_s32(&tmC2, s1, col0, row0);
-            }
-            tma_store_commit();
-          }
-        } else {
-          // row-re-mapped output (zero-bordered <-> compact pixel rows): 8 lanes move one 128-byte row segment, 4 rows per pass
-          __syncwarp();
-          const int seg = lane & 7;
-          const int n = col0 + seg * 8;
-#pragma unroll
-          for (int pass = 0; pass < 8; ++pass) {
-            const int r = pass * 4 + (lane >> 3);
-            const int mm = row0 + r;
-            bool ok = mm < M && n + 8 <= N;
-            int64_t orr = mm;
-            if (epi.rowmap == CB_ROWMAP_PAD) {
-              const int hw = epi.H * epi.W;
-              const int img = mm / hw;
-              const int rr = mm - img * hw;
-              const int y = rr / epi.W, x = rr - y * epi.W;
-              orr = (static_cast<int64_t>(img) * (epi.H + 2) + y + 1) * (epi.W + 2) + x + 1;
-            } else {
-              const int wp = epi.W + 2, hp = epi.H + 2;
-              const int img = mm / (hp * wp);
-              const int rr = mm - img * (hp * wp);
-              const int y = rr / wp, x = rr - y * wp;
-              ok = ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
-              orr = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
-            }
-            if (ok)
-              *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(epi.out) + orr * epi.out_ld + n) = lds128(s0 + r * 128 + ((seg ^ (r & 7)) << 4));
-          }
-          __syncwarp();                                 // every lane has read the slab before it is handed to the next loads
-        }
-        if (stamp) dbg_stamp(epi, 14);
-        // inputs of this warp's next tile: the slabs are free once this tile's store has read them
-        if (has_in && lane == 0 && tile + n_units < total_tiles) {
-          if (!remap && (has_res || has_aux)) tma_store_wait_read<0>();
-          request_inputs(local + 1, tile + n_units);
-        }
-      }
-      if (ew == 0 && lane == 0) dbg_stamp(epi, 8);
-      if (lane == 0) tma_store_wait_all<0>();           // every warp drains its own bulk groups before the CTA may exit
-      if (ew == 0 && lane == 0) dbg_stamp(epi, 9);
-    } else {
-      // ---------- staged epilogue: row re-map, fp32 output, pre-activation stash, wgrad accumulation ----------
-      uint8_t* stg = stg_base + ew * STG_BYTES;
-      uint8_t* my_row = stg + lane * STG_ROW;       // this thread's own row in the staging tile
-      const int srow = lane >> 3;                   // coalesced phase: 4 rows per instruction, 8 lanes x 16 B per row
-      const int sseg = lane & 7;
-      for (int tile = unit; tile < total_tiles; tile += n_units, ++local) {
-        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-        const int acc = local & 1;
-        const uint32_t acc_ph = (local >> 1) & 1;
-        const int m = t.m0 + q * 32 + lane;
-        mbar_wait(&tfull_bar[acc], acc_ph);
-        tc_fence_after();
-        if (ew == 0 && lane == 0 && local == 0) dbg_stamp(epi, 7);
-        const uint32_t trow = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16);
-        bool released = false;
-
-        if (MODE == 1) {
-          const bool row_ok = m < M;
-          const float rs = (row_ok && epi.scale) ? epi.scale[m] : 1.0f;
-          float* obase = reinterpret_cast<float*>(epi.out) + static_cast<int64_t>(t.tap) * N;
-          constexpr int NCH = BN / 32;
-#pragma unroll 1
-          for (int cc = grp; cc < NCH; cc += 2) {
-            const int c = cc * 32;
-            uint32_t v[32];
-            __syncwarp();
-            tmem_ld32(trow + c, v);
-            tmem_ld_wait();
-            if (cc + 2 >= NCH) {  // last TMEM read of this warp for this tile
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) release_acc(&tempty_bar[acc]);
-              released = true;
-            }
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<float4*>(my_row + j * 4) = make_float4(__uint_as_float(v[j]) * rs, __uint_as_float(v[j + 1]) * rs,
-                                                                        __uint_as_float(v[j + 2]) * rs, __uint_as_float(v[j + 3]) * rs);
-            __syncwarp();
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int r = j * 4 + srow;
-              const int mm = t.m0 + q * 32 + r;
-              const int n = t.n0 + c + sseg * 4;
-              if (mm < M && n + 4 <= N)
-                red_add_f32x4(obase + static_cast<int64_t>(mm) * epi.out_ld + n, *reinterpret_cast<const float4*>(stg + r * STG_ROW + sseg * 16));
-            }
-          }
-        } else {
-          bool row_ok = m < M;
-          int64_t orow = m;
-          if (epi.rowmap == CB_ROWMAP_PAD) {
-            const int hw = epi.H * epi.W;
-            const int img = m / hw;
-            const int r = m - img * hw;
-            const int y = r / epi.W, x = r - y * epi.W;
-            orow = (static_cast<int64_t>(img) * (epi.H + 2) + y + 1) * (epi.W + 2) + x + 1;
-          } else if (epi.rowmap == CB_ROWMAP_UNPAD) {
-            const int wp = epi.W + 2, hp = epi.H + 2;
-            const int img = m / (hp * wp);
-            const int r = m - img * (hp * wp);
-            const int y = r / wp, x = r - y * wp;
-            row_ok = row_ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
-            orow = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
-          }
-          constexpr int NCH = BN / 64;
-#pragma unroll 1
-          for (int cc = grp; cc < NCH; cc += 2) {
-            const int c = cc * 64;
-            const int ncol = t.n0 + c;      // first column of this 64-wide chunk
-            uint32_t res[32], axv[32];      // packed bf16 pairs of this thread's row (64 columns)
-            // ---- coalesced loads of the residual / aux blocks (rows in A-row space) through the staging tile ----
-            if (epi.residual) {
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int r = j * 4 + srow;
-                const int mm = t.m0 + q * 32 + r;
-                const int n = ncol + sseg * 8;
-                uint4 u = make_uint4(0, 0, 0, 0);
-                if (mm < M && n + 8 <= N) u = *reinterpret_cast<const uint4*>(epi.residual + static_cast<int64_t>(mm) * epi.res_ld + n);
-                *reinterpret_cast<uint4*>(stg + r * STG_ROW + sseg * 16) = u;
-              }
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const uint4 u = *reinterpret_cast<const uint4*>(my_row + j * 16);
-                res[4 * j] = u.x; res[4 * j + 1] = u.y; res[4 * j + 2] = u.z; res[4 * j + 3] = u.w;
-              }
-            }
-            if (epi.aux) {
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int r = j * 4 + srow;
-                const int mm = t.m0 + q * 32 + r;
-                const int n = ncol + sseg * 8;
-                uint4 u = make_uint4(0, 0, 0, 0);
-                if (mm < M && n + 8 <= N) u = *reinterpret_cast<const uint4*>(epi.aux + static_cast<int64_t>(mm) * epi.aux_ld + n);
-                *reinterpret_cast<uint4*>(stg + r * STG_ROW + sseg * 16) = u;
-              }
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const uint4 u = *reinterpret_cast<const uint4*>(my_row + j * 16);
-                axv[4 * j] = u.x; axv[4 * j + 1] = u.y; axv[4 * j + 2] = u.z; axv[4 * j + 3] = u.w;
-              }
-            }
-            uint32_t o2[32];                // packed pre-activation (out2), only when requested
-            uint32_t ob[32];                // packed bf16 output (bf16 path)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              uint32_t v[32];
-              __syncwarp();
-              tmem_ld32(trow + c + h * 32, v);
-              tmem_ld_wait();
-              if (cc + 2 >= NCH && h == 1) {  // last TMEM read of this warp for this tile
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) release_acc(&tempty_bar[acc]);
-                released = true;
-              }
-              float f[32];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-              const int nb = ncol + h * 32;
-              float shv[32];
-              const bool has_shift = epi.shift != nullptr;
-              if (has_shift) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                  float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                  if (nb + j + 4 <= N) s4 = __ldg(reinterpret_cast<const float4*>(epi.shift + nb + j));
-                  shv[j] = s4.x; shv[j + 1] = s4.y; shv[j + 2] = s4.z; shv[j + 3] = s4.w;
-                }
-              }
-              epilogue_math<32, true>(f, epi, shv, has_shift, dseed, nb, N, orow, reinterpret_cast<const uint32_t(&)[16]>(res[h * 16]), epi.residual != nullptr,
-                                      reinterpret_cast<const uint32_t(&)[16]>(axv[h * 16]), epi.aux != nullptr, reinterpret_cast<uint32_t(&)[16]>(o2[h * 16]),
-                                      epi.out2 != nullptr);
-              if (epi.out_fp32) {
-                // fp32 output: stage 32 columns (128 B per row) and store coalesced right away
-                __syncwarp();
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(my_row + j * 4) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-                __syncwarp();
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const int r = j * 4 + srow;
-                  const int64_t orr = __shfl_sync(0xffffffffu, orow, r);
-                  const int okr = __shfl_sync(0xffffffffu, static_cast<int>(row_ok), r);
-                  const int n = nb + sseg * 4;
-                  if (okr && n + 4 <= N)
-                    *reinterpret_cast<float4*>(reinterpret_cast<float*>(epi.out) + orr * epi.out_ld + n) =
-                        *reinterpret_cast<const float4*>(stg + r * STG_ROW + sseg * 16);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) ob[h * 16 + j] = pack_bf16x2(f[2 * j], f[2 * j + 1]);
-              }
-            }
-            // ---- coalesced bf16 stores: own row -> staging tile -> 4 rows x 128 B per warp instruction ----
-            if (epi.out2) {
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) *reinterpret_cast<uint4*>(my_row + j * 16) = make_uint4(o2[4 * j], o2[4 * j + 1], o2[4 * j + 2], o2[4 * j + 3]);
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int r = j * 4 + srow;
-                const int64_t orr = __shfl_sync(0xffffffffu, orow, r);
-                const int okr = __shfl_sync(0xffffffffu, static_cast<int>(row_ok), r);
-                const int n = ncol + sseg * 8;
-                if (okr && n + 8 <= N)
-                  *reinterpret_cast<uint4*>(epi.out2 + orr * epi.out2_ld + n) = *reinterpret_cast<const uint4*>(stg + r * STG_ROW + sseg * 16);
-              }
-            }
-            if (!epi.out_fp32) {
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) *reinterpret_cast<uint4*>(my_row + j * 16) = make_uint4(ob[4 * j], ob[4 * j + 1], ob[4 * j + 2], ob[4 * j + 3]);
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int r = j * 4 + srow;
-                const int64_t orr = __shfl_sync(0xffffffffu, orow, r);
-                const int okr = __shfl_sync(0xffffffffu, static_cast<int>(row_ok), r);
-                const int n = ncol + sseg * 8;
-                if (okr && n + 8 <= N)
-                  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(epi.out) + orr * epi.out_ld + n) =
-                      *reinterpret_cast<const uint4*>(stg + r * STG_ROW + sseg * 16);
-              }
-            }
-          }
-        }
-        if (!released) {   // this warp had no column chunk in this tile (narrow BN): still hand the stage back, in order
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) release_acc(&tempty_bar[acc]);
-        }
-      }
-      if (ew == 0 && lane == 0) dbg_stamp(epi, 8);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) dbg_stamp(epi, 10);
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+
+  // ===================== consumer warpgroups: wgmma main loop + epilogue =====================
+  const int wg = warp >> 2;                 // rows wg * 64 .. wg * 64 + 63 of the tile
+  const int wrow = wg * 64 + (warp & 3) * 16;   // first of this warp's 16 rows
+  const uint32_t smem0 = smem_u32(smem);
+  const uint64_t dseed = epi.drop_thresh ? drop_seed(epi.seed, epi.seed_off) : 0ull;   // after pdl_wait: the word is device data
+  float acc[BN / 2];
+  int s = 0;
+  uint32_t ph = 0;
+  int local = 0;
+
+  // TN / NN epilogue: lane (er, eh) handles row er of the warp's 16, columns eh * 16 .. eh * 16 + 15 of each 32-column slice
+  const int er = lane & 15, eh = lane >> 4;
+  float* stg = reinterpret_cast<float*>(stg_base) + warp * STG_WARP_FLOATS;
+  const bool has_out2 = epi.out2 != nullptr;
+  const bool has_res = epi.residual != nullptr, has_aux = epi.aux != nullptr;
+  const bool has_shift = epi.shift != nullptr;
+  // epilogue kind, fixed for the launch (see the EK_* functions)
+  const bool full = (N & 15) == 0 && epi.scale == nullptr;
+  const bool drop = epi.drop_thresh != 0;
+  int kind = EK_GENERIC;
+  if (full) {
+    if (!drop && !has_out2 && !has_aux && (epi.act == CB_ACT_NONE || epi.act == CB_ACT_RELU)) kind = EK_SHIFT_ACT;
+    else if (!drop && !has_out2 && !has_shift && has_aux && epi.aux_mode == CB_AUX_RELU_MASK && epi.act == CB_ACT_NONE) kind = EK_RELU_MASK;
+    else if (drop && !has_out2 && !has_aux && epi.act == CB_ACT_NONE) kind = EK_DROP_RES;
+    else if (!drop && has_out2 && !has_aux && !has_res && epi.act == CB_ACT_GELU_STASH_GRAD) kind = EK_GELU_STASH;
+    else if (!drop && !has_out2 && !has_shift && has_aux && epi.aux_mode == CB_AUX_MUL && epi.act == CB_ACT_NONE) kind = EK_AUX_MUL;
   }
-  if (threadIdx.x == 32) dbg_stamp(epi, 11);
+  const bool kind_relu = epi.act == CB_ACT_RELU;
+  const bool guard = (N & 15) != 0;                 // ragged last 16 columns: per-vector column checks in the generic epilogue
+
+  for (int tile = unit; tile < total_tiles; tile += n_units, ++local) {
+    const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
+    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 4);
+    mma_tile<BN, MODE == 1, MODE != 0>(acc, smem0, stage_bytes, KCH, STAGES, t.n_iters, wg, lane, s, ph, full_bar, empty_bar);
+    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 5);
+
+    if (MODE == 1) {
+      wgrad_epilogue<BN>(acc, reinterpret_cast<float*>(epi.out) + static_cast<int64_t>(t.tap) * N, epi.out_ld, epi.scale, M, N,
+                         t.m0 + wrow + (lane >> 2), t.n0, lane);
+      continue;
+    }
+
+    // ---- this lane's row: A-row space m (residual / aux), output row orow (re-mapped), row_ok ----
+    const int m = t.m0 + wrow + er;
+    bool row_ok = m < M;
+    int64_t orow = m;
+    if (epi.rowmap == CB_ROWMAP_PAD) {
+      const int hw = epi.H * epi.W;
+      const int img = m / hw;
+      const int r = m - img * hw;
+      const int y = r / epi.W, x = r - y * epi.W;
+      orow = (static_cast<int64_t>(img) * (epi.H + 2) + y + 1) * (epi.W + 2) + x + 1;
+    } else if (epi.rowmap == CB_ROWMAP_UNPAD) {
+      const int wp = epi.W + 2, hp = epi.H + 2;
+      const int img = m / (hp * wp);
+      const int r = m - img * (hp * wp);
+      const int y = r / wp, x = r - y * wp;
+      row_ok = row_ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
+      orow = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
+    }
+#pragma unroll
+    for (int sc = 0; sc < BN / 32; ++sc) {
+      // fragment -> staging: this warp's 16 rows x 32 columns, then one row segment per lane
+      __syncwarp();
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = sc * 4 + jj;
+        float* p = stg + (lane >> 2) * STG_PITCH + jj * 8 + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(p + 8 * STG_PITCH) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      __syncwarp();
+      const int nb = t.n0 + sc * 32 + eh * 16;        // global column of f[0]
+      if (!row_ok || nb >= N) continue;
+      constexpr int NC = 16;
+      float f[NC];
+      const uint32_t srow = smem_u32(stg + er * STG_PITCH + eh * 16);
+#pragma unroll
+      for (int j = 0; j < NC / 4; ++j) {
+        const uint4 u = lds128(srow + j * 16);
+        f[4 * j] = __uint_as_float(u.x); f[4 * j + 1] = __uint_as_float(u.y);
+        f[4 * j + 2] = __uint_as_float(u.z); f[4 * j + 3] = __uint_as_float(u.w);
+      }
+      uint32_t res16[NC / 2], aux16[NC / 2];
+      if (has_res) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          uint4 u = make_uint4(0, 0, 0, 0);
+          if (nb + 8 * j + 8 <= N) u = __ldg(reinterpret_cast<const uint4*>(epi.residual + static_cast<int64_t>(m) * epi.res_ld + nb + 8 * j));
+          res16[4 * j] = u.x; res16[4 * j + 1] = u.y; res16[4 * j + 2] = u.z; res16[4 * j + 3] = u.w;
+        }
+      }
+      if (has_aux) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          uint4 u = make_uint4(0, 0, 0, 0);
+          if (nb + 8 * j + 8 <= N) u = __ldg(reinterpret_cast<const uint4*>(epi.aux + static_cast<int64_t>(m) * epi.aux_ld + nb + 8 * j));
+          aux16[4 * j] = u.x; aux16[4 * j + 1] = u.y; aux16[4 * j + 2] = u.z; aux16[4 * j + 3] = u.w;
+        }
+      }
+      float shv[NC];                                  // shift (bias / FrozenBN shift) of these columns
+      if (has_shift) {
+#pragma unroll
+        for (int j = 0; j < NC; j += 4) {
+          float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (nb + j + 4 <= N) s4 = __ldg(reinterpret_cast<const float4*>(epi.shift + nb + j));
+          shv[j] = s4.x; shv[j + 1] = s4.y; shv[j + 2] = s4.z; shv[j + 3] = s4.w;
+        }
+      }
+      uint32_t o2_16[NC / 2];
+      switch (kind) {
+        case EK_SHIFT_ACT: epilogue_shift_act<NC>(f, shv, has_shift, res16, has_res, kind_relu); break;
+        case EK_RELU_MASK: epilogue_relu_mask<NC>(f, res16, has_res, aux16); break;
+        case EK_DROP_RES:
+          epilogue_drop_res<NC>(f, shv, has_shift, res16, has_res, dseed, static_cast<uint64_t>(orow) * static_cast<uint64_t>(N) + nb, epi.drop_thresh,
+                                epi.drop_inv_keep);
+          break;
+        case EK_GELU_STASH: epilogue_gelu_stash<NC>(f, shv, has_shift, o2_16); break;
+        case EK_AUX_MUL: epilogue_aux_mul<NC>(f, res16, has_res, aux16); break;
+        default:
+          if (guard) epilogue_math<NC, true>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
+          else epilogue_math<NC, false>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
+      }
+      if (epi.out_fp32) {
+        float* o = reinterpret_cast<float*>(epi.out) + orow * epi.out_ld + nb;
+#pragma unroll
+        for (int j = 0; j < NC; j += 4)
+          if (nb + j + 4 <= N) *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+      } else {
+        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(epi.out) + orow * epi.out_ld + nb;
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          if (nb + 8 * j + 8 <= N)
+            *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
+                                                              pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
+      }
+      if (has_out2) {
+        __nv_bfloat16* o = epi.out2 + orow * epi.out2_ld + nb;
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          if (nb + 8 * j + 8 <= N) *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(o2_16[4 * j], o2_16[4 * j + 1], o2_16[4 * j + 2], o2_16[4 * j + 3]);
+      }
+    }
+    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 8);
+  }
+  if (threadIdx.x == 0) dbg_stamp(epi, 11);
 }
 
 static int g_sm_limit = 0;    // tuning hook: cap on the persistent grid (0 = every SM). A long-running co-resident kernel (an NCCL
                               // all-reduce overlapped with the backward pass) pins some SMs for its whole duration; with the static
-                              // round-robin tile schedule the CTAs that cannot be placed run as a second wave, so a launch of 148
-                              // CTAs takes up to twice as long. Capping the grid at 148 - (NCCL CTAs) avoids the second wave.
+                              // round-robin tile schedule the CTAs that cannot be placed run as a second wave. Capping the grid at
+                              // the SM count minus the co-resident kernel's CTAs avoids the second wave.
 static int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return (g_sm_limit > 0 && g_sm_limit < n) ? g_sm_limit : n;
 }
@@ -889,26 +610,17 @@ static long long* g_gemm_timeline = nullptr;
 static int g_force_kch = 0;   // tuning hook: chunks per stage (0 = automatic)
 static int g_mn3d = 1;        // 1 (default) = MN-major operands through one 3-D TMA box per k-chunk (GemmEpi::mn3d); cb_debug_gemm_mn3d
 
-// Shared-memory plan of one launch: epilogue region first (TMA epilogue: one 4 KB slab per epilogue warp, a second one when the
-// launch has an aux input or a second output, 2 x 256 B of shift values per warp), then as many 64-deep operand chunks as fit,
-// grouped KCH per stage. Measured (profiles/r01_gemm_kch_probe.txt, r01_gemm_staged_probe.txt): every stage costs a ~450-cycle
-// barrier round trip whatever its size, so deep stages beat many stages (1312x768x3072: 26.5 / 18.3 / 15.8 us with 1 / 2 / 4
-// chunks per stage).
+// Shared-memory plan of one launch: the epilogue staging (TN / NN: 16 x 32 fp32 per consumer warp; WGRAD: none), then as many
+// 64-deep operand chunks as fit, grouped KCH per stage. Every stage costs one full / empty barrier round trip whatever its size,
+// so deep stages are preferred to many shallow ones.
 struct SmemPlan {
   int epi_bytes, kch, stages, chunk_bytes;
 };
-constexpr int SMEM_LIMIT_OCC2 = 113 * 1024;   // two CTAs per SM: (228 KB - 2 x 1 KB reserved) / 2
-static SmemPlan plan_smem(int bn, bool tma_epi, bool second, bool sh_smem, int kiters, int force_kch = 0, int occ = 1) {
+static SmemPlan plan_smem(int bn, bool staging, int kiters, int force_kch = 0, int occ = 1) {
   SmemPlan p;
   const int limit = occ == 2 ? SMEM_LIMIT_OCC2 : SMEM_LIMIT;
   p.chunk_bytes = BM * BK * 2 + bn * BK * 2;
-  if (tma_epi) {
-    const int ew = epi_warps(bn, 1);
-    p.epi_bytes = ew * SLAB_BYTES * (second ? 2 : 1) + (sh_smem ? ew * 512 : 0);
-    p.epi_bytes = (p.epi_bytes + 1023) & ~1023;
-  } else {
-    p.epi_bytes = (8 * STG_BYTES + 1023) & ~1023;     // staged epilogue: always 8 warps
-  }
+  p.epi_bytes = staging ? EPI_BYTES : 0;
   const int chunks_fit = (limit - 1024 - GemmCfg<64>::BAR_BYTES - p.epi_bytes) / p.chunk_bytes;
   p.kch = 1;
   if (force_kch > 0) p.kch = force_kch;
@@ -924,14 +636,13 @@ static SmemPlan plan_smem(int bn, bool tma_epi, bool second, bool sh_smem, int k
   return p;
 }
 
-template <int BN, int MODE, int EPI, int OCC = 1>
+template <int BN, int MODE, int OCC = 1>
 static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_t stream) {
   GemmEpi epi = epi_in;
   using Cfg = GemmCfg<BN>;
-  constexpr int GEMM_THREADS = gemm_threads(epi_warps(BN, EPI));
   constexpr int LIMIT = OCC == 2 ? SMEM_LIMIT_OCC2 : SMEM_LIMIT;
   static bool attr_set = false;
-  auto kern = gemm_kernel<BN, MODE, EPI, OCC>;
+  auto kern = gemm_kernel<BN, MODE, OCC>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LIMIT);
     if (e == cudaSuccess && OCC == 2)   // both CTAs of an SM need their 113 KB: ask for the full shared-memory carve-out
@@ -943,7 +654,7 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
     attr_set = true;
   }
   // Tensor maps are copied out of the cache into this frame (and from here into the kernel's parameter space)
-  alignas(64) CUtensorMap ta, tb, tc, tr, tx, tc2;
+  alignas(64) CUtensorMap ta, tb;
   bool mn3d = false;
   int iters_per_split = 0;
   const int tiles_m = ceil_div(d.m, BM), tiles_n = ceil_div(d.n, BN);
@@ -974,18 +685,8 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
     kiters = iters_per_split;
   }
   if (!ok) return CB_ERR_CUDA;
-  tc = tr = tx = tc2 = ta;   // placeholders for the maps this launch does not use (a __grid_constant__ parameter must be a valid object)
-  if (EPI == 1) {
-    // epilogue maps: one box = the 32-row x 64-column slab one epilogue warp loads / stores
-    if (d.rowmap == CB_ROWMAP_NONE && !get_tmap_2d(&tc, d.out, d.n, d.m, d.out_ld, 64, 32)) return CB_ERR_CUDA;
-    if (d.residual && !get_tmap_2d(&tr, d.residual, d.n, d.m, d.res_ld, 64, 32)) return CB_ERR_CUDA;
-    if (d.aux && !get_tmap_2d(&tx, d.aux, d.n, d.m, d.aux_ld, 64, 32)) return CB_ERR_CUDA;
-    if (d.out2 && !get_tmap_2d(&tc2, d.out2, d.n, d.m, d.out2_ld, 64, 32)) return CB_ERR_CUDA;
-  }
   epi.mn3d = mn3d ? 1 : 0;
-  const bool sh_smem = EPI == 1 && d.shift != nullptr && (reinterpret_cast<uintptr_t>(d.shift) & 15) == 0;
-  epi.shift_smem = sh_smem ? 1 : 0;
-  const SmemPlan sp = plan_smem(BN, EPI == 1, (d.residual && d.aux) || d.out2, sh_smem, kiters, (d.reserved >> 8) & 15, OCC);
+  const SmemPlan sp = plan_smem(BN, MODE != 1, kiters, (d.reserved >> 8) & 15, OCC);
   const int epi_bytes = sp.epi_bytes, kch = sp.kch, stages = sp.stages;
   if (stages < 2) {
     set_error("cb_gemm: not enough shared memory for a 2-stage pipeline (BN=%d, epilogue %d B, %d CTA(s) per SM)", BN, epi_bytes, OCC);
@@ -994,35 +695,27 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
   const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + epi_bytes + Cfg::BAR_BYTES + 1024;
   const int units = sm_count() * OCC;
   const int grid = total < units ? total : units;
-  launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, tc, tr, tx, tc2, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign,
-           iters_per_split, tiles_m, tiles_n, total, stages, kch, epi_bytes, epi);
+  launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, iters_per_split, tiles_m,
+                tiles_n, total, stages, kch, epi_bytes, epi);
   return check_launch("cb_gemm");
 }
 
 // ------------------------------------------------------------------------------------------------
-// Launch configuration. Measured on B200 (tools/probe_gemm_cta_timeline.py, profiles/r02c_gemm_cta_timeline.txt): a
-// persistent CTA sustains ~60-70 B/clk of TMA ingest, so its main loop costs about (k-iterations x stage bytes)
-// / 60 cycles and the launch is done when the busiest SM is. The model picks the tile width (and the wgrad
-// K-split) minimising that plus a per-tile epilogue term. 128 x 256 tiles reach 1.27 PFLOP/s on 8192^2 x 2048
-// (87 % of the measured sustained cuBLAS figure).
-// (A cta_group::2 CTA-pair variant existed in round 1; it measured 15-60 % SLOWER than single CTAs on every shape of
-// the step, compute-bound 3x3 convs included - profiles/r02c_gemm_cta_timeline.txt, "pair" rows - and was removed.)
+// Launch configuration: an analytic model picks the tile width (and the wgrad K-split). A persistent CTA's main loop costs about
+// (k-iterations x stage bytes) / (operand ingest rate) plus a barrier round trip per stage, and the launch is done when the
+// busiest SM is; a per-tile epilogue term is added.
 // ------------------------------------------------------------------------------------------------
 struct LaunchCfg {
   int bn, splits;
 };
 
-// Two CTAs per SM (the OCC = 2 instantiations: 128 x <=128 tiles, 8 epilogue warps, <= 113 KB of shared memory, 2 x BN <= 256
-// TMEM columns each). One CTA's prologue / epilogue / barrier round trips run under the other's main loop, and an HBM-bound
-// 1x1 conv keeps two operand + residual rings in flight per SM. The price is operand traffic: a 128 x 128 tile needs 128 B/clk
-// of L2 -> SM ingest for a full-rate tensor pipe against ~70 B/clk measured, so everything compute-bound stays on 128 x 256
-// tiles with one CTA per SM (measured, profiles/r02_ab_runs.txt: turning it on for all BERT GEMMs costs 4 % of the step).
-//   g_occ2_mode: 0 = never, 1 = only launches that ask for it (cb_gemm_desc.reserved bit 5: the tuning table), 2 = every
-//   eligible launch whose work is at most g_occ2_max_gflop (0 = no limit).
+// Two CTAs per SM (the OCC = 2 instantiations: 128 x 64 tiles, <= 113 KB of shared memory and <= 96 registers per thread
+// each). One CTA's epilogue runs under the other's main loop. g_occ2_mode: 0 = never, 1 = only launches that ask for it
+// (cb_gemm_desc.reserved bit 5), 2 = every eligible launch whose work is at most g_occ2_max_gflop (0 = no limit).
 static int g_occ2_mode = 1;
 static double g_occ2_max_gflop = 0.0;
 
-static LaunchCfg choose_config(const cb_gemm_desc& d, bool tma_epi, int occ = 1) {
+static LaunchCfg choose_config(const cb_gemm_desc& d, int occ = 1) {
   const int units = sm_count() * occ;
   const int kc = ceil_div(d.k, BK);
   const bool wgrad = d.mode == CB_GEMM_WGRAD;
@@ -1031,8 +724,9 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, bool tma_epi, int occ = 1)
   double best_cost = 1e30;
   for (int c = 0; c < 3; ++c) {
     const int bn = cand[c];
-    if (occ == 2 && bn > 128) continue;
+    if (occ == 2 && bn > 64) continue;
     if (d.block_n && bn != d.block_n) continue;
+    if (!d.block_n && !wgrad && bn == 256) continue;      // see GEMM_THREADS
     if (bn > 64 && d.n <= bn / 2) continue;               // mostly padding
     const int64_t base = static_cast<int64_t>(ceil_div(d.m, BM)) * ceil_div(d.n, bn) * (wgrad ? d.ntaps : 1);
     const int max_split = wgrad ? (d.split_k > 0 ? d.split_k : (kc < 32 ? kc : 32)) : 1;
@@ -1041,15 +735,13 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, bool tma_epi, int occ = 1)
       const int real_sp = wgrad ? ceil_div(kc, ips) : 1;
       const int64_t tiles = base * real_sp;
       const double rounds = static_cast<double>((tiles + units - 1) / units);
-      const SmemPlan pl = plan_smem(bn, tma_epi && !wgrad, (d.residual && d.aux) || d.out2,
-                                    tma_epi && !wgrad && d.shift != nullptr && (reinterpret_cast<uintptr_t>(d.shift) & 15) == 0, ips, (d.reserved >> 8) & 15, occ);
+      const SmemPlan pl = plan_smem(bn, !wgrad, ips, (d.reserved >> 8) & 15, occ);
       if (pl.stages < 2) continue;
-      // a ring of 2 chunks cannot cover the TMA round trip of a long K loop (measured: 128 x 256 tiles on a 2-chunk
-      // ring run their main loop 4x slower, profiles/r02g_gemm_cta_timeline_warp_private.txt, ffn1_fwd bn256)
+      // a ring of 2 chunks cannot cover the TMA round trip of a long K loop
       const double shallow = (pl.stages * pl.kch < 3 && ips > 2) ? 3.0 : 1.0;
-      // per stage: ~450-cycle barrier round trip + bytes at ~60 B/clk (shared by the CTAs of an SM); per tile: epilogue (fp32 red.add / staged bf16 / TMA bf16)
+      // per stage: ~450-cycle barrier round trip + bytes at ~60 B/clk (shared by the CTAs of an SM); per tile: epilogue
       const double stage_cost = 450.0 + pl.kch * pl.chunk_bytes / (60.0 / occ);
-      const double epi = wgrad ? bn * 24.0 : (tma_epi ? 2000.0 : bn * 30.0);   // TMA epilogue: every warp converts ONE 32 x 64 slab per tile
+      const double epi = wgrad ? bn * 24.0 : bn * 30.0;
       const double cost = rounds * (ceil_div(ips, pl.kch) * stage_cost * shallow + epi) + 2500.0;
       if (cost < best_cost) {
         best_cost = cost;
@@ -1066,10 +758,9 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, bool tma_epi, int occ = 1)
 // Linear layers of a BertLayer, the three / four convs of a bottleneck block). The problems of a group share the reduction
 // length (tokens / pixels), so their tiles cost the same and the static round-robin schedule stays balanced; what the group buys
 // is one prologue + one tail instead of four, tiles of all problems filling the SMs together, and - because four problems
-// together have enough tiles - no K-split, i.e. half the fp32 red.global traffic of the single launches
-// (profiles/r02i_gemm_autotune_report.txt: 56 us per BertLayer as four launches). Same warp roles, ring, TMEM double buffer
-// and staged red.add epilogue as gemm_kernel<BN, MODE 1, EPI 0>; the problem descriptors (tensor maps included) travel in the
-// kernel's parameter space.
+// together have enough tiles - no K-split, i.e. half the fp32 red.global traffic of the single launches. Same warp roles, ring
+// and red.add epilogue as gemm_kernel<BN, MODE 1>; the problem descriptors (tensor maps included) travel in the kernel's
+// parameter space.
 // ------------------------------------------------------------------------------------------------
 constexpr int WG_MAX_PROBLEMS = 8;
 struct WgradProblem {
@@ -1112,19 +803,14 @@ __device__ __forceinline__ WgTile wg_decode(const WgradGroup& g, int tile) {
 }
 
 template <int BN>
-__global__ void __launch_bounds__(gemm_threads(8), 1)
-    wgrad_group_kernel(const __grid_constant__ WgradGroup g, int STAGES, int KCH, int epi_bytes) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+    wgrad_group_kernel(const __grid_constant__ WgradGroup g, int STAGES, int KCH) {
   using Cfg = GemmCfg<BN>;
-  constexpr int EPI_WARPS = 8;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int stage_bytes = KCH * Cfg::STAGE_BYTES;
-  uint8_t* stg_base = smem + STAGES * stage_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + epi_bytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* tfull_bar = empty_bar + MAX_STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int unit = blockIdx.x, n_units = gridDim.x;
   pdl_trigger();
@@ -1135,24 +821,16 @@ __global__ void __launch_bounds__(gemm_threads(8), 1)
     }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], EPI_WARPS);
+      mbar_init(&empty_bar[s], CONSUMER_WARPS);
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp >= CONSUMER_WARPS) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (warp == CONSUMER_WARPS && lane == 0) {
       int s = 0;
       uint32_t ph = 0;
       for (int tile = unit; tile < g.total_tiles; tile += n_units) {
@@ -1184,102 +862,21 @@ __global__ void __launch_bounds__(gemm_threads(8), 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN, 1, 1);
-      int s = 0;
-      uint32_t ph = 0;
-      int local = 0;
-      for (int tile = unit; tile < g.total_tiles; tile += n_units, ++local) {
-        const WgTile t = wg_decode(g, tile);
-        const int acc = local & 1;
-        const uint32_t acc_ph = (local >> 1) & 1;
-        mbar_wait(&tempty_bar[acc], acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int i = 0; i < t.n_iters; i += KCH) {
-          const int nch = min(KCH, t.n_iters - i);
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          for (int ch = 0; ch < nch; ++ch) {
-            const uint32_t a_addr = smem_u32(smem + s * stage_bytes + ch * Cfg::STAGE_BYTES);
-            const uint32_t b_addr = a_addr + Cfg::A_BYTES;
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              const uint64_t ad = umma_smem_desc(a_addr + k * 2048, BK * 128, 1024);
-              const uint64_t bd = umma_smem_desc(b_addr + k * 2048, BK * 128, 1024);
-              umma_bf16(d_tmem, ad, bd, idesc, (i > 0 || ch > 0 || k > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty_bar[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);
-      }
-    }
-  } else {
-    // ===================== epilogue warps: TMEM -> smem staging -> coalesced fp32 red.global.add =====================
-    const int ew = warp - 2;
-    const int q = warp & 3;
-    const int grp = ew >> 2;
-    uint8_t* stg = stg_base + ew * STG_BYTES;
-    uint8_t* my_row = stg + lane * STG_ROW;
-    const int srow = lane >> 3, sseg = lane & 7;
-    int local = 0;
-    for (int tile = unit; tile < g.total_tiles; tile += n_units, ++local) {
-      const WgTile t = wg_decode(g, tile);
-      const WgradProblem& P = g.p[t.pi];
-      const int n0 = t.n0 * BN;
-      const int acc = local & 1;
-      const uint32_t acc_ph = (local >> 1) & 1;
-      const int m = t.m0 + q * 32 + lane;
-      mbar_wait(&tfull_bar[acc], acc_ph);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16);
-      const float rs = (m < P.M && P.scale) ? P.scale[m] : 1.0f;
-      float* obase = P.out + static_cast<int64_t>(t.tap) * P.N;
-      constexpr int NCH = BN / 32;
-      bool released = false;
-#pragma unroll 1
-      for (int cc = grp; cc < NCH; cc += 2) {
-        const int c = cc * 32;
-        uint32_t v[32];
-        __syncwarp();
-        tmem_ld32(trow + c, v);
-        tmem_ld_wait();
-        if (cc + 2 >= NCH) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-          released = true;
-        }
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(my_row + j * 4) = make_float4(__uint_as_float(v[j]) * rs, __uint_as_float(v[j + 1]) * rs,
-                                                                    __uint_as_float(v[j + 2]) * rs, __uint_as_float(v[j + 3]) * rs);
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int r = j * 4 + srow;
-          const int mm = t.m0 + q * 32 + r;
-          const int n = n0 + c + sseg * 4;
-          if (mm < P.M && n + 4 <= P.N)
-            red_add_f32x4(obase + static_cast<int64_t>(mm) * P.out_ld + n, *reinterpret_cast<const float4*>(stg + r * STG_ROW + sseg * 16));
-        }
-      }
-      if (!released) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;
+  const int wrow = wg * 64 + (warp & 3) * 16;
+  const uint32_t smem0 = smem_u32(smem);
+  float acc[BN / 2];
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = unit; tile < g.total_tiles; tile += n_units) {
+    const WgTile t = wg_decode(g, tile);
+    const WgradProblem& P = g.p[t.pi];
+    mma_tile<BN, 1, 1>(acc, smem0, stage_bytes, KCH, STAGES, t.n_iters, wg, lane, s, ph, full_bar, empty_bar);
+    wgrad_epilogue<BN>(acc, P.out + static_cast<int64_t>(t.tap) * P.N, P.out_ld, P.scale, P.M, P.N, t.m0 + wrow + (lane >> 2), t.n0 * BN, lane);
   }
 }
 
@@ -1323,20 +920,20 @@ static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cuda
     if (P.iters_per_split > max_iters) max_iters = P.iters_per_split;
   }
   g.total_tiles = total;
-  const SmemPlan sp = plan_smem(BN, false, false, false, max_iters, 0, 1);
+  const SmemPlan sp = plan_smem(BN, false, max_iters, 0, 1);
   if (sp.stages < 2) {
     set_error("cb_gemm_wgrad_group: not enough shared memory for a 2-stage pipeline (BN=%d)", BN);
     return CB_ERR_INVALID;
   }
-  const int smem_bytes = sp.stages * sp.kch * Cfg::STAGE_BYTES + sp.epi_bytes + Cfg::BAR_BYTES + 1024;
+  const int smem_bytes = sp.stages * sp.kch * Cfg::STAGE_BYTES + Cfg::BAR_BYTES + 1024;
   const int units = sm_count();
-  launch_gemm_k(kern, total < units ? total : units, gemm_threads(8), smem_bytes, stream, g, sp.stages, sp.kch, sp.epi_bytes);
+  launch_gemm_k(kern, total < units ? total : units, GEMM_THREADS, smem_bytes, stream, g, sp.stages, sp.kch);
   return check_launch("cb_gemm_wgrad_group");
 }
 
 }  // namespace cb
 
-/* bring-up / tuning hook (not part of the public header): device buffer of >= 16 x grid int64 receiving clock64() stamps of every CTA */
+/* bring-up / tuning hook (not part of the public header): device buffer of >= 32 x grid int64 receiving clock64() stamps of every CTA */
 extern "C" void cb_debug_gemm_timeline(void* device_buf) { cb::g_gemm_timeline = static_cast<long long*>(device_buf); }
 extern "C" void cb_debug_gemm_kch(int kch) { cb::g_force_kch = kch; }
 extern "C" void cb_debug_gemm_mn3d(int on) { cb::g_mn3d = on ? 1 : 0; }
@@ -1378,13 +975,15 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
   epi.seed = d.dropout_seed;
   epi.dbg = g_gemm_timeline;
   epi.mn3d = 0;
-  epi.shift_smem = 0;
   {
     const DropCfg dc = make_drop(d.dropout_p, d.dropout_seed);
     epi.drop_thresh = dc.thresh;
     epi.drop_inv_keep = dc.inv_keep;
     epi.seed_off = dc.offset;
   }
+  const double gflop = 2.0e-9 * d.m * d.n * d.k * d.ntaps;
+  const bool want_occ2 = (d.reserved & 64) == 0 && (!d.block_n || d.block_n == 64) &&
+                         ((d.reserved & 32) ? g_occ2_mode >= 1 : (g_occ2_mode == 2 && (g_occ2_max_gflop <= 0.0 || gflop <= g_occ2_max_gflop)));
 
   if (d.mode == CB_GEMM_TN || d.mode == CB_GEMM_NN) {
     const bool nn = d.mode == CB_GEMM_NN;
@@ -1397,54 +996,35 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
     CB_REQUIRE(!(d.out2 && d.out_fp32), "cb_gemm(TN): out2 requires a bf16 primary output");
     CB_REQUIRE(d.rowmap == CB_ROWMAP_NONE || (d.map_h > 0 && d.map_w > 0), "cb_gemm: rowmap needs map_h/map_w");
     CB_REQUIRE(d.ntaps == 1 || d.tap_w > 2, "cb_gemm: tap modes need tap_w (padded row pitch in pixels)");
-    // TMA-prefetch epilogue whenever the output is bf16 (residual / aux tiles arrive by TMA; the output leaves by TMA store
-    // or, when rows are re-mapped, by cooperative coalesced stores)
-    const bool tma_epi = !d.out_fp32 && (d.reserved & 1) == 0 && !(d.rowmap != CB_ROWMAP_NONE && (d.out2 || d.dropout_p > 0.0f)) &&
-                         (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 && (!d.out2 || (reinterpret_cast<uintptr_t>(d.out2) & 15) == 0) &&
-                         (!d.residual || (reinterpret_cast<uintptr_t>(d.residual) & 15) == 0) &&
-                         (!d.aux || (reinterpret_cast<uintptr_t>(d.aux) & 15) == 0);
-    // two CTAs per SM (see g_occ2_mode): TMA epilogue only (the staged bf16 epilogue needs 168 registers)
-    const double gflop = 2.0e-9 * d.m * d.n * d.k * d.ntaps;
-    const bool want_occ2 = tma_epi && (d.reserved & 64) == 0 && (!d.block_n || d.block_n <= 128) &&
-                           ((d.reserved & 32) ? g_occ2_mode >= 1 : (g_occ2_mode == 2 && (g_occ2_max_gflop <= 0.0 || gflop <= g_occ2_max_gflop)));
     if (want_occ2) {
-      const LaunchCfg l2 = choose_config(d, tma_epi, 2);
-      if (l2.bn == 64) return nn ? launch_gemm<64, 2, 1, 2>(d, epi, stream) : launch_gemm<64, 0, 1, 2>(d, epi, stream);
-      if (l2.bn == 128) return nn ? launch_gemm<128, 2, 1, 2>(d, epi, stream) : launch_gemm<128, 0, 1, 2>(d, epi, stream);
+      const LaunchCfg l2 = choose_config(d, 2);
+      if (l2.bn == 64) return nn ? launch_gemm<64, 2, 2>(d, epi, stream) : launch_gemm<64, 0, 2>(d, epi, stream);
     }
-    const LaunchCfg lc = choose_config(d, tma_epi);
-#define CB_DISPATCH(BN_)                                                                                                     \
-  return nn ? (tma_epi ? launch_gemm<BN_, 2, 1>(d, epi, stream) : launch_gemm<BN_, 2, 0>(d, epi, stream))            \
-            : (tma_epi ? launch_gemm<BN_, 0, 1>(d, epi, stream) : launch_gemm<BN_, 0, 0>(d, epi, stream))
+    const LaunchCfg lc = choose_config(d);
     switch (lc.bn) {
-      case 64: CB_DISPATCH(64);
-      case 128: CB_DISPATCH(128);
-      case 256: CB_DISPATCH(256);
+      case 64: return nn ? launch_gemm<64, 2>(d, epi, stream) : launch_gemm<64, 0>(d, epi, stream);
+      case 128: return nn ? launch_gemm<128, 2>(d, epi, stream) : launch_gemm<128, 0>(d, epi, stream);
+      case 256: return nn ? launch_gemm<256, 2>(d, epi, stream) : launch_gemm<256, 0>(d, epi, stream);
       default: CB_REQUIRE(false, "cb_gemm: block_n must be 0, 64, 128 or 256 (got %d)", lc.bn);
     }
-#undef CB_DISPATCH
   } else {
     CB_REQUIRE(d.out_fp32 == 1, "cb_gemm(WGRAD): output must be fp32");
     CB_REQUIRE(d.m % 8 == 0 && d.n % 8 == 0, "cb_gemm(WGRAD): m, n must be multiples of 8 (got %d, %d)", d.m, d.n);
     CB_REQUIRE(d.out_ld % 4 == 0, "cb_gemm(WGRAD): out_ld must be a multiple of 4");
     CB_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "cb_gemm(WGRAD): out must be 16-byte aligned");
-    const double gflop = 2.0e-9 * d.m * d.n * d.k * d.ntaps;
-    const bool want_occ2 = (d.reserved & 64) == 0 && (!d.block_n || d.block_n <= 128) &&
-                           ((d.reserved & 32) ? g_occ2_mode >= 1 : (g_occ2_mode == 2 && (g_occ2_max_gflop <= 0.0 || gflop <= g_occ2_max_gflop)));
     if (want_occ2) {
-      const LaunchCfg l2 = choose_config(d, false, 2);
+      const LaunchCfg l2 = choose_config(d, 2);
       cb_gemm_desc d2 = d;
       d2.split_k = l2.splits;
-      if (l2.bn == 64) return launch_gemm<64, 1, 0, 2>(d2, epi, stream);
-      if (l2.bn == 128) return launch_gemm<128, 1, 0, 2>(d2, epi, stream);
+      if (l2.bn == 64) return launch_gemm<64, 1, 2>(d2, epi, stream);
     }
-    const LaunchCfg lc = choose_config(d, false);
+    const LaunchCfg lc = choose_config(d);
     cb_gemm_desc d2 = d;
     d2.split_k = lc.splits;
     switch (lc.bn) {
-      case 64: return launch_gemm<64, 1, 0>(d2, epi, stream);
-      case 128: return launch_gemm<128, 1, 0>(d2, epi, stream);
-      case 256: return launch_gemm<256, 1, 0>(d2, epi, stream);
+      case 64: return launch_gemm<64, 1>(d2, epi, stream);
+      case 128: return launch_gemm<128, 1>(d2, epi, stream);
+      case 256: return launch_gemm<256, 1>(d2, epi, stream);
       default: CB_REQUIRE(false, "cb_gemm(WGRAD): block_n must be 0, 64, 128 or 256 (got %d)", lc.bn);
     }
   }

@@ -30,13 +30,13 @@ inline int check_launch(const char* what) {
 // Programmatic dependent launch (PDL). Every kernel of this library starts with griddepcontrol.wait (all of its global
 // memory traffic comes after it) and griddepcontrol.launch_dependents, and is launched with the programmatic-stream-
 // serialization attribute: the next kernel's CTAs are scheduled while this one drains and run their prologue (barrier
-// init, TMEM allocation, descriptor prefetch) under its tail. A step is ~500-900 dependent launches of 5-60 us, so the
+// init, descriptor prefetch) under its tail. A step is ~500-900 dependent launches of 5-60 us, so the
 // ~2-4 us launch + prologue bubble between them is a double-digit share of the step. Works inside CUDA-graph capture
-// (programmatic dependency edges). OFF by default (cb_set_pdl(1) / CB_PDL=1 enables): it is worth +1.6 % on a single
-// stream but defeats the two-stream wgrad overlap (+9.6 %), see include/clipbert_b200.h.
+// (programmatic dependency edges). OFF by default (cb_set_pdl(1) / CB_PDL=1 enables): it can defeat the two-stream wgrad
+// overlap, see include/clipbert_b200.h.
 extern std::atomic<int> g_pdl;
 
-// g_pdl: 0 off, 1 every kernel, 2 every kernel EXCEPT the persistent tcgen05 GEMMs (their early-launched CTAs would hold ~200 KB
+// g_pdl: 0 off, 1 every kernel, 2 every kernel EXCEPT the persistent GEMMs (their early-launched CTAs would hold ~200 KB
 // of shared memory per SM while they wait; an LN / attention / column-sum CTA holds a few KB)
 template <bool kGemm, typename... KArgs, typename... Args>
 inline void launch_k_impl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
@@ -67,7 +67,7 @@ inline void launch_gemm_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t 
 bool get_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows, uint64_t ld,
                  uint32_t box_inner, uint32_t box_rows);
 
-// the same matrix as {64, rows, cols / 64}: one box = nblk swizzled [box_rows x 64] slabs (MN-major UMMA operands)
+// the same matrix as {64, rows, cols / 64}: one box = nblk swizzled [box_rows x 64] slabs (MN-major wgmma operands)
 bool get_tmap_3d_mn(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t ld, uint32_t box_rows, uint32_t nblk);
 
 #define CB_REQUIRE(cond, ...)        \

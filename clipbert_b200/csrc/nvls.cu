@@ -1,4 +1,4 @@
-// Hand-written all-reduce of a flat fp32 gradient buffer through the NVSwitch (NVLink SHARP, "NVLS") - the B200-native form of
+// Hand-written all-reduce of a flat fp32 gradient buffer through the NVSwitch (NVLink SHARP, "NVLS") - the NVSwitch-native form of
 // the data-parallel exchange that Horovod + NCCL perform for the reference (src/tasks/run_video_retrieval.py:299-301,432).
 //
 // Every rank allocates the buffer as symmetric memory and maps it at a MULTICAST address (torch.distributed._symmetric_memory:

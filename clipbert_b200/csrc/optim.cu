@@ -141,7 +141,7 @@ int cb_sumsq(const float* x, int64_t n, const int64_t* chunks, int nchunks, floa
     return check_launch("cb_sumsq");
   }
   const int64_t want = (n / 4 + 255) / 256;
-  const int grid = static_cast<int>(want < 1 ? 1 : (want > 148 * 8 ? 148 * 8 : want));   // 8 resident 256-thread CTAs per SM
+  const int grid = static_cast<int>(want < 1 ? 1 : (want > 132 * 8 ? 132 * 8 : want));   // 8 resident 256-thread CTAs per H100 SM
   launch_k(sumsq_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), x, n, out);
   return check_launch("cb_sumsq");
 }

@@ -18,7 +18,7 @@ from .modeling import (ClipBertForMultipleChoice, ClipBertForPreTraining, ClipBe
 def allreduce_flat(grads, group=None, average=True, async_op=False):
     """Sum (or average) a list of flat gradient buffers over the data-parallel group, in place.
 
-    The B200 replacement of ``hvd.DistributedOptimizer``'s per-parameter allreduce + ``synchronize()``
+    The H100 replacement of ``hvd.DistributedOptimizer``'s per-parameter allreduce + ``synchronize()``
     (src/tasks/run_video_retrieval.py:299-301,432): two flat fp32 buffers, one NCCL all-reduce each.
     """
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
@@ -391,7 +391,7 @@ class ClipBert(nn.Module):
         dist.all_reduce(flag, op=dist.ReduceOp.MIN, group=group)
         return bool(int(flag.item()))
 
-    def enable_overlapped_allreduce(self, group=None, average=True, cnn_buckets=False, exchange="nccl", max_ctas=None, wire="fp32", tail_ctas=148):
+    def enable_overlapped_allreduce(self, group=None, average=True, cnn_buckets=False, exchange="nccl", max_ctas=None, wire="fp32", tail_ctas=132):
         """Start the all-reduce of the transformer gradient buffer (75 % of the payload) as soon as the last
         outstanding transformer backward of the step has finished, so that it overlaps the remaining CNN backward
         (what Horovod's background fusion thread did for the reference). ``allreduce_grads()`` then only exchanges
@@ -402,8 +402,7 @@ class ClipBert(nn.Module):
         The collective is issued from the wgrad side stream, which is the stream those gradients are written on.
         ``wire="bf16"``: exchange the gradients as bf16 (see ``_bf16_wire_exchange``).
         ``max_ctas``: CTAs of the NVLS kernel while it overlaps the backward; ``None`` picks by world size - a rank reduces 1/world of
-        the buffer, so two ranks need twice the CTAs of four to finish inside the CNN backward (measured, profiles/r02_multi_gpu.txt:
-        N = 2: 64 CTAs 10.28 ms/step, 32 CTAs 11.1-11.3; N = 4: 64 CTAs 10.15, 32 CTAs 10.21; N = 8: 32 CTAs 10.36 ms, 64 CTAs 10.50)."""
+        the buffer, so two ranks need twice the CTAs of four to finish inside the CNN backward."""
         assert exchange in ("nccl", "nvls") and wire in ("fp32", "bf16")
         if not max_ctas:
             world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1

@@ -1,5 +1,5 @@
-"""GridFeatBackbone on B200: detectron2 MSRA ResNet-50 (res5) + grid_encoder, forward and backward,
-as tcgen05 implicit-GEMM convolutions over NHWC bf16 activations.
+"""GridFeatBackbone on H100: detectron2 MSRA ResNet-50 (res5) + grid_encoder, forward and backward,
+as wgmma implicit-GEMM convolutions over NHWC bf16 activations.
 
 Mirrors the reference module ``src/modeling/grid_feat.py:GridFeatBackbone`` (same constructor
 arguments, ``forward(x: (B,T,3,H,W)) -> (B,T,h,w,768)``, ``.feature``, ``.grid_encoder``,
@@ -160,7 +160,7 @@ class GridFeatBackbone(nn.Module):
         if freeze_at < 1:
             # the reference ships FREEZE_AT: 2 (Base-RCNN-grid.yaml) and only ever freezes more (freeze_cnn_backbone); the
             # backward of the stem (max-pool scatter + 7x7 wgrad) is not built, and silently returning no gradient is worse
-            raise NotImplementedError("GridFeatBackbone: FREEZE_AT = 0 (trainable stem) is not supported on the B200 path")
+            raise NotImplementedError("GridFeatBackbone: FREEZE_AT = 0 (trainable stem) is not supported on the H100 path")
         bb = self.feature.backbone
         if freeze_at >= 1:
             for p in bb.stem.parameters():
@@ -379,7 +379,7 @@ class GridFeatBackbone(nn.Module):
         cur = torch.empty(n * hh * ww, 64, dtype=bf16, device=dev)
         mode = self.stem_mode
         if mode == "s2d":
-            # space-to-depth frame (no patch matrix) -> 4-row-tap tcgen05 GEMM over its overlapping 64-element rows; the
+            # space-to-depth frame (no patch matrix) -> 4-row-tap wgmma GEMM over its overlapping 64-element rows; the
             # output keeps the (ho+3) x (wo+3) grid of the s2d frame, the pool reads it with those pitches
             hs, ws = ho + 3, wo + 3
             rows = n * hs * ws

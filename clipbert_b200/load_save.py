@@ -1,4 +1,4 @@
-"""Checkpoint key layouts of the reference, into and out of the B200 modules (SURVEY.md §8 f4).
+"""Checkpoint key layouts of the reference, into and out of the H100 modules (SURVEY.md §8 f4).
 
 Mirrors the three entry points the reference task scripts use to get weights into ``ClipBert``
 (src/tasks/run_video_retrieval.py:202-210):

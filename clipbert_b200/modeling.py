@@ -1,11 +1,11 @@
-"""Cross-modal transformer half of ClipBERT on B200.
+"""Cross-modal transformer half of ClipBERT on H100.
 
 Mirrors the reference classes in ``src/modeling/modeling.py`` / ``src/modeling/transformers.py``
 (ClipBertBaseModel, ClipBertForVideoTextRetrieval, ClipBertForSequenceClassification,
 ClipBertForMultipleChoice, ClipBertForPreTraining): same constructor (a BertConfig-like object),
 same forward signatures and return dicts, same state_dict keys (SURVEY.md App. B). The torch.nn
 modules below are PARAMETER CONTAINERS only — their own ``forward`` is never called. All arithmetic
-is the hand-written sm_100a kernels behind libclipbert_sm100.so:
+is the hand-written sm_90a kernels behind libclipbert_sm90.so:
 
   embeddings     cb_embed_text_fwd / cb_embed_visual_fwd (gather + sum + LN + dropout; the visual
                  kernel also fuses the frame mean, the row/col/type adds, repeat_tensor_rows and
@@ -809,7 +809,7 @@ class ClipBertForRegression(nn.Module):
 
     def __init__(self, config):
         super().__init__()
-        raise NotImplementedError("ClipBertForRegression is not built on the B200 path (unused by every reference task script)")
+        raise NotImplementedError("ClipBertForRegression is not built on the H100 path (unused by every reference task script)")
 
 
 class BertPredictionHeadTransform(nn.Module):

@@ -96,8 +96,8 @@ def launch_count():
 
 
 def set_attention_flash(on):
-    """Forward attention of sequences longer than 64 tokens: 1 (default) = tensor-core online-softmax kernel (2.1x on config 5,
-    profiles/r02_ab_runs.txt), 0 = the CUDA-core kernel."""
+    """Forward attention of sequences longer than 64 tokens: 1 (default) = tensor-core online-softmax kernel, 0 = the
+    CUDA-core kernel."""
     L.lib().cb_debug_attention_flash(int(bool(on)))
 
 
@@ -162,7 +162,7 @@ def set_pdl(enable):
 class SideQueue:
     """Runs launches that nothing downstream in the backward pass waits for (wgrad GEMMs, bias column sums) on a second
     CUDA stream, forked from / joined back into the current stream with events, so that they fill SMs the dgrad chain
-    leaves idle (grids below 148 CTAs, tails, the LayerNorm / attention kernels between GEMMs). Works under CUDA-graph
+    leaves idle (grids below one CTA per SM, tails, the LayerNorm / attention kernels between GEMMs). Works under CUDA-graph
     capture (fork/join become graph edges). Operands are kept referenced until ``join()`` so the caching allocator cannot
     hand their memory to a later launch on the main stream while the side stream still reads them."""
     _streams = {}
@@ -219,7 +219,8 @@ def set_gemm_timing(events):
     _gemm_timing = events
 
 
-# Measured launch configurations (tools/autotune_gemm.py on a B200 -> clipbert_b200/gemm_tuning.json): for each GEMM
+# Measured launch configurations (tools/autotune_gemm.py on the target GPU -> clipbert_b200/gemm_tuning.json, meant to be
+# committed together with the GPU model it was measured on; absent by default): for each GEMM
 # shape of the workload the fastest (tile width, wgrad K-split, k-chunks per stage). Shapes that are not in the table use
 # the library's analytic model (choose_config in csrc/gemm.cu).
 _tuning = None

@@ -1,5 +1,5 @@
 /*
- * clipbert_b200.h — C ABI of libclipbert_sm100.so, the B200 (sm_100a) kernels behind the ClipBERT
+ * clipbert_b200.h — C ABI of libclipbert_sm90.so, the H100 (sm_90a) kernels behind the ClipBERT
  * forward/backward hot path.
  *
  * The reference (jayleicn/ClipBERT) has no FFI: its hot path is a stack of torch.nn modules whose
@@ -32,16 +32,16 @@ typedef enum cb_status {
 } cb_status;
 
 const char* cb_last_error(void);
-/* library version and the SM architecture it was compiled for (100 = sm_100a) */
+/* library version and the SM architecture it was compiled for (90 = sm_90a) */
 int cb_version(void);
 int cb_sm_arch(void);
 /* number of kernels this library has launched since load (process-wide, all threads). */
 int64_t cb_launch_count(void);
 /* Programmatic dependent launch between this library's kernels (default OFF; env CB_PDL=1 or cb_set_pdl(1) enables):
  * each kernel's prologue overlaps the previous kernel's tail; every kernel issues griddepcontrol.wait before its first
- * global access, so results are identical to plain stream order. Measured on B200 (profiles/r01b_ab_runs.txt): +1.6 %
- * on a single-stream step, but it cancels the +9.6 % of running the wgrad GEMMs on a second stream, because early-
- * launched dependent CTAs hold their 200 KB of shared memory while they wait and keep the other stream off those SMs.
+ * global access, so results are identical to plain stream order. It can cancel the gain of running the wgrad GEMMs on a
+ * second stream: early-launched dependent GEMM CTAs hold their ~200 KB of shared memory while they wait and keep the other
+ * stream off those SMs.
  * enable = 2: every kernel EXCEPT the persistent GEMMs (an LN / attention / column-sum CTA waiting early holds a few KB).
  * Returns the previous setting. Replaces nothing in the reference (its ~400 launches per clip are plain stream-
  * ordered cuDNN/cuBLAS/ATen kernels, SURVEY.md section 8 a1). */
@@ -61,7 +61,7 @@ int cb_dropout_offset_bind(const uint64_t* device_word);
 int cb_dropout_offset_advance(uint64_t* counter, uint64_t* snapshot, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Tensor-core contraction (tcgen05.mma, TMA operand staging, TMEM accumulators).
+ * Tensor-core contraction (wgmma, TMA operand staging, register accumulators).
  *
  * One descriptor covers every dense contraction on the path:
  *   nn.Linear            src/modeling/transformers.py:218-220,292,357,372,467  modeling.py:534-539
@@ -137,10 +137,11 @@ typedef struct cb_gemm_desc {
   int32_t rowmap, map_h, map_w; /* spatial size (unpadded) for cb_rowmap */
   float dropout_p;
   uint64_t dropout_seed;
-  int32_t block_n;  /* 0 = let the library choose (64 / 128 / 256) */
-  int32_t reserved; /* tuning / test knobs: bit0 force the staged (non-TMA) epilogue, bit5 ask for / bit6 forbid the
-                       two-CTAs-per-SM instantiation (128 x <=128 tiles), bits 8-11 k-chunks per pipeline stage
-                       (0 = automatic); other bits ignored */
+  int32_t block_n;  /* 0 = let the library choose (64 / 128; 256 for CB_GEMM_WGRAD). An explicit 256 for TN / NN runs correctly
+                       but is slow on sm_90a: nine warps per CTA cap a thread at 168 registers and the 128 x 256 fused
+                       epilogue spills at that budget */
+  int32_t reserved; /* tuning / test knobs: bit5 ask for / bit6 forbid the two-CTAs-per-SM instantiation (128 x 64
+                       tiles), bits 8-11 k-chunks per pipeline stage (0 = automatic); other bits ignored */
 } cb_gemm_desc;
 
 int cb_gemm(const cb_gemm_desc* desc, void* stream);

@@ -44,7 +44,7 @@ FROZEN_BN_EPS = 1e-5
 # Rounding hooks. With the defaults (identity) every function below is the plain fp32 restatement
 # that is pinned against the reference. ``Rounding.bf16()`` turns the SAME functions into the
 # "bf16-rounding-matched oracle" of SURVEY.md §7: values are rounded to bf16 at exactly the points
-# where the B200 path stores bf16 (activations after each fused conv / linear epilogue, tensor-core
+# where the H100 path stores bf16 (activations after each fused conv / linear epilogue, tensor-core
 # weight operands, FrozenBN scale folded into the conv weight before rounding), all sums stay fp32.
 # ----------------------------------------------------------------------------------------------
 class Rounding:

@@ -3,7 +3,7 @@ import torch
 
 
 def cnn_relu_masks(stash, prefix="cnn.feature.backbone."):
-    """ReLU activation patterns of a B200 forward (from its backward stash) as oracle-side NCHW bool masks."""
+    """ReLU activation patterns of an H100 forward (from its backward stash) as oracle-side NCHW bool masks."""
     n = stash["n"]
     masks = {}
     for st in stash["blocks"]:
@@ -19,7 +19,7 @@ def cnn_relu_masks(stash, prefix="cnn.feature.backbone."):
 
 
 def cnn_patterns(stash, grid, prefix="cnn."):
-    """Rounding object carrying the ReLU pattern and the max-pool selection of a B200 CNN forward."""
+    """Rounding object carrying the ReLU pattern and the max-pool selection of an H100 CNN forward."""
     import torch.nn.functional as F
     from oracle import clipbert_ref as R
     n, h, w = stash["n"], stash["h"], stash["w"]

@@ -3,7 +3,7 @@
 Purpose: run the Python orchestration of clipbert_b200/modeling.py (buffer planning, stash, forward/backward call order,
 epilogue flags, index bookkeeping) on a machine without a GPU and compare it with the oracle. It swaps the functions of
 clipbert_b200.ops for torch code that does what the header says each entry point does (bf16 buffers in, fp32 arithmetic,
-bf16 / fp32 out); nothing in the product imports this file, and the kernels themselves are only ever checked on a B200
+bf16 / fp32 out); nothing in the product imports this file, and the kernels themselves are only ever checked on an H100
 (tests/test_gpu_*.py). Dropout must be off (the counter RNG of the kernels is not restated here).
 """
 import contextlib

@@ -132,6 +132,46 @@ def test_bench_other_baseline_configs_on_cpu(monkeypatch, capsys, config):
         assert d["fused_optimizer"] is None and calls["attention_bwd"] == 0 and calls["attention_fwd"] > 0
 
 
+@pytest.mark.parametrize("flags", [["--clip_batching", "1"], ["--clip_batching", "0"], ["--config", "c5", "--n_clips", "3", "--n_ex", "2"]])
+def test_bench_dump_outputs_on_cpu(monkeypatch, capsys, tmp_path, flags):
+    """--dump-outputs DIR: after the timed steps the last step's logits (both clip paths), loss and gradient sample / norms
+    (training) land in DIR as float32 / float64 .npy files, well under 64 MB; inference writes the logits only."""
+    import numpy as np
+    import bench
+    from ops_emulator import emulated_ops
+    cpu = torch.device("cpu")
+    for name, val in (("Stream", _Stream), ("Event", _Event), ("CUDAGraph", _Graph), ("graph", _ctx), ("stream", _ctx),
+                      ("current_stream", lambda *a: _Stream()), ("synchronize", lambda *a: None), ("set_device", lambda *a: None),
+                      ("is_available", lambda: False)):
+        monkeypatch.setattr(torch.cuda, name, val)
+    monkeypatch.setattr(bench, "_device", lambda r: cpu)
+    monkeypatch.setattr(bench, "_pin", lambda t: t)
+    out_dir = tmp_path / "dump"
+    argv = ["bench.py", "--gpus", "1", "--steps", "2", "--warmup", "1", "--batch", "2", "--n_clips", "2", "--n_frm", "1", "--size", "64",
+            "--txt_len", "12", "--no_cpu", "1", "--overlap_wgrad", "0", "--optimizer", "0", "--graph", "0", "--prefetch", "0",
+            "--dump-outputs", str(out_dir)] + flags
+    monkeypatch.setattr(sys, "argv", argv)
+    for k in ("RANK", "LOCAL_RANK", "WORLD_SIZE"):
+        monkeypatch.delenv(k, raising=False)
+    with emulated_ops(ignore_dropout=True):
+        bench.main()
+    out, _ = capsys.readouterr()
+    d = json.loads([l for l in out.splitlines() if l.startswith("{")][-1])
+    assert d["steps"] == 2
+    inference = "--config" in flags
+    files = sorted(os.listdir(out_dir))
+    assert files == (["logits.npy"] if inference else ["grad_norms.npy", "grad_sample.npy", "logits.npy", "loss.npy"])
+    logits = np.load(out_dir / "logits.npy")
+    assert logits.dtype == np.float32 and np.isfinite(logits).all()
+    n_clips = 3 if inference else 2
+    assert logits.shape[0] == n_clips
+    if not inference:
+        assert np.load(out_dir / "loss.npy").dtype == np.float32 and np.load(out_dir / "grad_sample.npy").dtype == np.float32
+        norms = np.load(out_dir / "grad_norms.npy")
+        assert norms.dtype == np.float64 and (norms > 0).any()
+    assert sum(os.path.getsize(out_dir / f) for f in files) < 64 << 20
+
+
 def calls_per_step_expected(flags):
     # GEMM launches of one training step: CNN 53 convs forward + backward of res3-5 / grid_encoder, transformer 12 layers + heads;
     # the per-clip loop runs the whole thing once per clip

@@ -1,4 +1,4 @@
-"""Model-level parity of the B200 path against the CPU oracle (same seeded weights and inputs).
+"""Model-level parity of the H100 path against the CPU oracle (same seeded weights and inputs).
 
 Forward: per stage and end to end, against BOTH the plain fp32 oracle and the bf16-rounding-matched
 oracle (oracle.clipbert_ref.Rounding.bf16). Backward: every trainable parameter gradient and the

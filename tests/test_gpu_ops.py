@@ -20,7 +20,14 @@ def _rnd(g, *shape, scale=1.0, dev="cuda"):
 
 
 # ------------------------------------------------------------------------------------------------ GEMM
-SINGLE, STAGED, OCC2 = 2, 1, 32      # cb_gemm_desc.reserved test knobs (OCC2: the two-CTAs-per-SM instantiations)
+# cb_gemm_desc.reserved values: SINGLE (bit 1, no meaning to the kernel) makes ops.gemm launch exactly the given descriptor
+# (no tuning-table lookup); OCC2 (bit 5) asks for the two-CTAs-per-SM instantiation. NARROW is a test-side flag, not a reserved
+# bit: the case runs on 128 x 64 tiles (block_n = 64) instead of the width the launch model picks.
+SINGLE, NARROW, OCC2 = 2, 1, 32
+
+
+def _tiles(flag):
+    return dict(block_n=64) if flag & NARROW else {}
 
 
 @pytest.mark.parametrize("cfg", [(64, SINGLE), (128, SINGLE), (256, SINGLE)])
@@ -52,19 +59,20 @@ def test_gemm_nn_dgrad(cuda, shape, knob):
 
 @pytest.fixture(params=["tma_store", "two_ctas_per_sm"])
 def epilogue_variant(request):
-    """The GEMM's TMA epilogue in its two instantiations: 16 epilogue warps / one CTA per SM (default), and two CTAs per SM
-    (ops.set_occ2(2): 128 x <=128 tiles, 8 epilogue warps taking their 32 columns in two passes, a single output chunk
-    buffer when the shared-memory half is tight)."""
+    """The GEMM in its two instantiations: one CTA per SM (id "tma_store", kept so that the test ids stay stable; the operands
+    arrive by TMA, the epilogue runs in the consumer warpgroups), and two CTAs per SM (ops.set_occ2(2): every eligible launch
+    on 128 x 64 tiles with <= 113 KB of shared memory)."""
     ops = _ops()
     ops.set_occ2(2 if request.param == "two_ctas_per_sm" else 0)
     yield request.param
     ops.set_occ2(1)
 
 
-@pytest.mark.parametrize("staged", [0, STAGED])
-@pytest.mark.parametrize("shape", [(500, 384, 256), (20000, 512, 128), (3000, 64, 64)])
-def test_gemm_epilogues(cuda, staged, shape, epilogue_variant):
-    """Both epilogue I/O paths (TMA-prefetched / TMA-stored vs. per-warp staged), several tiles per persistent CTA."""
+@pytest.mark.parametrize("narrow", [0, NARROW])
+@pytest.mark.parametrize("shape", [(500, 384, 256), (20000, 512, 128), (3000, 64, 64), (500, 392, 256)])
+def test_gemm_epilogues(cuda, narrow, shape, epilogue_variant):
+    """Every epilogue kind on the width the launch model picks and on 128 x 64 tiles (narrow = NARROW), several tiles per
+    persistent CTA; N = 392 (N % 16 == 8) takes the guarded epilogue with a ragged last column group in bf16."""
     ops = _ops()
     M, N, K = shape
     g = torch.Generator().manual_seed(3)
@@ -72,26 +80,27 @@ def test_gemm_epilogues(cuda, staged, shape, epilogue_variant):
     scale = (torch.rand(N, generator=g) + 0.5).to(cuda)
     shift = torch.randn(N, generator=g).to(cuda)
     acc = A.float() @ B.float().t()
-    base = dict(mode=ops.CB_GEMM_TN, m=M, n=N, k=K, a=A, a_rows=M, a_ld=K, b=B, b_rows=N, b_ld=K, out_ld=N, reserved=staged)
+    base = dict(mode=ops.CB_GEMM_TN, m=M, n=N, k=K, a=A, a_rows=M, a_ld=K, b=B, b_rows=N, b_ld=K, out_ld=N, reserved=SINGLE)
+    tiles = _tiles(narrow)
     C, C2 = torch.zeros(M, N, device=cuda, dtype=torch.bfloat16), torch.zeros(M, N, device=cuda, dtype=torch.bfloat16)
-    ops.gemm(**base, scale=scale, shift=shift, residual=R, res_ld=N, act=ops.ACT_RELU, out=C, out2=C2, out2_ld=N)
+    ops.gemm(**base, **tiles, scale=scale, shift=shift, residual=R, res_ld=N, act=ops.ACT_RELU, out=C, out2=C2, out2_ld=N)
     pre = acc * scale + shift + R.float()
     assert relerr(C, pre.relu()) < TOL_BF16_OP and relerr(C2, pre) < TOL_BF16_OP
-    ops.gemm(**base, shift=shift, act=ops.ACT_GELU, out=C)
+    ops.gemm(**base, **tiles, shift=shift, act=ops.ACT_GELU, out=C)
     assert relerr(C, F.gelu(acc + shift)) < TOL_BF16_OP
-    ops.gemm(**base, shift=shift, act=ops.ACT_TANH, out=C)
+    ops.gemm(**base, **tiles, shift=shift, act=ops.ACT_TANH, out=C)
     assert relerr(C, torch.tanh(acc + shift)) < TOL_BF16_OP
     # gelu + stashed derivative from one erf (BertIntermediate forward), consumed by AUX_MUL in the backward
     u = acc + shift
-    ops.gemm(**base, shift=shift, act=ops.ACT_GELU_STASH_GRAD, out=C, out2=C2, out2_ld=N)
+    ops.gemm(**base, **tiles, shift=shift, act=ops.ACT_GELU_STASH_GRAD, out=C, out2=C2, out2_ld=N)
     dgelu = 0.5 * (1 + torch.erf(u / math.sqrt(2))) + u * torch.exp(-0.5 * u * u) / math.sqrt(2 * math.pi)
     assert relerr(C, F.gelu(u)) < TOL_BF16_OP and relerr(C2, dgelu) < TOL_BF16_OP
     a = AUX.float()
-    ops.gemm(**base, aux=AUX, aux_ld=N, aux_mode=ops.AUX_MUL, out=C)
+    ops.gemm(**base, **tiles, aux=AUX, aux_ld=N, aux_mode=ops.AUX_MUL, out=C)
     assert relerr(C, acc * a) < TOL_BF16_OP
     gelu_grad = 0.5 * (1 + torch.erf(a / math.sqrt(2))) + a * torch.exp(-0.5 * a * a) / math.sqrt(2 * math.pi)
     for mode, fac in [(ops.AUX_RELU_MASK, (a > 0).float()), (ops.AUX_GELU_GRAD, gelu_grad), (ops.AUX_TANH_GRAD, 1 - a * a)]:
-        ops.gemm(**base, residual=R, res_ld=N, aux=AUX, aux_ld=N, aux_mode=mode, out=C)
+        ops.gemm(**base, **tiles, residual=R, res_ld=N, aux=AUX, aux_ld=N, aux_mode=mode, out=C)
         assert relerr(C, (acc + R.float()) * fac) < TOL_BF16_OP
     # plain bf16 output, aux only, dropout + residual, every tile width
     for bn in (64, 128, 256):
@@ -99,14 +108,14 @@ def test_gemm_epilogues(cuda, staged, shape, epilogue_variant):
         assert relerr(C, acc) < TOL_BF16_OP
         ops.gemm(**base, aux=AUX, aux_ld=N, aux_mode=ops.AUX_RELU_MASK, out=C, block_n=bn)
         assert relerr(C, acc * (a > 0)) < TOL_BF16_OP
-    ops.gemm(**base, shift=shift, residual=R, res_ld=N, dropout_p=0.1, dropout_seed=5, out=C)
+    ops.gemm(**base, **tiles, shift=shift, residual=R, res_ld=N, dropout_p=0.1, dropout_seed=5, out=C)
     ones = torch.ones(M, N, device=cuda, dtype=torch.bfloat16)
     msk = torch.empty_like(ones)
     ops.dropout(ones, msk, 0.1, 5)
     assert relerr(C, (acc + shift) * msk.float() + R.float()) < TOL_BF16_OP
 
 
-@pytest.mark.parametrize("knob", [SINGLE, SINGLE | STAGED])
+@pytest.mark.parametrize("knob", [SINGLE, SINGLE | NARROW])
 @pytest.mark.parametrize("dims", [(2, 7, 7, 64, 64), (3, 14, 14, 128, 128), (2, 28, 28, 64, 192), (1, 3, 5, 512, 64), (64, 14, 14, 256, 256)])
 def test_conv3x3_fwd_and_dgrad(cuda, dims, knob, epilogue_variant):
     ops = _ops()
@@ -120,19 +129,19 @@ def test_conv3x3_fwd_and_dgrad(cuda, dims, knob, epilogue_variant):
     y = torch.zeros(NB * H * W, Cout, device=cuda, dtype=torch.bfloat16)
     wk = w.permute(0, 2, 3, 1).contiguous().view(Cout, 9 * Cin)
     ops.gemm(mode=ops.CB_GEMM_TN, m=P, n=Cout, k=Cin, a=xp, a_rows=P, a_ld=Cin, b=wk, b_rows=Cout, b_ld=9 * Cin, ntaps=9,
-             tap_w=W + 2, tap_sign=1, out=y, out_ld=Cout, rowmap=ops.ROWMAP_UNPAD, map_h=H, map_w=W, reserved=knob)
+             tap_w=W + 2, tap_sign=1, out=y, out_ld=Cout, rowmap=ops.ROWMAP_UNPAD, map_h=H, map_w=W, reserved=SINGLE, **_tiles(knob))
     ref = F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), padding=1).permute(0, 2, 3, 1).reshape(-1, Cout)
     assert relerr(y, ref) < TOL_BF16_OP
     # dgrad of a conv whose forward weight is wf [Cin(out), Cout(in), 3, 3] stored KRSC: x plays dY
     wf = _rnd(g, Cin, Cout, 3, 3, scale=0.05)
     wfk = wf.permute(0, 2, 3, 1).contiguous().view(Cin, 9 * Cout)         # [out_f, (r,s,in_f)] = forward layout
     ops.gemm(mode=ops.CB_GEMM_NN, m=P, n=Cout, k=Cin, a=xp, a_rows=P, a_ld=Cin, b=wfk, b_rows=Cin, b_ld=9 * Cout, ntaps=9,
-             tap_w=W + 2, tap_sign=-1, out=y, out_ld=Cout, rowmap=ops.ROWMAP_UNPAD, map_h=H, map_w=W, reserved=knob)
+             tap_w=W + 2, tap_sign=-1, out=y, out_ld=Cout, rowmap=ops.ROWMAP_UNPAD, map_h=H, map_w=W, reserved=SINGLE, **_tiles(knob))
     ref = F.conv_transpose2d(x.float().permute(0, 3, 1, 2), wf.float(), padding=1).permute(0, 2, 3, 1).reshape(-1, Cout)
     assert relerr(y, ref) < TOL_BF16_OP
 
 
-@pytest.mark.parametrize("knob", [0, STAGED])
+@pytest.mark.parametrize("knob", [0, NARROW])
 @pytest.mark.parametrize("dims", [(3, 5, 6, 64, 64), (40, 28, 28, 256, 128)])
 def test_rowmap_pad_keeps_border_zero(cuda, dims, knob, epilogue_variant):
     ops = _ops()
@@ -142,7 +151,7 @@ def test_rowmap_pad_keeps_border_zero(cuda, dims, knob, epilogue_variant):
     A, B, AUX = _rnd(g, M, K), _rnd(g, N, K, scale=0.1), _rnd(g, M, N)
     yp = torch.zeros(NB, H + 2, W + 2, N, device=cuda, dtype=torch.bfloat16)
     ops.gemm(mode=ops.CB_GEMM_TN, m=M, n=N, k=K, a=A, a_rows=M, a_ld=K, b=B, b_rows=N, b_ld=K, out=yp, out_ld=N,
-             rowmap=ops.ROWMAP_PAD, map_h=H, map_w=W, aux=AUX, aux_ld=N, aux_mode=ops.AUX_RELU_MASK, reserved=knob)
+             rowmap=ops.ROWMAP_PAD, map_h=H, map_w=W, aux=AUX, aux_ld=N, aux_mode=ops.AUX_RELU_MASK, reserved=SINGLE, **_tiles(knob))
     ref = ((A.float() @ B.float().t()) * (AUX.float() > 0)).view(NB, H, W, N)
     assert relerr(yp[:, 1:-1, 1:-1], ref) < TOL_BF16_OP
     border = yp.clone()

@@ -1,7 +1,7 @@
 """Host-side orchestration of clipbert_b200/modeling.py on CPU: the real Python engine (flat parameter buffers, stash, call
 order, epilogue flags, index bookkeeping) driven through tests/ops_emulator.py - torch restatements of what include/
 clipbert_b200.h says each entry point computes - and compared with the oracle's autograd. This checks the host logic
-without a GPU; the kernels behind the same calls are checked on a B200 by tests/test_gpu_*.py.
+without a GPU; the kernels behind the same calls are checked on an H100 by tests/test_gpu_*.py.
 """
 import numpy as np
 import pytest

@@ -1,6 +1,6 @@
 """CPU tests of the checkpoint key-layout helpers (SURVEY §8 f4, clipbert_b200/load_save.py) - index/key work, so the
-bar is exact equality. Where /root/reference exists the reference's own two functions are executed (their source is cut out
-of src/utils/load_save.py with ast - the module itself imports apex / easydict) and compared key for key."""
+bar is exact equality. What the reference's own two functions return on the same inputs (src/utils/load_save.py, run by
+tools/make_golden_reference_runs.py) is pinned in tests/golden/reference_runs.pt and compared key for key."""
 import ast
 import os
 import types
@@ -10,10 +10,14 @@ import torch
 
 from util import make_cfg
 
-REF = os.path.join(os.environ.get("CLIPBERT_REFERENCE_ROOT", "/root/reference"), "src", "utils", "load_save.py")
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_runs.pt")
 
 
 def _reference_functions():
+    """The two helpers of the reference's src/utils/load_save.py, cut out with ast (the module itself imports apex / easydict);
+    used by tools/make_golden_reference_runs.py."""
+    from oracle import ref_import
+    REF = os.path.join(ref_import.REFERENCE_ROOT, "src", "utils", "load_save.py")
     src = open(REF).read()
     tree = ast.parse(src)
     wanted = {"load_state_dict_with_mismatch", "convert_torchvision_ckpt_to_detectron2"}
@@ -86,26 +90,33 @@ def test_load_state_dict_with_mismatch_skips_foreign_and_misshapen_keys_and_roun
     assert all(torch.equal(a, b) for a, b in zip(fresh.state_dict().values(), model.state_dict().values()))
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="needs /root/reference")
+def _assert_matches_checksums(sd, want):
+    assert list(sd.keys()) == list(want.keys())
+    for k, (shape, s1, s2, head) in want.items():
+        f = torch.as_tensor(sd[k]).detach().double().flatten()
+        # the sums are float64 reductions whose order depends on the CPU: equal up to the last bits
+        assert tuple(sd[k].shape) == shape and abs(float(f.sum()) - s1) <= 1e-12 * max(1.0, abs(s1)), k
+        assert abs(float((f * f).sum()) - s2) <= 1e-12 * max(1.0, s2), k
+        assert torch.equal(f[:16].float(), head), k
+
+
 def test_helpers_agree_with_the_reference_functions(tmp_path):
     from clipbert_b200 import load_save as LS
-    ref = _reference_functions()
+    want = torch.load(GOLD, map_location="cpu", weights_only=False)["load_save"]
     tv = _tv_resnet50_state_dict()
     path = str(tmp_path / "tv.pth")
     torch.save(tv, path)
-    want = ref["convert_torchvision_ckpt_to_detectron2"](path)
     got = LS.convert_torchvision_ckpt_to_detectron2(path)
-    assert list(got["model"].keys()) == list(want["model"].keys()) and got["matching_heuristics"] == want["matching_heuristics"]
-    assert all(torch.equal(got["model"][k], want["model"][k]) for k in want["model"])
+    assert list(got["model"].keys()) == want["convert_keys"] and got["matching_heuristics"] == want["convert_heuristics"]
+    _assert_matches_checksums(got["model"], want["convert_checksums"])
     # load_state_dict_with_mismatch: run the reference's function and ours on two copies of the transformer
     from oracle import synth
     sd = {k[len("transformer."):]: v for k, v in synth.full_state_dict(7).items() if k.startswith("transformer.")}
     sd["classifier.2.weight"] = torch.zeros(7, 1536)
     sd["extra.weight"] = torch.zeros(3)
-    a, b = _model().transformer, _model().transformer
-    ref["load_state_dict_with_mismatch"](a, sd)
+    b = _model().transformer
     LS.load_state_dict_with_mismatch(b, sd)
-    assert all(torch.equal(x, y) for x, y in zip(a.state_dict().values(), b.state_dict().values()))
+    _assert_matches_checksums(b.state_dict(), want["mismatch_checksums"])
 
 
 def test_clipbert_load_state_dict_is_strict_except_for_the_dead_d2_heads():

@@ -1,5 +1,5 @@
 """The model-level GPU parity tests (tests/test_gpu_model.py) replayed on CPU: same test bodies, same oracle, same tolerances,
-with the C-ABI calls answered by tests/ops_emulator.py instead of the sm_100a kernels. What this checks is everything
+with the C-ABI calls answered by tests/ops_emulator.py instead of the sm_90a kernels. What this checks is everything
 *around* the kernels - the forward/backward engines, buffer layouts, flag plumbing, index plans - so that a host-side
 regression shows up in the CPU suite; the kernels themselves are only ever checked by the `-m gpu` run of the same bodies.
 """

@@ -1,5 +1,5 @@
-"""GPU parity tests for the paths added after the round's GPU budget was spent (written against the CPU oracle, first run on
-a B200 by the round-end driver). They sort last so that a surprise here cannot hide the result of the established suites.
+"""GPU parity tests of the clip-batched, long-sequence and loss-kernel paths (written against the CPU oracle). They sort last so
+that a surprise here cannot hide the result of the established suites.
 Every kernel they launch is one the earlier suites already cover; what is new is the host-side index bookkeeping.
 """
 import os
@@ -35,7 +35,7 @@ def _pretraining_model(weights, cuda, **cfg_extra):
 
 def test_pretraining_random_visual_token_sampling(cuda, weights):
     """VisualInputEmbedding's train-mode sampling (src/modeling/modeling.py:15-34,80-88): with numpy seeded like the oracle's
-    draw the B200 path keeps the same sorted subset; forward, the scattered grid gradient and the row / column position
+    draw the H100 path keeps the same sorted subset; forward, the scattered grid gradient and the row / column position
     table gradients (index_add of the virtual-grid gradient) against fp32 autograd on the oracle."""
     from oracle import clipbert_ref as R, synth
     model, sd = _pretraining_model(weights, cuda, pixel_random_sampling_size=7)
@@ -168,7 +168,7 @@ def test_fused_clip_lse_loss_kernel(cuda):
 def test_attention_tensor_core_forward_for_long_sequences(cuda, dims, variant):
     """The mma.sync online-softmax forward for L > 64 (attn_tc_fwd_flash_kernel; 448 px frames L = 69, paragraph retrieval
     L = 521) against fp32 torch attention and against the CUDA-core kernel it replaces: context, saved log-sum-exp (the general
-    backward consumes it), and the same dropout stream. Default for L > 64 since it passed on a B200 (profiles/r02_ab_runs.txt)."""
+    backward consumes it), and the same dropout stream. Default for L > 64."""
     from clipbert_b200 import ops
     from util import TOL_BF16_OP
     nseq, L, lt = dims

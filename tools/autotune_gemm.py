@@ -2,7 +2,8 @@
 
 Records the cb_gemm descriptors of one fwd+bwd step of the bench workload, then for each distinct shape times the candidate
 (tile width, wgrad K-split, k-chunks per stage) inside a CUDA graph and writes the winners to
-clipbert_b200/gemm_tuning.json, which ops.gemm consults at run time ("measure, don't guess").
+clipbert_b200/gemm_tuning.json, which ops.gemm consults at run time ("measure, don't guess"). The table is meant to be
+committed with the GPU model it was measured on (its "device" field); the per-shape report goes to tool_out/.
 """
 import argparse
 import json
@@ -171,8 +172,8 @@ def main():
             for bn in bns:
                 for kch in (0, 1, 2, 4):
                     cands.append((bn, 0, kch))
-        # two CTAs per SM (reserved bit 5): 128 x <=128 tiles only
-        cands = [c + (0,) for c in cands] + [c + (1,) for c in cands if c[0] <= 128 and c[2] in (0, 1)]
+        # two CTAs per SM (reserved bit 5): 128 x 64 tiles only
+        cands = [c + (0,) for c in cands] + [c + (1,) for c in cands if c[0] == 64 and c[2] in (0, 1)]
         best, best_t = None, base if base is not None else 1e9
         for (bn, sp, kch, occ2) in cands:
             t = time_cfg(ops, dict(call, block_n=bn, split_k=sp, reserved=(kch << 8) | (32 if occ2 else 64)))
@@ -194,8 +195,8 @@ def main():
     json.dump(dict(device=torch.cuda.get_device_name(0), note="(block_n, split_k, kch, two CTAs per SM) per GEMM shape; see tools/autotune_gemm.py",
                    configs=old), open(args.out, "w"), indent=0, sort_keys=True)
     print("tuned %d / %d shapes; predicted saving %.2f ms per step; wrote %s (%.1f s)" % (len(table), len(uniq), saved / 1e3, args.out, time.time() - t0))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    open(os.path.join(ROOT, "gpurun_out", "autotune_report_%s.txt" % args.config), "w").write("\n".join(report) + "\n")
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    open(os.path.join(ROOT, "tool_out", "autotune_report_%s.txt" % args.config), "w").write("\n".join(report) + "\n")
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 """Config 5 of BASELINE.json (paragraph-retrieval inference: 16 clips x 1 frame per video, 512-token captions, 8 captions per
-forward) on one B200 - a measurement tool for the next round, NOT the contract bench (bench.py measures the training step).
+forward) on one H100 - a measurement tool for the next round, NOT the contract bench (bench.py measures the training step).
 
     python tools/bench_inference.py [--flash 0|1] [--clips 16] [--captions 8] [--txt_len 512] [--size 224] [--steps 10]
 

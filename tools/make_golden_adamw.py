@@ -1,6 +1,6 @@
 """Generate tests/golden/adamw.pt from the REFERENCE's own optimizer class (src/optimization/adamw.py, imported where it
-lies) and torch.nn.utils.clip_grad_norm_, exactly as src/tasks/run_video_retrieval.py:477-487 drives them. Run in the
-authoring container only (needs /root/reference)."""
+lies) and torch.nn.utils.clip_grad_norm_, exactly as src/tasks/run_video_retrieval.py:477-487 drives them. Run beside a
+checkout of the reference (CLIPBERT_REFERENCE_ROOT)."""
 import importlib.util
 import os
 import sys
@@ -13,7 +13,8 @@ from torch.nn.utils import clip_grad_norm_  # noqa: E402
 
 
 def reference_adamw():
-    spec = importlib.util.spec_from_file_location("ref_adamw", "/root/reference/src/optimization/adamw.py")
+    from oracle import ref_import
+    spec = importlib.util.spec_from_file_location("ref_adamw", os.path.join(ref_import.REFERENCE_ROOT, "src", "optimization", "adamw.py"))
     m = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(m)
     return m.AdamW

@@ -1,5 +1,4 @@
-"""Per-stage parity numbers of the B200 path against the CPU oracle (run on the GPU box).
-Writes gpurun_out/parity_report.txt; a copy is committed under profiles/."""
+"""Per-stage parity numbers of the H100 path against the CPU oracle (needs a GPU); written to a text report."""
 import os
 import sys
 
@@ -106,8 +105,8 @@ def main():
         e, c = relerr(p.grad, r), cosine(p.grad, r)
         if ("layer." not in name) or (".layer.0." in name) or (".layer.11." in name) or e > 2e-2:
             out("  %-60s %.3e  %.6f" % (name, e, c))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "parity_report.txt"), "w") as f:
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    with open(os.path.join(ROOT, "tool_out", "parity_report.txt"), "w") as f:
         f.write("\n".join(lines) + "\n")
 
 

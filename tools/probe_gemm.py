@@ -1,6 +1,6 @@
-"""GPU bring-up probe for cb_gemm (tcgen05 GEMM): each case runs in its own subprocess under a
+"""GPU bring-up probe for cb_gemm (wgmma GEMM): each case runs in its own subprocess under a
 timeout so that a trapped or dead-locked kernel cannot take the box down. Not a pytest file;
-`python tools/probe_gemm.py` prints one line per case and writes gpurun_out/probe_gemm.json.
+`python tools/probe_gemm.py` prints one line per case and writes tool_out/probe_gemm.json.
 """
 import json
 import os
@@ -273,8 +273,8 @@ def main():
             results[c] = {"ok": False, "timeout": True}
         results[c]["secs"] = round(time.time() - t0, 1)
         print(c, json.dumps(results[c]), flush=True)
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/probe_gemm.json", "w") as f:
+    os.makedirs("tool_out", exist_ok=True)
+    with open("tool_out/probe_gemm.json", "w") as f:
         json.dump(results, f, indent=1)
 
 

@@ -1,5 +1,5 @@
 """Per-kernel device-time breakdown of one training step (eager launches, CUDA events around every launch).
-Writes gpurun_out/step_breakdown.txt. Usage: python tools/profile_step.py [--batch 32 --n_clips 2 ...]"""
+Writes tool_out/step_breakdown.txt. Usage: python tools/profile_step.py [--batch 32 --n_clips 2 ...]"""
 import argparse
 import os
 import sys
@@ -22,7 +22,7 @@ def main():
     ap.add_argument("--txt_len", type=int, default=32)
     ap.add_argument("--n_ex", type=int, default=1)
     ap.add_argument("--clip_batching", type=int, default=1)
-    ap.add_argument("--out", default="gpurun_out/step_breakdown.txt")
+    ap.add_argument("--out", default="tool_out/step_breakdown.txt")
     ap.add_argument("--ncu", type=int, default=0, help="1: bracket ONE step with cudaProfilerStart/Stop for "
                     "`ncu --profile-from-start off` instead of timing with events")
     args = ap.parse_args()

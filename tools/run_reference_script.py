@@ -4,7 +4,7 @@
     python -m torch.distributed.run --nproc-per-node 8 tools/run_reference_script.py /path/to/ClipBERT src/tasks/run_video_retrieval.py ...
 
 It (1) registers stand-ins for `horovod.torch` and `apex` when they are not installed (clipbert_b200.compat.install),
-(2) aliases `src.modeling.{e2e_model,modeling,grid_feat}` to the B200 modules (compat.alias_reference_modules) so that the
+(2) aliases `src.modeling.{e2e_model,modeling,grid_feat}` to the H100 modules (compat.alias_reference_modules) so that the
 script's own `from src.modeling.e2e_model import ClipBert` lines import them, (3) runs the script as `__main__` from the
 reference root. Everything else the script imports (easydict, tensorboardX, ujson, av, lmdb: data loading and logging) must be
 installed - those sit outside the hot path this package replaces.

@@ -1,7 +1,6 @@
-"""Stand-alone check + bandwidth probe of the NVLS all-reduce (csrc/nvls.cu) on N GPUs of one box - to be run in the next round:
+"""Stand-alone check + bandwidth probe of the NVLS all-reduce (csrc/nvls.cu) on N GPUs of one node:
 
-    /usr/local/graft/bin/gpurun --gpus 2 --timeout 600 -- \
-      'python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29611 tools/test_nvls.py'
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29611 tools/test_nvls.py
 
 Each rank fills a symmetric-memory fp32 buffer with rank-dependent values, runs barrier -> cb_nvls_allreduce_f32 -> barrier,
 checks the average element-wise (bit-exact: the sums are small integers), then times the exchange of the two buffer sizes of a
