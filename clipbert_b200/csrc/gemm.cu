@@ -16,6 +16,14 @@
 //               small per-warp fp32 staging tile so that every lane holds 16 consecutive columns of one row, applies the
 //               fused epilogue (bias / FrozenBN shift, residual, dropout, activation, stashes) and writes 16-byte vectors,
 //               re-mapping the output row (zero-bordered <-> compact pixel rows) where asked.
+//               The residual / aux tiles (bf16, rows m0 .. m0+127 of the A-row space in every row-map mode; with UNPAD that
+//               includes the zero-border rows the epilogue then drops, e.g. 81 / 49 of the useful aux rows on a 7 x 7 map) arrive by TMA in
+//               128B-swizzled [128 x 64] boxes: the producer loads them into one of N_IN epilogue-input buffers (own full /
+//               empty barrier pair), so they travel under the main loop and, with two buffers, under the previous tile's
+//               epilogue (see the producer for the order); a K loop longer than four chunks instead takes them in the operand
+//               ring stage after its operands and keeps its ring depth (plan_smem). A 1x1 conv at K = 64 is HBM-bound and its main loop is one
+//               k-chunk: reading residual / aux with per-lane global loads inside the epilogue left four dependent HBM round
+//               trips per tile and warp exposed.
 //   Epilogue (WGRAD): red.global.add.v2.f32 straight from the fragment (four lanes cover 32 contiguous bytes of a row).
 #include "common.cuh"
 #include "host_util.h"
@@ -34,14 +42,14 @@ constexpr int SMEM_LIMIT_OCC2 = 113 * 1024;     // two CTAs per SM: (228 KB - 2 
 constexpr int STG_PITCH = 36;                   // fp32 staging row pitch in floats (32 + 4: conflict-free 16-byte row reads)
 constexpr int STG_WARP_FLOATS = 16 * STG_PITCH; // one warp: 16 rows x 32 columns
 constexpr int EPI_BYTES = CONSUMER_WARPS * STG_WARP_FLOATS * 4;
+constexpr int IN_BOX_BYTES = BM * 64 * 2;       // one epilogue-input box: 128 rows x 64 bf16 columns, 128B swizzle
+constexpr int MAX_IN_BUFS = 2;
 
 struct GemmEpi {
   const float* scale;
   const float* shift;
-  const __nv_bfloat16* residual;
-  int64_t res_ld;
+  const __nv_bfloat16* residual;   // (read through the tmR / tmX tensor maps; the pointers only say which inputs exist)
   const __nv_bfloat16* aux;
-  int64_t aux_ld;
   int aux_mode;
   int act;
   void* out;
@@ -349,17 +357,32 @@ __device__ __forceinline__ void wgrad_epilogue(const float (&acc)[BN / 2], float
   }
 }
 
+// Shared-memory address of 16 bytes (8 bf16 columns, chunk q = 0..7 of the 128-byte row) in row r of a 128B-swizzled TMA box
+// (1024-byte aligned): the 16-byte chunks of a row are permuted by r % 8, so the 8 consecutive rows a quarter-warp reads at the
+// same logical chunk fall into 8 different bank groups.
+__device__ __forceinline__ uint32_t swz128(uint32_t box, int r, int q) { return box + r * 128 + ((q ^ (r & 7)) << 4); }
+
 template <int BN, int MODE, int OCC>
 __global__ void __launch_bounds__(GEMM_THREADS, OCC)
-    gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K, int ntaps, int tap_w,
-                int tap_sign, int iters_per_split, int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, int epi_bytes, GemmEpi epi) {
+    gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmR,
+                const __grid_constant__ CUtensorMap tmX, int M, int N, int K, int ntaps, int tap_w, int tap_sign, int iters_per_split,
+                int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, int N_IN, int epi_bytes, GemmEpi epi) {
   using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int stage_bytes = KCH * Cfg::STAGE_BYTES;           // a stage holds KCH consecutive 64-deep k-chunks (one barrier round trip)
-  uint8_t* stg_base = smem + STAGES * stage_bytes;          // epilogue staging (TN / NN)
+  // epilogue inputs of one tile (TN / NN): the residual boxes, then the aux boxes, BN / 64 of each. N_IN = 1 or 2: as many
+  // dedicated buffers of in_bytes; N_IN = 0 with inputs: they occupy the ring stage after the tile's operands (in_bytes <=
+  // stage_bytes), so that a long K loop keeps the whole ring for its operands
+  const bool has_res = MODE != 1 && epi.residual != nullptr, has_aux = MODE != 1 && epi.aux != nullptr;
+  constexpr int IN_TILE_BYTES = (BN / 64) * IN_BOX_BYTES;
+  const int in_bytes = (has_res + has_aux) * IN_TILE_BYTES;
+  uint8_t* in_base = smem + STAGES * stage_bytes;           // (1024-byte aligned: stage sizes are multiples of 8 KB)
+  uint8_t* stg_base = in_base + N_IN * in_bytes;            // epilogue staging (TN / NN)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + epi_bytes);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
+  uint64_t* in_full = empty_bar + MAX_STAGES;
+  uint64_t* in_empty = in_full + MAX_IN_BUFS;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -370,9 +393,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (has_res) tma_prefetch_desc(&tmR);
+    if (has_aux) tma_prefetch_desc(&tmX);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], CONSUMER_WARPS);
+    }
+    for (int b = 0; b < N_IN; ++b) {
+      mbar_init(&in_full[b], 1);
+      mbar_init(&in_empty[b], CONSUMER_WARPS);
     }
     fence_mbar_init();
   }
@@ -391,8 +420,43 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
       constexpr int B_BOXES = (MODE == 0) ? 1 : BN / 64;
       int s = 0;        // smem ring position / phase, carried across tiles
       uint32_t ph = 0;
+      int ib = 0;       // epilogue-input buffer / phase
+      uint32_t iph = 0;
+      // residual / aux boxes of a tile into the next input buffer, or into the next ring stage (N_IN = 0); rows and columns
+      // outside [M, N] arrive as zeros
+      auto load_inputs = [&](const TileInfo& t) {
+        uint64_t* bar;
+        uint8_t* dst;
+        if (N_IN) {
+          mbar_wait(&in_empty[ib], iph ^ 1);
+          bar = &in_full[ib];
+          dst = in_base + ib * in_bytes;
+          if (++ib == N_IN) { ib = 0; iph ^= 1; }
+        } else {
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          bar = &full_bar[s];
+          dst = smem + s * stage_bytes;
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+        mbar_expect_tx(bar, in_bytes);
+        if (has_res) {
+#pragma unroll
+          for (int j = 0; j < BN / 64; ++j) tma_load_2d(dst + j * IN_BOX_BYTES, &tmR, bar, t.n0 + j * 64, t.m0);
+          dst += IN_TILE_BYTES;
+        }
+        if (has_aux) {
+#pragma unroll
+          for (int j = 0; j < BN / 64; ++j) tma_load_2d(dst + j * IN_BOX_BYTES, &tmX, bar, t.n0 + j * 64, t.m0);
+        }
+      };
       for (int tile = unit; tile < total_tiles; tile += n_units) {
         const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
+        // A CTA's first N_IN tiles find their input buffer free: their inputs go out ahead of the operands. Later tiles' inputs
+        // follow their operands, so that the wait for a buffer (the epilogue N_IN tiles back) never holds back operand chunks the
+        // ring has room for; they then travel under the tile's main loop and, with two buffers, the previous tile's epilogue.
+        // In the ring (N_IN = 0) they always take the stage after the tile's operands.
+        const bool inputs_first = tile < unit + N_IN * n_units;
+        if (in_bytes && inputs_first) load_inputs(t);
         for (int i = 0; i < t.n_iters; i += KCH) {
           const int nch = min(KCH, t.n_iters - i);
           mbar_wait(&empty_bar[s], ph ^ 1);
@@ -437,6 +501,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
           if (++s == STAGES) { s = 0; ph ^= 1; }
           if (i == 0 && tile == unit) dbg_stamp(epi, 2);
         }
+        if (in_bytes && !inputs_first) load_inputs(t);
       }
       dbg_stamp(epi, 3);
     }
@@ -457,7 +522,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
   const int er = lane & 15, eh = lane >> 4;
   float* stg = reinterpret_cast<float*>(stg_base) + warp * STG_WARP_FLOATS;
   const bool has_out2 = epi.out2 != nullptr;
-  const bool has_res = epi.residual != nullptr, has_aux = epi.aux != nullptr;
   const bool has_shift = epi.shift != nullptr;
   // epilogue kind, fixed for the launch (see the EK_* functions)
   const bool full = (N & 15) == 0 && epi.scale == nullptr;
@@ -503,6 +567,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
       row_ok = row_ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
       orow = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
     }
+    // this tile's epilogue inputs (residual boxes, then aux boxes): tiles take the N_IN buffers in turn (the producer's order),
+    // or, with N_IN = 0, the ring stage after the tile's operands
+    const int ib = N_IN == 2 ? (local & 1) : 0;
+    const uint32_t in_buf = N_IN ? smem_u32(in_base) + ib * in_bytes : smem0 + s * stage_bytes;
+    if (in_bytes) {
+      if (N_IN) mbar_wait(&in_full[ib], static_cast<uint32_t>(N_IN == 2 ? local >> 1 : local) & 1u);
+      else mbar_wait(&full_bar[s], ph);
+    }
 #pragma unroll
     for (int sc = 0; sc < BN / 32; ++sc) {
       // fragment -> staging: this warp's 16 rows x 32 columns, then one row segment per lane
@@ -526,20 +598,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
         f[4 * j] = __uint_as_float(u.x); f[4 * j + 1] = __uint_as_float(u.y);
         f[4 * j + 2] = __uint_as_float(u.z); f[4 * j + 3] = __uint_as_float(u.w);
       }
+      // residual / aux of these 16 columns: box (column / 64), 16-byte chunks q, q + 1 of row wrow + er (zeros beyond N)
       uint32_t res16[NC / 2], aux16[NC / 2];
+      const int tc = sc * 32 + eh * 16;               // tile column of f[0]
+      const int q = (tc & 63) >> 3;
       if (has_res) {
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
-          uint4 u = make_uint4(0, 0, 0, 0);
-          if (nb + 8 * j + 8 <= N) u = __ldg(reinterpret_cast<const uint4*>(epi.residual + static_cast<int64_t>(m) * epi.res_ld + nb + 8 * j));
+          const uint4 u = lds128(swz128(in_buf + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
           res16[4 * j] = u.x; res16[4 * j + 1] = u.y; res16[4 * j + 2] = u.z; res16[4 * j + 3] = u.w;
         }
       }
       if (has_aux) {
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
-          uint4 u = make_uint4(0, 0, 0, 0);
-          if (nb + 8 * j + 8 <= N) u = __ldg(reinterpret_cast<const uint4*>(epi.aux + static_cast<int64_t>(m) * epi.aux_ld + nb + 8 * j));
+          const uint4 u = lds128(swz128(in_buf + (has_res ? IN_TILE_BYTES : 0) + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
           aux16[4 * j] = u.x; aux16[4 * j + 1] = u.y; aux16[4 * j + 2] = u.z; aux16[4 * j + 3] = u.w;
         }
       }
@@ -586,6 +659,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
           if (nb + 8 * j + 8 <= N) *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(o2_16[4 * j], o2_16[4 * j + 1], o2_16[4 * j + 2], o2_16[4 * j + 3]);
       }
     }
+    if (in_bytes) {                                 // this warp is done with the tile's inputs: hand the buffer / stage back
+      __syncwarp();
+      if (lane == 0) mbar_arrive(N_IN ? &in_empty[ib] : &empty_bar[s]);
+      if (!N_IN && ++s == STAGES) { s = 0; ph ^= 1; }
+    }
     if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 8);
   }
   if (threadIdx.x == 0) dbg_stamp(epi, 11);
@@ -610,18 +688,26 @@ static long long* g_gemm_timeline = nullptr;
 static int g_force_kch = 0;   // tuning hook: chunks per stage (0 = automatic)
 static int g_mn3d = 1;        // 1 (default) = MN-major operands through one 3-D TMA box per k-chunk (GemmEpi::mn3d); cb_debug_gemm_mn3d
 
-// Shared-memory plan of one launch: the epilogue staging (TN / NN: 16 x 32 fp32 per consumer warp; WGRAD: none), then as many
-// 64-deep operand chunks as fit, grouped KCH per stage. Every stage costs one full / empty barrier round trip whatever its size,
-// so deep stages are preferred to many shallow ones.
+// Shared-memory plan of one launch: the epilogue staging (TN / NN: 16 x 32 fp32 per consumer warp; WGRAD: none), n_in
+// epilogue-input buffers of in_bytes (the residual / aux boxes of one tile), then as many 64-deep operand chunks as fit, grouped
+// KCH per stage. Every stage costs one full / empty barrier round trip whatever its size, so deep stages are preferred to many
+// shallow ones. No ring is deeper than the K loop plus one stage: letting the producer of a persistent CTA run several one-chunk
+// tiles ahead measured slower on the plain K = 64 convolutions (H100 SXM, 400 W: 401408 x 256 x 64 +9 %, 401408 x 64 x 64 +17 %).
+// Epilogue inputs (residual / aux boxes of one tile, in_bytes): two dedicated buffers let the next tile's inputs load under this
+// tile's epilogue; they are taken when the ring beside them still holds a whole tile's K loop (the short K loops of the
+// HBM-bound 1x1 convs). A K loop of at most 4 chunks that cannot have both gets one buffer. A longer K loop keeps the ring it
+// has without inputs and lands its inputs in the ring stage after its operands (n_in = 0; needs in_bytes <= one stage): they load
+// under the end of its main loop, and the buffer does not cost the compute-bound main loop ring depth.
 struct SmemPlan {
-  int epi_bytes, kch, stages, chunk_bytes;
+  int epi_bytes, kch, stages, chunk_bytes, n_in;
 };
-static SmemPlan plan_smem(int bn, bool staging, int kiters, int force_kch = 0, int occ = 1) {
+static SmemPlan plan_ring(int bn, bool staging, int kiters, int force_kch, int occ, int in_bytes, int n_in) {
   SmemPlan p;
   const int limit = occ == 2 ? SMEM_LIMIT_OCC2 : SMEM_LIMIT;
   p.chunk_bytes = BM * BK * 2 + bn * BK * 2;
   p.epi_bytes = staging ? EPI_BYTES : 0;
-  const int chunks_fit = (limit - 1024 - GemmCfg<64>::BAR_BYTES - p.epi_bytes) / p.chunk_bytes;
+  p.n_in = n_in;
+  const int chunks_fit = (limit - 1024 - GemmCfg<64>::BAR_BYTES - p.epi_bytes - n_in * in_bytes) / p.chunk_bytes;
   p.kch = 1;
   if (force_kch > 0) p.kch = force_kch;
   else if (g_force_kch > 0) p.kch = g_force_kch;
@@ -634,6 +720,18 @@ static SmemPlan plan_smem(int bn, bool staging, int kiters, int force_kch = 0, i
   const int stage_iters = ceil_div(kiters, p.kch);
   if (p.stages > stage_iters + 1) p.stages = stage_iters + 1 > 2 ? stage_iters + 1 : 2;   // no ring deeper than the K loop
   return p;
+}
+static SmemPlan plan_smem(int bn, bool staging, int kiters, int force_kch = 0, int occ = 1, int in_bytes = 0) {
+  const SmemPlan none = plan_ring(bn, staging, kiters, force_kch, occ, 0, 0);
+  if (in_bytes == 0) return none;
+  const SmemPlan two = plan_ring(bn, staging, kiters, force_kch, occ, in_bytes, 2);
+  if (two.stages >= 2 && two.stages * two.kch >= kiters) return two;
+  if (kiters > 4 && none.stages >= 2 && none.kch * none.chunk_bytes >= in_bytes) return none;
+  return plan_ring(bn, staging, kiters, force_kch, occ, in_bytes, 1);
+}
+// bytes of one tile's residual / aux boxes (TN / NN)
+static int epi_in_bytes(const cb_gemm_desc& d, int bn) {
+  return d.mode == CB_GEMM_WGRAD ? 0 : ((d.residual != nullptr) + (d.aux != nullptr)) * (bn / 64) * IN_BOX_BYTES;
 }
 
 template <int BN, int MODE, int OCC = 1>
@@ -654,7 +752,7 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
     attr_set = true;
   }
   // Tensor maps are copied out of the cache into this frame (and from here into the kernel's parameter space)
-  alignas(64) CUtensorMap ta, tb;
+  alignas(64) CUtensorMap ta, tb, tr, tx;
   bool mn3d = false;
   int iters_per_split = 0;
   const int tiles_m = ceil_div(d.m, BM), tiles_n = ceil_div(d.n, BN);
@@ -684,19 +782,26 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
     total *= splits * d.ntaps;
     kiters = iters_per_split;
   }
+  // epilogue inputs (TN / NN): residual / aux [M, N] at the tile's A rows, 128 x 64 boxes; unused map slots carry a copy of ta
+  tr = ta;
+  tx = ta;
+  if (MODE != 1 && d.residual) ok = ok && get_tmap_2d(&tr, d.residual, d.n, d.m, d.res_ld, 64, BM);
+  if (MODE != 1 && d.aux) ok = ok && get_tmap_2d(&tx, d.aux, d.n, d.m, d.aux_ld, 64, BM);
   if (!ok) return CB_ERR_CUDA;
   epi.mn3d = mn3d ? 1 : 0;
-  const SmemPlan sp = plan_smem(BN, MODE != 1, kiters, (d.reserved >> 8) & 15, OCC);
-  const int epi_bytes = sp.epi_bytes, kch = sp.kch, stages = sp.stages;
-  if (stages < 2) {
-    set_error("cb_gemm: not enough shared memory for a 2-stage pipeline (BN=%d, epilogue %d B, %d CTA(s) per SM)", BN, epi_bytes, OCC);
-    return CB_ERR_INVALID;
-  }
-  const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + epi_bytes + Cfg::BAR_BYTES + 1024;
   const int units = sm_count() * OCC;
   const int grid = total < units ? total : units;
-  launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, iters_per_split, tiles_m,
-                tiles_n, total, stages, kch, epi_bytes, epi);
+  const int in_bytes = epi_in_bytes(d, BN);
+  const SmemPlan sp = plan_smem(BN, MODE != 1, kiters, (d.reserved >> 8) & 15, OCC, in_bytes);
+  const int epi_bytes = sp.epi_bytes, kch = sp.kch, stages = sp.stages;
+  if (stages < 2) {
+    set_error("cb_gemm: not enough shared memory for a 2-stage pipeline (BN=%d, epilogue %d B + inputs %d B, %d CTA(s) per SM)", BN, epi_bytes,
+              in_bytes, OCC);
+    return CB_ERR_INVALID;
+  }
+  const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + sp.n_in * in_bytes + epi_bytes + Cfg::BAR_BYTES + 1024;
+  launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, iters_per_split,
+                tiles_m, tiles_n, total, stages, kch, sp.n_in, epi_bytes, epi);
   return check_launch("cb_gemm");
 }
 
@@ -735,7 +840,8 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, int occ = 1) {
       const int real_sp = wgrad ? ceil_div(kc, ips) : 1;
       const int64_t tiles = base * real_sp;
       const double rounds = static_cast<double>((tiles + units - 1) / units);
-      const SmemPlan pl = plan_smem(bn, !wgrad, ips, (d.reserved >> 8) & 15, occ);
+      // the ring left beside the epilogue-input buffers of this tile width
+      const SmemPlan pl = plan_smem(bn, !wgrad, ips, (d.reserved >> 8) & 15, occ, epi_in_bytes(d, bn));
       if (pl.stages < 2) continue;
       // a ring of 2 chunks cannot cover the TMA round trip of a long K loop
       const double shallow = (pl.stages * pl.kch < 3 && ips > 2) ? 3.0 : 1.0;
@@ -959,9 +1065,7 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
   epi.scale = d.scale;
   epi.shift = d.shift;
   epi.residual = static_cast<const __nv_bfloat16*>(d.residual);
-  epi.res_ld = d.res_ld;
   epi.aux = static_cast<const __nv_bfloat16*>(d.aux);
-  epi.aux_ld = d.aux_ld;
   epi.aux_mode = d.aux ? d.aux_mode : CB_AUX_NONE;
   epi.act = d.act;
   epi.out = d.out;
@@ -992,6 +1096,8 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
     CB_REQUIRE(d.out_ld % 8 == 0, "cb_gemm(TN): out_ld must be a multiple of 8");
     CB_REQUIRE(!d.residual || d.res_ld % 8 == 0, "cb_gemm(TN): res_ld must be a multiple of 8");
     CB_REQUIRE(!d.aux || d.aux_ld % 8 == 0, "cb_gemm(TN): aux_ld must be a multiple of 8");
+    CB_REQUIRE((reinterpret_cast<uintptr_t>(d.residual) & 15) == 0, "cb_gemm(TN): residual must be 16-byte aligned");
+    CB_REQUIRE((reinterpret_cast<uintptr_t>(d.aux) & 15) == 0, "cb_gemm(TN): aux must be 16-byte aligned");
     CB_REQUIRE(!d.out2 || d.out2_ld % 8 == 0, "cb_gemm(TN): out2_ld must be a multiple of 8");
     CB_REQUIRE(!(d.out2 && d.out_fp32), "cb_gemm(TN): out2 requires a bf16 primary output");
     CB_REQUIRE(d.rowmap == CB_ROWMAP_NONE || (d.map_h > 0 && d.map_w > 0), "cb_gemm: rowmap needs map_h/map_w");

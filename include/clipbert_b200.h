@@ -123,7 +123,7 @@ typedef struct cb_gemm_desc {
   /* epilogue */
   const float* scale;
   const float* shift;
-  const void* residual;
+  const void* residual; /* residual / aux: bf16 [m, n] at the A row m (TN / NN), base 16-byte aligned, ld a multiple of 8 */
   int64_t res_ld;
   const void* aux;
   int64_t aux_ld;
@@ -139,7 +139,8 @@ typedef struct cb_gemm_desc {
   uint64_t dropout_seed;
   int32_t block_n;  /* 0 = let the library choose (64 / 128; 256 for CB_GEMM_WGRAD). An explicit 256 for TN / NN runs correctly
                        but is slow on sm_90a: nine warps per CTA cap a thread at 168 registers and the 128 x 256 fused
-                       epilogue spills at that budget */
+                       epilogue spills at that budget; with both residual and aux its input tiles do not fit beside a
+                       2-stage ring, and the launch runs on 64-wide tiles */
   int32_t reserved; /* tuning / test knobs: bit5 ask for / bit6 forbid the two-CTAs-per-SM instantiation (128 x 64
                        tiles), bits 8-11 k-chunks per pipeline stage (0 = automatic); other bits ignored */
 } cb_gemm_desc;
