@@ -50,6 +50,13 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// arrive only where pred holds, predicated inside the instruction: no divergent branch between a warpgroup's wgmma (ptxas
+// serialises wgmma around compiler-inserted warpgroup arrives on divergent paths)
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(smem_u32(bar)),
+               "r"(static_cast<uint32_t>(pred))
+               : "memory");
+}
 // try_wait with a suspend-time hint: the thread is parked in hardware until the phase completes or ~2 us pass, instead of
 // returning after the ~30-cycle default limit, so that a waiting producer lane does not take issue slots from the warps that
 // share its scheduler.
@@ -68,6 +75,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > CB_SPIN_LIMIT) __trap();
+  }
+}
+// The same without the spin guard, for warps that raised their register budget with setmaxnreg.inc: ptxas allocates the code
+// around a trap within the kernel's entry budget, which spills a 232-register consumer. A dead-locked pipeline still traps in
+// the producer, which waits on the same ring.
+__device__ __forceinline__ void mbar_wait_unguarded(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
   }
 }
 
@@ -140,6 +154,21 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// signal a named barrier without waiting on it (the other nthreads - 32 x warps arriving threads wait in bar.sync)
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// register reallocation between the warpgroups of a CTA (sm_90a): every warp of the warpgroup executes the same instruction.
+// dec gives registers back to the CTA's pool; inc blocks until the pool has enough. The kernel must be compiled for the full
+// per-thread budget of its launch bounds, so that the registers given back cover those asked for.
+template <uint32_t NREG>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(NREG));
+}
+template <uint32_t NREG>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(NREG));
 }
 
 // ---------------------------------------------------------------------------------------

@@ -6,25 +6,37 @@
 //   MODE 1 (WGRAD) : dW = dY^T X with both operands read MN-major from the activation layout,
 //                    split over the pixel/token dimension, fp32 red.global accumulation.
 //
-// Structure (persistent CTAs, grid = min(#tiles, #SMs x CTAs per SM), static round-robin tile schedule):
-//   warp 8      TMA producer   : smem ring of STAGES x (A 128x64 | B BNx64) bf16 tiles, 128B swizzle
-//   warps 0..7  two consumer warpgroups: warpgroup g multiplies rows 64g .. 64g+63 of the tile with wgmma m64nBNk16 into
-//               registers, hands every smem stage back as soon as the products that read it have retired (one stage of
-//               wgmma stays in flight), then runs the epilogue of its rows while the producer already fills the ring
-//               with the next tile's operands.
-//   Epilogue (TN / NN): each warp owns 16 rows of the tile. Per 32-column slice it moves its accumulator fragment through a
-//               small per-warp fp32 staging tile so that every lane holds 16 consecutive columns of one row, applies the
-//               fused epilogue (bias / FrozenBN shift, residual, dropout, activation, stashes) and writes 16-byte vectors,
-//               re-mapping the output row (zero-bordered <-> compact pixel rows) where asked.
-//               The residual / aux tiles (bf16, rows m0 .. m0+127 of the A-row space in every row-map mode; with UNPAD that
-//               includes the zero-border rows the epilogue then drops, e.g. 81 / 49 of the useful aux rows on a 7 x 7 map) arrive by TMA in
-//               128B-swizzled [128 x 64] boxes: the producer loads them into one of N_IN epilogue-input buffers (own full /
-//               empty barrier pair), so they travel under the main loop and, with two buffers, under the previous tile's
-//               epilogue (see the producer for the order); a K loop longer than four chunks instead takes them in the operand
-//               ring stage after its operands and keeps its ring depth (plan_smem). A 1x1 conv at K = 64 is HBM-bound and its main loop is one
-//               k-chunk: reading residual / aux with per-lane global loads inside the epilogue left four dependent HBM round
-//               trips per tile and warp exposed.
-//   Epilogue (WGRAD): red.global.add.v2.f32 straight from the fragment (four lanes cover 32 contiguous bytes of a row).
+// Every kernel is persistent (grid = min(#tiles, #SMs x CTAs per SM), static round-robin tile schedule) and fills a shared-memory
+// ring of STAGES x KCH x (A 128x64 | B BNx64) bf16 k-chunks, 128B swizzle, from ONE elected TMA producer lane.
+//
+// TN / NN: gemm_pingpong_kernel, 384 threads = three warpgroups, one CTA per SM.
+//   warpgroup 0   TMA producer. Its warps give registers back (setmaxnreg.dec 40); one lane issues the operand boxes and the
+//                 epilogue-input boxes in tile order.
+//   warpgroups 1, 2  consumers (setmaxnreg.inc 232). Each owns WHOLE 128 x BN tiles (BN = 64 / 128): per k16 step two wgmma
+//                 m64nBNk16, rows 0-63 and 64-127, into BN fp32 accumulators per thread. A CTA's local tile j belongs to
+//                 consumer j & 1 ("ping-pong"). The main loops run in tile order: a consumer starts tile j's main loop when the
+//                 other one has issued the last wgmma of tile j-1 (named barrier per consumer); the other consumer then runs
+//                 tile j-1's epilogue while this one's wgmma run. So a tile's epilogue - fused
+//                 arithmetic and 16-byte stores, which at K = 64 takes several times as long as the main loop - overlaps the
+//                 next tile's main loop and, when it is the longer part, the other consumer's epilogue. Both consumers walk the
+//                 one operand ring, each skipping the other's stages (n_iters is the same for every TN / NN tile). A stage is
+//                 read by one consumer, so its empty barrier counts that consumer's four warps.
+//   Epilogue:     each warp owns rows 16w .. 16w+15 of both 64-row halves of its tile. Per half and 32-column slice it moves its
+//                 accumulator fragment through a small per-warp fp32 staging tile so that every lane holds 16 consecutive
+//                 columns of one row, applies the fused epilogue (bias / FrozenBN shift, residual, dropout, activation,
+//                 stashes) and writes 16-byte vectors, re-mapping the output row (zero-bordered <-> compact pixel rows) where
+//                 asked. The residual / aux tiles (bf16, rows m0 .. m0+127 of the A-row space in every row-map mode; with UNPAD
+//                 that includes the zero-border rows the epilogue then drops) arrive by TMA in 128B-swizzled [128 x 64] boxes:
+//                 into one of N_IN epilogue-input buffers with their own full / empty barrier pair (with two buffers, each
+//                 consumer has its own), or, for K loops longer than four chunks, into the operand ring stage after the
+//                 tile's operands (plan_smem). Reading them with per-lane global loads inside the epilogue left four dependent
+//                 HBM round trips per tile and warp exposed on the one-chunk main loops of the HBM-bound 1x1 convs.
+//
+// WGRAD: gemm_kernel (and wgrad_group_kernel below), 288 threads: warp 8 is the TMA producer, warps 0..7 two consumer
+//   warpgroups that multiply rows 64g .. 64g+63 of one 128 x BN tile (BN up to 256) with wgmma m64nBNk16, hand every ring stage
+//   back as soon as the products that read it have retired (one stage of wgmma stays in flight), then add the tile into the fp32
+//   output with red.global.add.v2.f32 straight from the fragment (four lanes cover 32 contiguous bytes of a row). Optionally two
+//   CTAs per SM (OCC = 2, 128 x 64 tiles), so that one CTA's epilogue runs under the other's main loop.
 #include "common.cuh"
 #include "host_util.h"
 
@@ -32,10 +44,14 @@ namespace cb {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int CONSUMER_WARPS = 8;                          // two warpgroups of 64 tile rows each
+constexpr int CONSUMER_WARPS = 8;                          // WGRAD: two warpgroups of 64 tile rows each
 constexpr int GEMM_THREADS = (CONSUMER_WARPS + 1) * 32;    // + the TMA producer warp
-// (Nine warps put three on each SM sub-partition, which caps a thread at 168 registers: the 128 x 256 tiles of the TN / NN
-// epilogue spill at that budget, so the launch model only picks them for the weight gradients, whose epilogue is lean.)
+// (Nine warps put three on each SM sub-partition, which caps a thread at 168 registers; the lean red.add epilogue of the weight
+// gradients fits 128 x 256 tiles in that budget.)
+constexpr int PP_THREADS = 3 * 128;                        // TN / NN: producer warpgroup + two consumer warpgroups
+constexpr int PP_PRODUCER_REGS = 40;                       // 128 x 40 + 256 x 232 = 64512 = 384 x 168, the entry budget
+constexpr int PP_CONSUMER_REGS = 232;
+constexpr int PP_BAR_TURN = 1;                             // named barriers 1, 2: consumer 0 / 1 may start its next main loop
 constexpr int MAX_STAGES = 8;
 constexpr int SMEM_LIMIT = 232448;              // 227 KB opt-in limit per CTA
 constexpr int SMEM_LIMIT_OCC2 = 113 * 1024;     // two CTAs per SM: (228 KB - 2 x 1 KB reserved) / 2
@@ -43,7 +59,6 @@ constexpr int STG_PITCH = 36;                   // fp32 staging row pitch in flo
 constexpr int STG_WARP_FLOATS = 16 * STG_PITCH; // one warp: 16 rows x 32 columns
 constexpr int EPI_BYTES = CONSUMER_WARPS * STG_WARP_FLOATS * 4;
 constexpr int IN_BOX_BYTES = BM * 64 * 2;       // one epilogue-input box: 128 rows x 64 bf16 columns, 128B swizzle
-constexpr int MAX_IN_BUFS = 2;
 
 struct GemmEpi {
   const float* scale;
@@ -338,6 +353,60 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], uint32_t smem0, i
   }
 }
 
+// The same for one consumer warpgroup of the ping-pong kernel, which owns the whole 128-row tile: per k16 step one wgmma for rows
+// 0-63 (acc[0]) and one for rows 64-127 (acc[1]), so every accumulator sees its k steps in the order of mma_tile. Once the last
+// wgmma group of the tile is committed, the other consumer may start its main loop (pass_bar, 0 = no next tile); in_stage: the
+// tile's epilogue inputs follow its operands in the ring, and have landed before the turn passes.
+template <int BN, int TB>
+__device__ __forceinline__ void mma_tile_pp(float (&acc)[2][BN / 2], uint32_t smem0, int stage_bytes, int KCH, int STAGES, int n_iters,
+                                            int lane, int& s, uint32_t& ph, uint64_t* full_bar, uint64_t* empty_bar, int pass_bar,
+                                            bool in_stage) {
+  using Cfg = GemmCfg<BN>;
+  int prev = -1;
+  for (int i = 0; i < n_iters; i += KCH) {
+    const int nch = min(KCH, n_iters - i);
+    mbar_wait_unguarded(&full_bar[s], ph);
+    __syncwarp();
+    wgmma_fence();
+    wgmma_fence_acc(acc[0]);
+    wgmma_fence_acc(acc[1]);
+    for (int ch = 0; ch < nch; ++ch) {
+      const uint32_t a_addr = smem0 + s * stage_bytes + ch * Cfg::STAGE_BYTES;
+      const uint32_t b_addr = a_addr + Cfg::A_BYTES;
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t bd = TB ? gmma_desc(b_addr + k * 2048, BK * 128, 1024) : gmma_desc(b_addr + k * 32, 16, 1024);
+        const uint32_t accum = (i > 0 || ch > 0 || k > 0) ? 1u : 0u;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) wgmma_bf16<BN, 0, TB>(acc[h], gmma_desc(a_addr + h * (64 * 128) + k * 32, 16, 1024), bd, accum);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_fence_acc(acc[0]);
+    wgmma_fence_acc(acc[1]);
+    if (prev >= 0) {
+      __syncwarp();
+      mbar_arrive_if(&empty_bar[prev], lane == 0);
+    }
+    prev = s;
+    if (++s == STAGES) { s = 0; ph ^= 1; }
+    if (pass_bar && i + KCH >= n_iters) {
+      // the tile's inputs in the ring stage after its operands (see the consumer loop of gemm_pingpong_kernel): that stage's
+      // slot was last held by an operand stage of this tile that has just been handed back, so the producer can fill it
+      if (in_stage) mbar_wait_unguarded(&full_bar[s], ph);
+      named_bar_arrive(pass_bar, 2 * 128);
+    }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc[0]);
+  wgmma_fence_acc(acc[1]);
+  if (prev >= 0) {
+    __syncwarp();
+    mbar_arrive_if(&empty_bar[prev], lane == 0);
+  }
+}
+
 // ---- weight-gradient epilogue: out[tap * N + n] of rows m += acc * scale[m], straight from the wgmma fragment ----------------------
 // Fragment layout of m64nNk16 (f32): warp w of the warpgroup holds rows 16w + lane/4 (d[4j], d[4j+1]) and 16w + lane/4 + 8
 // (d[4j+2], d[4j+3]) at columns 8j + 2 (lane % 4) + {0, 1}.
@@ -362,29 +431,31 @@ __device__ __forceinline__ void wgrad_epilogue(const float (&acc)[BN / 2], float
 // same logical chunk fall into 8 different bank groups.
 __device__ __forceinline__ uint32_t swz128(uint32_t box, int r, int q) { return box + r * 128 + ((q ^ (r & 7)) << 4); }
 
-template <int BN, int MODE, int OCC>
-__global__ void __launch_bounds__(GEMM_THREADS, OCC)
-    gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmR,
-                const __grid_constant__ CUtensorMap tmX, int M, int N, int K, int ntaps, int tap_w, int tap_sign, int iters_per_split,
-                int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, int N_IN, int epi_bytes, GemmEpi epi) {
+// ===================================== TN / NN: ping-pong consumers =====================================
+template <int BN, int MODE>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+    gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmR,
+                         const __grid_constant__ CUtensorMap tmX, int M, int N, int K, int ntaps, int tap_w, int tap_sign, int tiles_m,
+                         int tiles_n, int total_tiles, int STAGES, int KCH, int N_IN, GemmEpi epi) {
+  static_assert(MODE != 1 && BN <= 128, "TN / NN tiles of 128 x 64 or 128 x 128");
   using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int stage_bytes = KCH * Cfg::STAGE_BYTES;           // a stage holds KCH consecutive 64-deep k-chunks (one barrier round trip)
-  // epilogue inputs of one tile (TN / NN): the residual boxes, then the aux boxes, BN / 64 of each. N_IN = 1 or 2: as many
-  // dedicated buffers of in_bytes; N_IN = 0 with inputs: they occupy the ring stage after the tile's operands (in_bytes <=
-  // stage_bytes), so that a long K loop keeps the whole ring for its operands
-  const bool has_res = MODE != 1 && epi.residual != nullptr, has_aux = MODE != 1 && epi.aux != nullptr;
+  // epilogue inputs of one tile: the residual boxes, then the aux boxes, BN / 64 of each. N_IN = 2: one dedicated buffer per
+  // consumer; N_IN = 1: one buffer the consumers take in turn; N_IN = 0 with inputs: they occupy the ring stage after the
+  // tile's operands (in_bytes <= stage_bytes), so that a long K loop keeps the whole ring for its operands
+  const bool has_res = epi.residual != nullptr, has_aux = epi.aux != nullptr;
   constexpr int IN_TILE_BYTES = (BN / 64) * IN_BOX_BYTES;
   const int in_bytes = (has_res + has_aux) * IN_TILE_BYTES;
   uint8_t* in_base = smem + STAGES * stage_bytes;           // (1024-byte aligned: stage sizes are multiples of 8 KB)
-  uint8_t* stg_base = in_base + N_IN * in_bytes;            // epilogue staging (TN / NN)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + epi_bytes);
+  uint8_t* stg_base = in_base + N_IN * in_bytes;            // epilogue staging
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + EPI_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* in_full = empty_bar + MAX_STAGES;
-  uint64_t* in_empty = in_full + MAX_IN_BUFS;
+  uint64_t* in_full = empty_bar + MAX_STAGES;               // [consumer]: that consumer's tile inputs have landed
+  uint64_t* in_empty = in_full + 2;                         // [buffer]: its consumer is done with it
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
   const int unit = blockIdx.x;                                          // persistent work unit
   const int n_units = gridDim.x;
@@ -397,41 +468,44 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
     if (has_aux) tma_prefetch_desc(&tmX);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CONSUMER_WARPS);
+      mbar_init(&empty_bar[s], 4);            // a stage is read by ONE consumer warpgroup
     }
-    for (int b = 0; b < N_IN; ++b) {
+    for (int b = 0; b < 2; ++b) {
       mbar_init(&in_full[b], 1);
-      mbar_init(&in_empty[b], CONSUMER_WARPS);
+      mbar_init(&in_empty[b], 4);
     }
     fence_mbar_init();
   }
   __syncthreads();
   const int kc_per_tap = (K + BK - 1) / BK;
+  const int n_iters = ntaps * kc_per_tap;                       // the same for every tile
+  const bool in_stage = in_bytes && !N_IN;
+  const int tile_stages = (n_iters + KCH - 1) / KCH + (in_stage ? 1 : 0);   // ring stages one tile takes
   // PDL: barrier init and descriptor prefetch above overlapped the previous kernel's tail; from here on this kernel touches
   // global memory (TMA loads, epilogue loads/stores), so its producers must have completed.
   pdl_wait();
   if (threadIdx.x == 0) dbg_stamp(epi, 1);
 
-  if (warp >= CONSUMER_WARPS) {
-    // ===================== TMA producer =====================
-    // One elected lane owns the barriers and issues the TMA boxes of a stage (KCH chunks x {A boxes, B boxes}).
-    if (warp == CONSUMER_WARPS && lane == 0) {
-      constexpr int A_BOXES = (MODE == 1) ? BM / 64 : 1;
+  if (warp < 4) {
+    // ===================== TMA producer warpgroup =====================
+    setmaxnreg_dec<PP_PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
       constexpr int B_BOXES = (MODE == 0) ? 1 : BN / 64;
       int s = 0;        // smem ring position / phase, carried across tiles
       uint32_t ph = 0;
-      int ib = 0;       // epilogue-input buffer / phase
-      uint32_t iph = 0;
-      // residual / aux boxes of a tile into the next input buffer, or into the next ring stage (N_IN = 0); rows and columns
-      // outside [M, N] arrive as zeros
-      auto load_inputs = [&](const TileInfo& t) {
+      // residual / aux boxes of a tile into its input buffer, or into the next ring stage (N_IN = 0); rows and columns outside
+      // [M, N] arrive as zeros
+      auto load_inputs = [&](int tile) {
+        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, 0);
         uint64_t* bar;
         uint8_t* dst;
         if (N_IN) {
-          mbar_wait(&in_empty[ib], iph ^ 1);
-          bar = &in_full[ib];
-          dst = in_base + ib * in_bytes;
-          if (++ib == N_IN) { ib = 0; iph ^= 1; }
+          const int local = (tile - unit) / n_units;
+          const int b = N_IN == 2 ? (local & 1) : 0;
+          const int uses = N_IN == 2 ? (local >> 1) : local;     // earlier tiles of this buffer
+          mbar_wait(&in_empty[b], (static_cast<uint32_t>(uses) & 1u) ^ 1u);
+          bar = &in_full[local & 1];
+          dst = in_base + b * in_bytes;
         } else {
           mbar_wait(&empty_bar[s], ph ^ 1);
           bar = &full_bar[s];
@@ -449,78 +523,73 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
           for (int j = 0; j < BN / 64; ++j) tma_load_2d(dst + j * IN_BOX_BYTES, &tmX, bar, t.n0 + j * 64, t.m0);
         }
       };
+      int pend = -1;    // tile whose inputs wait for the next tile's operands
       for (int tile = unit; tile < total_tiles; tile += n_units) {
-        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-        // A CTA's first N_IN tiles find their input buffer free: their inputs go out ahead of the operands. Later tiles' inputs
-        // follow their operands, so that the wait for a buffer (the epilogue N_IN tiles back) never holds back operand chunks the
-        // ring has room for; they then travel under the tile's main loop and, with two buffers, the previous tile's epilogue.
-        // In the ring (N_IN = 0) they always take the stage after the tile's operands.
+        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, 0);
+        // A CTA's first N_IN tiles find their input buffer free: their inputs go out ahead of the operands. A later tile's
+        // inputs wait for the buffer (the epilogue N_IN tiles back), so they go out after the NEXT tile's operands: that wait
+        // never holds back operands the ring has room for, and the inputs still land under the tile's own main loop. In the
+        // ring (N_IN = 0) they take the stage after the tile's operands.
         const bool inputs_first = tile < unit + N_IN * n_units;
-        if (in_bytes && inputs_first) load_inputs(t);
-        for (int i = 0; i < t.n_iters; i += KCH) {
-          const int nch = min(KCH, t.n_iters - i);
+        if (in_bytes && N_IN && inputs_first) load_inputs(tile);
+        for (int i = 0; i < n_iters; i += KCH) {
+          const int nch = min(KCH, n_iters - i);
           mbar_wait(&empty_bar[s], ph ^ 1);
           mbar_expect_tx(&full_bar[s], nch * Cfg::STAGE_BYTES);
-          auto load = [&](void* dst, const CUtensorMap* map, int c0, int c1) { tma_load_2d(dst, map, &full_bar[s], c0, c1); };
           // the producer thread is issue-bound: per-chunk index math is done once, box loops are fully unrolled
-          int kit = t.it_begin + i;
-          int tp = 0, kc = kit;
-          if (MODE != 1 && ntaps > 1) { tp = kit / kc_per_tap; kc = kit - tp * kc_per_tap; }
-          for (int ch = 0; ch < nch; ++ch, ++kit) {
+          int tp = 0, kc = i;
+          if (ntaps > 1) { tp = i / kc_per_tap; kc = i - tp * kc_per_tap; }
+          for (int ch = 0; ch < nch; ++ch) {
             uint8_t* sa = smem + s * stage_bytes + ch * Cfg::STAGE_BYTES;
             uint8_t* sb = sa + Cfg::A_BYTES;
-            if (MODE == 1) {
-              int shift = 0;
-              if (ntaps == 9) shift = tap_sign * ((t.tap / 3 - 1) * tap_w + (t.tap % 3 - 1));
-              const int p = kit * BK;
-              if (epi.mn3d) {
-                tma_load_3d(sa, &tmA, &full_bar[s], 0, p, t.m0 >> 6);
-                tma_load_3d(sb, &tmB, &full_bar[s], 0, p + shift, t.nb0 >> 6);
-              } else {
-#pragma unroll
-                for (int j = 0; j < A_BOXES; ++j) load(sa + j * (BK * 128), &tmA, t.m0 + j * 64, p);
-#pragma unroll
-                for (int j = 0; j < B_BOXES; ++j) load(sb + j * (BK * 128), &tmB, t.nb0 + j * 64, p + shift);
-              }
+            int shift = 0;
+            if (ntaps == 9) shift = tap_sign * ((tp / 3 - 1) * tap_w + (tp % 3 - 1));
+            else if (ntaps > 1) shift = tap_sign * tp * tap_w;        // row taps (space-to-depth stem): tap t reads row m + t * tap_w
+            tma_load_2d(sa, &tmA, &full_bar[s], kc * BK, t.m0 + shift);
+            if (MODE == 0) {
+              tma_load_2d(sb, &tmB, &full_bar[s], tp * K + kc * BK, t.nb0);
+            } else if (epi.mn3d) {
+              tma_load_3d(sb, &tmB, &full_bar[s], 0, kc * BK, (tp * N + t.nb0) >> 6);
             } else {
-              int shift = 0;
-              if (ntaps == 9) shift = tap_sign * ((tp / 3 - 1) * tap_w + (tp % 3 - 1));
-              else if (ntaps > 1) shift = tap_sign * tp * tap_w;        // row taps (space-to-depth stem): tap t reads row m + t * tap_w
-              load(sa, &tmA, kc * BK, t.m0 + shift);
-              if (MODE == 0) {
-                load(sb, &tmB, tp * K + kc * BK, t.nb0);
-              } else if (epi.mn3d) {
-                tma_load_3d(sb, &tmB, &full_bar[s], 0, kc * BK, (tp * N + t.nb0) >> 6);
-              } else {
 #pragma unroll
-                for (int j = 0; j < B_BOXES; ++j) load(sb + j * (BK * 128), &tmB, tp * N + t.nb0 + j * 64, kc * BK);
-              }
-              if (++kc == kc_per_tap) { kc = 0; ++tp; }
+              for (int j = 0; j < B_BOXES; ++j) tma_load_2d(sb + j * (BK * 128), &tmB, &full_bar[s], tp * N + t.nb0 + j * 64, kc * BK);
             }
+            if (++kc == kc_per_tap) { kc = 0; ++tp; }
           }
           if (++s == STAGES) { s = 0; ph ^= 1; }
           if (i == 0 && tile == unit) dbg_stamp(epi, 2);
         }
-        if (in_bytes && !inputs_first) load_inputs(t);
+        if (in_stage) load_inputs(tile);
+        if (pend >= 0) load_inputs(pend);
+        pend = (in_bytes && N_IN && !inputs_first) ? tile : -1;
       }
+      if (pend >= 0) load_inputs(pend);
       dbg_stamp(epi, 3);
     }
     return;
   }
 
-  // ===================== consumer warpgroups: wgmma main loop + epilogue =====================
-  const int wg = warp >> 2;                 // rows wg * 64 .. wg * 64 + 63 of the tile
-  const int wrow = wg * 64 + (warp & 3) * 16;   // first of this warp's 16 rows
+  // ===================== consumer warpgroups: wgmma main loop + epilogue, ping-pong over the CTA's tiles =====================
+  setmaxnreg_inc<PP_CONSUMER_REGS>();
+  const int wg = (warp >> 2) - 1;           // consumer 0 / 1: local tiles 0, 2, 4, ... / 1, 3, 5, ...
+  const int wq = warp & 3;                  // rows 16 wq .. 16 wq + 15 of each 64-row half of the tile
   const uint32_t smem0 = smem_u32(smem);
   const uint64_t dseed = epi.drop_thresh ? drop_seed(epi.seed, epi.seed_off) : 0ull;   // after pdl_wait: the word is device data
-  float acc[BN / 2];
+  float acc[2][BN / 2];
+  // ring position / phase: a consumer reads its own tiles' stages and steps over the other consumer's (tile_stages each).
+  // A wait on a stage never runs two phases ahead of it: the turn barrier orders this consumer's main loop after the other's
+  // wait on every stage of the previous tile (its inputs included, see mma_tile_pp).
   int s = 0;
   uint32_t ph = 0;
-  int local = 0;
+  auto ring_skip = [&](int n) {
+    s += n;
+    while (s >= STAGES) { s -= STAGES; ph ^= 1; }
+  };
+  if (wg == 1) ring_skip(tile_stages);
 
-  // TN / NN epilogue: lane (er, eh) handles row er of the warp's 16, columns eh * 16 .. eh * 16 + 15 of each 32-column slice
+  // epilogue: lane (er, eh) handles row er of the warp's 16, columns eh * 16 .. eh * 16 + 15 of each 32-column slice
   const int er = lane & 15, eh = lane >> 4;
-  float* stg = reinterpret_cast<float*>(stg_base) + warp * STG_WARP_FLOATS;
+  float* stg = reinterpret_cast<float*>(stg_base) + (warp - 4) * STG_WARP_FLOATS;
   const bool has_out2 = epi.out2 != nullptr;
   const bool has_shift = epi.shift != nullptr;
   // epilogue kind, fixed for the launch (see the EK_* functions)
@@ -537,133 +606,232 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC)
   const bool kind_relu = epi.act == CB_ACT_RELU;
   const bool guard = (N & 15) != 0;                 // ragged last 16 columns: per-vector column checks in the generic epilogue
 
-  for (int tile = unit; tile < total_tiles; tile += n_units, ++local) {
-    const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 4);
-    mma_tile<BN, MODE == 1, MODE != 0>(acc, smem0, stage_bytes, KCH, STAGES, t.n_iters, wg, lane, s, ph, full_bar, empty_bar);
-    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 5);
+  for (int local = wg, tile = unit + wg * n_units; tile < total_tiles; local += 2, tile += 2 * n_units) {
+    const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, 0);
+    if (local > 0) named_bar_sync(PP_BAR_TURN + wg, 2 * 128);         // the other consumer has issued tile local - 1
+    const int pass = tile + n_units < total_tiles ? PP_BAR_TURN + (wg ^ 1) : 0;
+    mma_tile_pp<BN, MODE != 0>(acc, smem0, stage_bytes, KCH, STAGES, n_iters, lane, s, ph, full_bar, empty_bar, pass, in_stage);
 
-    if (MODE == 1) {
-      wgrad_epilogue<BN>(acc, reinterpret_cast<float*>(epi.out) + static_cast<int64_t>(t.tap) * N, epi.out_ld, epi.scale, M, N,
-                         t.m0 + wrow + (lane >> 2), t.n0, lane);
-      continue;
-    }
-
-    // ---- this lane's row: A-row space m (residual / aux), output row orow (re-mapped), row_ok ----
-    const int m = t.m0 + wrow + er;
-    bool row_ok = m < M;
-    int64_t orow = m;
-    if (epi.rowmap == CB_ROWMAP_PAD) {
-      const int hw = epi.H * epi.W;
-      const int img = m / hw;
-      const int r = m - img * hw;
-      const int y = r / epi.W, x = r - y * epi.W;
-      orow = (static_cast<int64_t>(img) * (epi.H + 2) + y + 1) * (epi.W + 2) + x + 1;
-    } else if (epi.rowmap == CB_ROWMAP_UNPAD) {
-      const int wp = epi.W + 2, hp = epi.H + 2;
-      const int img = m / (hp * wp);
-      const int r = m - img * (hp * wp);
-      const int y = r / wp, x = r - y * wp;
-      row_ok = row_ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
-      orow = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
-    }
-    // this tile's epilogue inputs (residual boxes, then aux boxes): tiles take the N_IN buffers in turn (the producer's order),
-    // or, with N_IN = 0, the ring stage after the tile's operands
-    const int ib = N_IN == 2 ? (local & 1) : 0;
-    const uint32_t in_buf = N_IN ? smem_u32(in_base) + ib * in_bytes : smem0 + s * stage_bytes;
+    // this tile's epilogue inputs (residual boxes, then aux boxes): this consumer's buffer (N_IN = 2), the shared one (N_IN = 1),
+    // or the ring stage after the tile's operands (N_IN = 0)
+    const uint32_t in_buf = N_IN ? smem_u32(in_base) + (N_IN == 2 ? wg : 0) * in_bytes : smem0 + s * stage_bytes;
     if (in_bytes) {
-      if (N_IN) mbar_wait(&in_full[ib], static_cast<uint32_t>(N_IN == 2 ? local >> 1 : local) & 1u);
-      else mbar_wait(&full_bar[s], ph);
+      if (N_IN) mbar_wait_unguarded(&in_full[wg], static_cast<uint32_t>(local >> 1) & 1u);
+      else mbar_wait_unguarded(&full_bar[s], ph);
     }
+    // this lane's row in each 64-row half: A-row space m (residual / aux) -> output row (re-mapped; -1 = not written)
+    int orow_half[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = t.m0 + h * 64 + wq * 16 + er;
+      bool row_ok = m < M;
+      int64_t orow = m;
+      if (epi.rowmap == CB_ROWMAP_PAD) {
+        const int hw = epi.H * epi.W;
+        const int img = m / hw;
+        const int r = m - img * hw;
+        const int y = r / epi.W, x = r - y * epi.W;
+        orow = (static_cast<int64_t>(img) * (epi.H + 2) + y + 1) * (epi.W + 2) + x + 1;
+      } else if (epi.rowmap == CB_ROWMAP_UNPAD) {
+        const int wp = epi.W + 2, hp = epi.H + 2;
+        const int img = m / (hp * wp);
+        const int r = m - img * (hp * wp);
+        const int y = r / wp, x = r - y * wp;
+        row_ok = row_ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
+        orow = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
+      }
+      orow_half[h] = row_ok ? static_cast<int>(orow) : -1;     // (output rows are int: cb_gemm's row counts are)
+    }
+    // per 32-column slice, the staging pass of each half: rows wrow .. wrow + 15 of the tile from accumulator half h
 #pragma unroll
     for (int sc = 0; sc < BN / 32; ++sc) {
-      // fragment -> staging: this warp's 16 rows x 32 columns, then one row segment per lane
-      __syncwarp();
+      // (not unrolled: two interleaved copies of the fused epilogue would not fit the consumer's registers beside the
+      // accumulators; the half is picked per element with a select)
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        const int wrow = h * 64 + wq * 16;
+        // fragment -> staging: this warp's 16 rows x 32 columns, then one row segment per lane
+        __syncwarp();
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int j = sc * 4 + jj;
-        float* p = stg + (lane >> 2) * STG_PITCH + jj * 8 + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(p + 8 * STG_PITCH) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
-      __syncwarp();
-      const int nb = t.n0 + sc * 32 + eh * 16;        // global column of f[0]
-      if (!row_ok || nb >= N) continue;
-      constexpr int NC = 16;
-      float f[NC];
-      const uint32_t srow = smem_u32(stg + er * STG_PITCH + eh * 16);
-#pragma unroll
-      for (int j = 0; j < NC / 4; ++j) {
-        const uint4 u = lds128(srow + j * 16);
-        f[4 * j] = __uint_as_float(u.x); f[4 * j + 1] = __uint_as_float(u.y);
-        f[4 * j + 2] = __uint_as_float(u.z); f[4 * j + 3] = __uint_as_float(u.w);
-      }
-      // residual / aux of these 16 columns: box (column / 64), 16-byte chunks q, q + 1 of row wrow + er (zeros beyond N)
-      uint32_t res16[NC / 2], aux16[NC / 2];
-      const int tc = sc * 32 + eh * 16;               // tile column of f[0]
-      const int q = (tc & 63) >> 3;
-      if (has_res) {
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const uint4 u = lds128(swz128(in_buf + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
-          res16[4 * j] = u.x; res16[4 * j + 1] = u.y; res16[4 * j + 2] = u.z; res16[4 * j + 3] = u.w;
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = sc * 4 + jj;
+          float* p = stg + (lane >> 2) * STG_PITCH + jj * 8 + 2 * (lane & 3);
+          const bool h1 = h != 0;
+          *reinterpret_cast<float2*>(p) = make_float2(h1 ? acc[1][4 * j] : acc[0][4 * j], h1 ? acc[1][4 * j + 1] : acc[0][4 * j + 1]);
+          *reinterpret_cast<float2*>(p + 8 * STG_PITCH) =
+              make_float2(h1 ? acc[1][4 * j + 2] : acc[0][4 * j + 2], h1 ? acc[1][4 * j + 3] : acc[0][4 * j + 3]);
         }
-      }
-      if (has_aux) {
+        __syncwarp();
+        const int nb = t.n0 + sc * 32 + eh * 16;        // global column of f[0]
+        const int64_t orow = h ? orow_half[1] : orow_half[0];
+        if (orow < 0 || nb >= N) continue;
+        constexpr int NC = 16;
+        float f[NC];
+        const uint32_t srow = smem_u32(stg + er * STG_PITCH + eh * 16);
 #pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const uint4 u = lds128(swz128(in_buf + (has_res ? IN_TILE_BYTES : 0) + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
-          aux16[4 * j] = u.x; aux16[4 * j + 1] = u.y; aux16[4 * j + 2] = u.z; aux16[4 * j + 3] = u.w;
+        for (int j = 0; j < NC / 4; ++j) {
+          const uint4 u = lds128(srow + j * 16);
+          f[4 * j] = __uint_as_float(u.x); f[4 * j + 1] = __uint_as_float(u.y);
+          f[4 * j + 2] = __uint_as_float(u.z); f[4 * j + 3] = __uint_as_float(u.w);
         }
-      }
-      float shv[NC];                                  // shift (bias / FrozenBN shift) of these columns
-      if (has_shift) {
+        // residual / aux of these 16 columns: box (column / 64), 16-byte chunks q, q + 1 of row wrow + er (zeros beyond N)
+        uint32_t res16[NC / 2], aux16[NC / 2];
+        const int tc = sc * 32 + eh * 16;               // tile column of f[0]
+        const int q = (tc & 63) >> 3;
+        if (has_res) {
 #pragma unroll
-        for (int j = 0; j < NC; j += 4) {
-          float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (nb + j + 4 <= N) s4 = __ldg(reinterpret_cast<const float4*>(epi.shift + nb + j));
-          shv[j] = s4.x; shv[j + 1] = s4.y; shv[j + 2] = s4.z; shv[j + 3] = s4.w;
+          for (int j = 0; j < 2; ++j) {
+            const uint4 u = lds128(swz128(in_buf + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
+            res16[4 * j] = u.x; res16[4 * j + 1] = u.y; res16[4 * j + 2] = u.z; res16[4 * j + 3] = u.w;
+          }
         }
-      }
-      uint32_t o2_16[NC / 2];
-      switch (kind) {
-        case EK_SHIFT_ACT: epilogue_shift_act<NC>(f, shv, has_shift, res16, has_res, kind_relu); break;
-        case EK_RELU_MASK: epilogue_relu_mask<NC>(f, res16, has_res, aux16); break;
-        case EK_DROP_RES:
-          epilogue_drop_res<NC>(f, shv, has_shift, res16, has_res, dseed, static_cast<uint64_t>(orow) * static_cast<uint64_t>(N) + nb, epi.drop_thresh,
-                                epi.drop_inv_keep);
-          break;
-        case EK_GELU_STASH: epilogue_gelu_stash<NC>(f, shv, has_shift, o2_16); break;
-        case EK_AUX_MUL: epilogue_aux_mul<NC>(f, res16, has_res, aux16); break;
-        default:
-          if (guard) epilogue_math<NC, true>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
-          else epilogue_math<NC, false>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
-      }
-      if (epi.out_fp32) {
-        float* o = reinterpret_cast<float*>(epi.out) + orow * epi.out_ld + nb;
+        if (has_aux) {
 #pragma unroll
-        for (int j = 0; j < NC; j += 4)
-          if (nb + j + 4 <= N) *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-      } else {
-        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(epi.out) + orow * epi.out_ld + nb;
+          for (int j = 0; j < 2; ++j) {
+            const uint4 u = lds128(swz128(in_buf + (has_res ? IN_TILE_BYTES : 0) + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
+            aux16[4 * j] = u.x; aux16[4 * j + 1] = u.y; aux16[4 * j + 2] = u.z; aux16[4 * j + 3] = u.w;
+          }
+        }
+        float shv[NC];                                  // shift (bias / FrozenBN shift) of these columns
+        if (has_shift) {
 #pragma unroll
-        for (int j = 0; j < 2; ++j)
-          if (nb + 8 * j + 8 <= N)
-            *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                                                              pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
-      }
-      if (has_out2) {
-        __nv_bfloat16* o = epi.out2 + orow * epi.out2_ld + nb;
+          for (int j = 0; j < NC; j += 4) {
+            float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (nb + j + 4 <= N) s4 = __ldg(reinterpret_cast<const float4*>(epi.shift + nb + j));
+            shv[j] = s4.x; shv[j + 1] = s4.y; shv[j + 2] = s4.z; shv[j + 3] = s4.w;
+          }
+        }
+        uint32_t o2_16[NC / 2];
+        switch (kind) {
+          case EK_SHIFT_ACT: epilogue_shift_act<NC>(f, shv, has_shift, res16, has_res, kind_relu); break;
+          case EK_RELU_MASK: epilogue_relu_mask<NC>(f, res16, has_res, aux16); break;
+          case EK_DROP_RES:
+            epilogue_drop_res<NC>(f, shv, has_shift, res16, has_res, dseed, static_cast<uint64_t>(orow) * static_cast<uint64_t>(N) + nb,
+                                  epi.drop_thresh, epi.drop_inv_keep);
+            break;
+          case EK_GELU_STASH: epilogue_gelu_stash<NC>(f, shv, has_shift, o2_16); break;
+          case EK_AUX_MUL: epilogue_aux_mul<NC>(f, res16, has_res, aux16); break;
+          default:
+            if (guard) epilogue_math<NC, true>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
+            else epilogue_math<NC, false>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
+        }
+        if (epi.out_fp32) {
+          float* o = reinterpret_cast<float*>(epi.out) + orow * epi.out_ld + nb;
 #pragma unroll
-        for (int j = 0; j < 2; ++j)
-          if (nb + 8 * j + 8 <= N) *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(o2_16[4 * j], o2_16[4 * j + 1], o2_16[4 * j + 2], o2_16[4 * j + 3]);
+          for (int j = 0; j < NC; j += 4)
+            if (nb + j + 4 <= N) *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+        } else {
+          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(epi.out) + orow * epi.out_ld + nb;
+#pragma unroll
+          for (int j = 0; j < 2; ++j)
+            if (nb + 8 * j + 8 <= N)
+              *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
+                                                                pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
+        }
+        if (has_out2) {
+          __nv_bfloat16* o = epi.out2 + orow * epi.out2_ld + nb;
+#pragma unroll
+          for (int j = 0; j < 2; ++j)
+            if (nb + 8 * j + 8 <= N) *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(o2_16[4 * j], o2_16[4 * j + 1], o2_16[4 * j + 2], o2_16[4 * j + 3]);
+        }
       }
     }
     if (in_bytes) {                                 // this warp is done with the tile's inputs: hand the buffer / stage back
       __syncwarp();
-      if (lane == 0) mbar_arrive(N_IN ? &in_empty[ib] : &empty_bar[s]);
+      if (lane == 0) mbar_arrive(N_IN ? &in_empty[N_IN == 2 ? wg : 0] : &empty_bar[s]);
       if (!N_IN && ++s == STAGES) { s = 0; ph ^= 1; }
     }
+    ring_skip(tile_stages);                         // past the other consumer's next tile
+  }
+  if (threadIdx.x == 4 * 32) dbg_stamp(epi, 11);
+}
+
+// ===================================== WGRAD =====================================
+template <int BN, int OCC>
+__global__ void __launch_bounds__(GEMM_THREADS, OCC)
+    gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K, int ntaps, int tap_w,
+                int tap_sign, int iters_per_split, int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, GemmEpi epi) {
+  using Cfg = GemmCfg<BN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  const int stage_bytes = KCH * Cfg::STAGE_BYTES;           // a stage holds KCH consecutive 64-deep k-chunks (one barrier round trip)
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
+  uint64_t* empty_bar = full_bar + MAX_STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int unit = blockIdx.x;                                          // persistent work unit
+  const int n_units = gridDim.x;
+  if (threadIdx.x == 0) dbg_stamp(epi, 0);   // (debug-only buffer, not produced by any kernel: safe before pdl_wait)
+  pdl_trigger();   // PDL: let the next kernel's CTAs take this SM as soon as this CTA leaves it
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], CONSUMER_WARPS);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  // PDL: barrier init and descriptor prefetch above overlapped the previous kernel's tail; from here on this kernel touches
+  // global memory, so its producers must have completed.
+  pdl_wait();
+  if (threadIdx.x == 0) dbg_stamp(epi, 1);
+
+  if (warp >= CONSUMER_WARPS) {
+    // ===================== TMA producer =====================
+    // One elected lane owns the barriers and issues the TMA boxes of a stage (KCH chunks x {A boxes, B boxes}).
+    if (warp == CONSUMER_WARPS && lane == 0) {
+      int s = 0;        // smem ring position / phase, carried across tiles
+      uint32_t ph = 0;
+      for (int tile = unit; tile < total_tiles; tile += n_units) {
+        const TileInfo t = decode_tile<BN, 1>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
+        int shift = 0;
+        if (ntaps == 9) shift = tap_sign * ((t.tap / 3 - 1) * tap_w + (t.tap % 3 - 1));
+        for (int i = 0; i < t.n_iters; i += KCH) {
+          const int nch = min(KCH, t.n_iters - i);
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          mbar_expect_tx(&full_bar[s], nch * Cfg::STAGE_BYTES);
+          int kit = t.it_begin + i;
+          for (int ch = 0; ch < nch; ++ch, ++kit) {
+            uint8_t* sa = smem + s * stage_bytes + ch * Cfg::STAGE_BYTES;
+            uint8_t* sb = sa + Cfg::A_BYTES;
+            const int p = kit * BK;
+            if (epi.mn3d) {
+              tma_load_3d(sa, &tmA, &full_bar[s], 0, p, t.m0 >> 6);
+              tma_load_3d(sb, &tmB, &full_bar[s], 0, p + shift, t.nb0 >> 6);
+            } else {
+#pragma unroll
+              for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), &tmA, &full_bar[s], t.m0 + j * 64, p);
+#pragma unroll
+              for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), &tmB, &full_bar[s], t.nb0 + j * 64, p + shift);
+            }
+          }
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+          if (i == 0 && tile == unit) dbg_stamp(epi, 2);
+        }
+      }
+      dbg_stamp(epi, 3);
+    }
+    return;
+  }
+
+  // ===================== consumer warpgroups: wgmma main loop + red.add epilogue =====================
+  const int wg = warp >> 2;                 // rows wg * 64 .. wg * 64 + 63 of the tile
+  const int wrow = wg * 64 + (warp & 3) * 16;   // first of this warp's 16 rows
+  const uint32_t smem0 = smem_u32(smem);
+  float acc[BN / 2];
+  int s = 0;
+  uint32_t ph = 0;
+  int local = 0;
+  for (int tile = unit; tile < total_tiles; tile += n_units, ++local) {
+    const TileInfo t = decode_tile<BN, 1>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
+    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 4);
+    mma_tile<BN, 1, 1>(acc, smem0, stage_bytes, KCH, STAGES, t.n_iters, wg, lane, s, ph, full_bar, empty_bar);
+    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 5);
+    wgrad_epilogue<BN>(acc, reinterpret_cast<float*>(epi.out) + static_cast<int64_t>(t.tap) * N, epi.out_ld, epi.scale, M, N,
+                       t.m0 + wrow + (lane >> 2), t.n0, lane);
     if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 8);
   }
   if (threadIdx.x == 0) dbg_stamp(epi, 11);
@@ -688,16 +856,20 @@ static long long* g_gemm_timeline = nullptr;
 static int g_force_kch = 0;   // tuning hook: chunks per stage (0 = automatic)
 static int g_mn3d = 1;        // 1 (default) = MN-major operands through one 3-D TMA box per k-chunk (GemmEpi::mn3d); cb_debug_gemm_mn3d
 
+
 // Shared-memory plan of one launch: the epilogue staging (TN / NN: 16 x 32 fp32 per consumer warp; WGRAD: none), n_in
 // epilogue-input buffers of in_bytes (the residual / aux boxes of one tile), then as many 64-deep operand chunks as fit, grouped
 // KCH per stage. Every stage costs one full / empty barrier round trip whatever its size, so deep stages are preferred to many
-// shallow ones. No ring is deeper than the K loop plus one stage: letting the producer of a persistent CTA run several one-chunk
-// tiles ahead measured slower on the plain K = 64 convolutions (H100 SXM, 400 W: 401408 x 256 x 64 +9 %, 401408 x 64 x 64 +17 %).
-// Epilogue inputs (residual / aux boxes of one tile, in_bytes): two dedicated buffers let the next tile's inputs load under this
-// tile's epilogue; they are taken when the ring beside them still holds a whole tile's K loop (the short K loops of the
-// HBM-bound 1x1 convs). A K loop of at most 4 chunks that cannot have both gets one buffer. A longer K loop keeps the ring it
-// has without inputs and lands its inputs in the ring stage after its operands (n_in = 0; needs in_bytes <= one stage): they load
-// under the end of its main loop, and the buffer does not cost the compute-bound main loop ring depth.
+// shallow ones. Ring depth cap:
+//   WGRAD (one tile at a time): the K loop plus one stage.
+//   TN / NN (ping-pong): both consumers' current tiles plus one stage, so that the producer has the next tile's first stage
+//   in flight while the two tiles in hand are multiplied and the other consumer's epilogue runs. For the one-chunk 1x1 convs
+//   that is three stages.
+// Epilogue inputs (residual / aux boxes of one tile, in_bytes): two dedicated buffers, one per consumer, let a tile's inputs
+// load under the other consumer's epilogue; they are taken when the ring beside them still holds a whole tile's K loop (the
+// short K loops of the HBM-bound 1x1 convs). A K loop of at most 4 chunks that cannot have both gets one buffer. A longer K loop
+// keeps the ring it has without inputs and lands its inputs in the ring stage after its operands (n_in = 0; needs in_bytes <=
+// one stage): they load under the end of its main loop, and the buffer does not cost the compute-bound main loop ring depth.
 struct SmemPlan {
   int epi_bytes, kch, stages, chunk_bytes, n_in;
 };
@@ -718,7 +890,8 @@ static SmemPlan plan_ring(int bn, bool staging, int kiters, int force_kch, int o
   p.stages = chunks_fit / p.kch;
   if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
   const int stage_iters = ceil_div(kiters, p.kch);
-  if (p.stages > stage_iters + 1) p.stages = stage_iters + 1 > 2 ? stage_iters + 1 : 2;   // no ring deeper than the K loop
+  const int cap = staging ? 2 * stage_iters + 1 : (stage_iters + 1 > 2 ? stage_iters + 1 : 2);
+  if (p.stages > cap) p.stages = cap;
   return p;
 }
 static SmemPlan plan_smem(int bn, bool staging, int kiters, int force_kch = 0, int occ = 1, int in_bytes = 0) {
@@ -734,13 +907,18 @@ static int epi_in_bytes(const cb_gemm_desc& d, int bn) {
   return d.mode == CB_GEMM_WGRAD ? 0 : ((d.residual != nullptr) + (d.aux != nullptr)) * (bn / 64) * IN_BOX_BYTES;
 }
 
+// MODE 0 / 2 (TN / NN): gemm_pingpong_kernel, one CTA per SM, BN = 64 / 128. MODE 1 (WGRAD): gemm_kernel, OCC CTAs per SM.
 template <int BN, int MODE, int OCC = 1>
 static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_t stream) {
+  static_assert(MODE == 1 || (OCC == 1 && BN <= 128), "TN / NN: one CTA per SM, 128 x 64 or 128 x 128 tiles");
   GemmEpi epi = epi_in;
   using Cfg = GemmCfg<BN>;
   constexpr int LIMIT = OCC == 2 ? SMEM_LIMIT_OCC2 : SMEM_LIMIT;
   static bool attr_set = false;
-  auto kern = gemm_kernel<BN, MODE, OCC>;
+  auto kern = [] {
+    if constexpr (MODE == 1) return gemm_kernel<BN, OCC>;
+    else return gemm_pingpong_kernel<BN, MODE>;
+  }();
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LIMIT);
     if (e == cudaSuccess && OCC == 2)   // both CTAs of an SM need their 113 KB: ask for the full shared-memory carve-out
@@ -793,30 +971,37 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
   const int grid = total < units ? total : units;
   const int in_bytes = epi_in_bytes(d, BN);
   const SmemPlan sp = plan_smem(BN, MODE != 1, kiters, (d.reserved >> 8) & 15, OCC, in_bytes);
-  const int epi_bytes = sp.epi_bytes, kch = sp.kch, stages = sp.stages;
+  const int kch = sp.kch, stages = sp.stages;
   if (stages < 2) {
-    set_error("cb_gemm: not enough shared memory for a 2-stage pipeline (BN=%d, epilogue %d B + inputs %d B, %d CTA(s) per SM)", BN, epi_bytes,
-              in_bytes, OCC);
+    set_error("cb_gemm: not enough shared memory for a 2-stage pipeline (BN=%d, epilogue %d B + inputs %d B, %d CTA(s) per SM)", BN,
+              sp.epi_bytes, in_bytes, OCC);
     return CB_ERR_INVALID;
   }
-  const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + sp.n_in * in_bytes + epi_bytes + Cfg::BAR_BYTES + 1024;
-  launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, iters_per_split,
-                tiles_m, tiles_n, total, stages, kch, sp.n_in, epi_bytes, epi);
+  const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + sp.n_in * in_bytes + sp.epi_bytes + Cfg::BAR_BYTES + 1024;
+  if constexpr (MODE == 1)
+    launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, iters_per_split,
+                  tiles_m, tiles_n, total, stages, kch, epi);
+  else
+    launch_gemm_k(kern, grid, PP_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, tiles_m,
+                  tiles_n, total, stages, kch, sp.n_in, epi);
   return check_launch("cb_gemm");
 }
 
 // ------------------------------------------------------------------------------------------------
 // Launch configuration: an analytic model picks the tile width (and the wgrad K-split). A persistent CTA's main loop costs about
 // (k-iterations x stage bytes) / (operand ingest rate) plus a barrier round trip per stage, and the launch is done when the
-// busiest SM is; a per-tile epilogue term is added.
+// busiest SM is; a per-tile epilogue term is added. In the TN / NN ping-pong kernel a tile's epilogue overlaps the next tile's
+// main loop and the other consumer's epilogue: a tile costs max(main loop, (main loop + epilogue) / 2), plus the last
+// epilogue's exposed half.
 // ------------------------------------------------------------------------------------------------
 struct LaunchCfg {
   int bn, splits;
 };
 
-// Two CTAs per SM (the OCC = 2 instantiations: 128 x 64 tiles, <= 113 KB of shared memory and <= 96 registers per thread
-// each). One CTA's epilogue runs under the other's main loop. g_occ2_mode: 0 = never, 1 = only launches that ask for it
-// (cb_gemm_desc.reserved bit 5), 2 = every eligible launch whose work is at most g_occ2_max_gflop (0 = no limit).
+// Two CTAs per SM for the weight gradients (the WGRAD OCC = 2 instantiations: 128 x 64 tiles, <= 113 KB of shared memory and
+// <= 96 registers per thread each). One CTA's epilogue runs under the other's main loop. g_occ2_mode: 0 = never, 1 = only
+// launches that ask for it (cb_gemm_desc.reserved bit 5), 2 = every eligible launch whose work is at most g_occ2_max_gflop
+// (0 = no limit). TN / NN launches always run the ping-pong kernel.
 static int g_occ2_mode = 1;
 static double g_occ2_max_gflop = 0.0;
 
@@ -824,14 +1009,17 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, int occ = 1) {
   const int units = sm_count() * occ;
   const int kc = ceil_div(d.k, BK);
   const bool wgrad = d.mode == CB_GEMM_WGRAD;
+  // TN / NN: 128 x 256 would need 256 fp32 accumulators per consumer thread, more than its 232 registers; an explicit
+  // block_n = 256 runs on 128-wide tiles
+  const int block_n = (!wgrad && d.block_n == 256) ? 128 : d.block_n;
   static const int cand[3] = {64, 128, 256};
   LaunchCfg best = {0, 1};      // bn = 0: no candidate fits (only possible with occ = 2)
   double best_cost = 1e30;
   for (int c = 0; c < 3; ++c) {
     const int bn = cand[c];
     if (occ == 2 && bn > 64) continue;
-    if (d.block_n && bn != d.block_n) continue;
-    if (!d.block_n && !wgrad && bn == 256) continue;      // see GEMM_THREADS
+    if (block_n && bn != block_n) continue;
+    if (!wgrad && bn == 256) continue;
     if (bn > 64 && d.n <= bn / 2) continue;               // mostly padding
     const int64_t base = static_cast<int64_t>(ceil_div(d.m, BM)) * ceil_div(d.n, bn) * (wgrad ? d.ntaps : 1);
     const int max_split = wgrad ? (d.split_k > 0 ? d.split_k : (kc < 32 ? kc : 32)) : 1;
@@ -847,8 +1035,15 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, int occ = 1) {
       const double shallow = (pl.stages * pl.kch < 3 && ips > 2) ? 3.0 : 1.0;
       // per stage: ~450-cycle barrier round trip + bytes at ~60 B/clk (shared by the CTAs of an SM); per tile: epilogue
       const double stage_cost = 450.0 + pl.kch * pl.chunk_bytes / (60.0 / occ);
-      const double epi = wgrad ? bn * 24.0 : bn * 30.0;
-      const double cost = rounds * (ceil_div(ips, pl.kch) * stage_cost * shallow + epi) + 2500.0;
+      const double main_loop = ceil_div(ips, pl.kch) * stage_cost * shallow;
+      double cost;
+      if (wgrad) {
+        cost = rounds * (main_loop + bn * 24.0) + 2500.0;
+      } else {
+        const double epi = bn * 30.0;
+        const double per_tile = main_loop > 0.5 * (main_loop + epi) ? main_loop : 0.5 * (main_loop + epi);
+        cost = rounds * per_tile + 0.5 * epi + 2500.0;
+      }
       if (cost < best_cost) {
         best_cost = cost;
         best = {bn, real_sp};
@@ -865,7 +1060,7 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, int occ = 1) {
 // length (tokens / pixels), so their tiles cost the same and the static round-robin schedule stays balanced; what the group buys
 // is one prologue + one tail instead of four, tiles of all problems filling the SMs together, and - because four problems
 // together have enough tiles - no K-split, i.e. half the fp32 red.global traffic of the single launches. Same warp roles, ring
-// and red.add epilogue as gemm_kernel<BN, MODE 1>; the problem descriptors (tensor maps included) travel in the kernel's
+// and red.add epilogue as gemm_kernel<BN, 1>; the problem descriptors (tensor maps included) travel in the kernel's
 // parameter space.
 // ------------------------------------------------------------------------------------------------
 constexpr int WG_MAX_PROBLEMS = 8;
@@ -1102,16 +1297,13 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
     CB_REQUIRE(!(d.out2 && d.out_fp32), "cb_gemm(TN): out2 requires a bf16 primary output");
     CB_REQUIRE(d.rowmap == CB_ROWMAP_NONE || (d.map_h > 0 && d.map_w > 0), "cb_gemm: rowmap needs map_h/map_w");
     CB_REQUIRE(d.ntaps == 1 || d.tap_w > 2, "cb_gemm: tap modes need tap_w (padded row pitch in pixels)");
-    if (want_occ2) {
-      const LaunchCfg l2 = choose_config(d, 2);
-      if (l2.bn == 64) return nn ? launch_gemm<64, 2, 2>(d, epi, stream) : launch_gemm<64, 0, 2>(d, epi, stream);
-    }
+    CB_REQUIRE(d.block_n == 0 || d.block_n == 64 || d.block_n == 128 || d.block_n == 256, "cb_gemm: block_n must be 0, 64, 128 or 256 (got %d)",
+               d.block_n);
     const LaunchCfg lc = choose_config(d);
     switch (lc.bn) {
       case 64: return nn ? launch_gemm<64, 2>(d, epi, stream) : launch_gemm<64, 0>(d, epi, stream);
       case 128: return nn ? launch_gemm<128, 2>(d, epi, stream) : launch_gemm<128, 0>(d, epi, stream);
-      case 256: return nn ? launch_gemm<256, 2>(d, epi, stream) : launch_gemm<256, 0>(d, epi, stream);
-      default: CB_REQUIRE(false, "cb_gemm: block_n must be 0, 64, 128 or 256 (got %d)", lc.bn);
+      default: CB_REQUIRE(false, "cb_gemm: no tile width for block_n %d", d.block_n);
     }
   } else {
     CB_REQUIRE(d.out_fp32 == 1, "cb_gemm(WGRAD): output must be fp32");

@@ -119,8 +119,10 @@ def set_mn3d(on):
 
 
 def set_occ2(mode, max_gflop=0.0):
-    """Two GEMM CTAs per SM (128 x <=128 tiles, 8 epilogue warps, <= 113 KB smem each): 0 = never, 1 = only launches that ask
-    for it (tuning table / reserved bit 5), 2 = every eligible launch of at most ``max_gflop`` GFLOP (0 = no limit)."""
+    """Two weight-gradient GEMM CTAs per SM (128 x 64 tiles, <= 113 KB smem each): 0 = never, 1 = only launches that ask for it
+    (tuning table / reserved bit 5), 2 = every eligible launch of at most ``max_gflop`` GFLOP (0 = no limit). TN / NN launches
+    always run the one-CTA-per-SM ping-pong kernel, whose two consumer warpgroups already overlap one tile's epilogue with the
+    next tile's main loop."""
     f = L.lib().cb_debug_gemm_occ2
     f.argtypes = [ctypes.c_int, ctypes.c_double]
     f.restype = None

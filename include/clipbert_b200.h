@@ -137,12 +137,12 @@ typedef struct cb_gemm_desc {
   int32_t rowmap, map_h, map_w; /* spatial size (unpadded) for cb_rowmap */
   float dropout_p;
   uint64_t dropout_seed;
-  int32_t block_n;  /* 0 = let the library choose (64 / 128; 256 for CB_GEMM_WGRAD). An explicit 256 for TN / NN runs correctly
-                       but is slow on sm_90a: nine warps per CTA cap a thread at 168 registers and the 128 x 256 fused
-                       epilogue spills at that budget; with both residual and aux its input tiles do not fit beside a
-                       2-stage ring, and the launch runs on 64-wide tiles */
-  int32_t reserved; /* tuning / test knobs: bit5 ask for / bit6 forbid the two-CTAs-per-SM instantiation (128 x 64
-                       tiles), bits 8-11 k-chunks per pipeline stage (0 = automatic); other bits ignored */
+  int32_t block_n;  /* 0 = let the library choose (64 / 128; 256 for CB_GEMM_WGRAD). TN / NN run 128 x 64 or 128 x 128 tiles:
+                       a 128 x 256 tile would need 256 fp32 accumulators per thread of the warpgroup that owns it, more
+                       than its 232 registers, so an explicit 256 for TN / NN runs on 128-wide tiles */
+  int32_t reserved; /* tuning / test knobs: bit5 ask for / bit6 forbid the two-CTAs-per-SM weight-gradient instantiation
+                       (128 x 64 tiles; CB_GEMM_WGRAD only), bits 8-11 k-chunks per pipeline stage (0 = automatic); other
+                       bits ignored */
 } cb_gemm_desc;
 
 int cb_gemm(const cb_gemm_desc* desc, void* stream);
