@@ -860,7 +860,7 @@ static int g_mn3d = 1;        // 1 (default) = MN-major operands through one 3-D
 // Shared-memory plan of one launch: the epilogue staging (TN / NN: 16 x 32 fp32 per consumer warp; WGRAD: none), n_in
 // epilogue-input buffers of in_bytes (the residual / aux boxes of one tile), then as many 64-deep operand chunks as fit, grouped
 // KCH per stage. Every stage costs one full / empty barrier round trip whatever its size, so deep stages are preferred to many
-// shallow ones. Ring depth cap:
+// shallow ones, except that a K loop longer than the ring keeps at least three stages. Ring depth cap:
 //   WGRAD (one tile at a time): the K loop plus one stage.
 //   TN / NN (ping-pong): both consumers' current tiles plus one stage, so that the producer has the next tile's first stage
 //   in flight while the two tiles in hand are multiplied and the other consumer's epilogue runs. For the one-chunk 1x1 convs
@@ -880,11 +880,16 @@ static SmemPlan plan_ring(int bn, bool staging, int kiters, int force_kch, int o
   p.epi_bytes = staging ? EPI_BYTES : 0;
   p.n_in = n_in;
   const int chunks_fit = (limit - 1024 - GemmCfg<64>::BAR_BYTES - p.epi_bytes - n_in * in_bytes) / p.chunk_bytes;
+  // K loop longer than the ring: the ring cycles within a tile, and the stage count, not the stage size, sets how far the
+  // producer runs ahead. A stage depth is only taken if it leaves at least three stages (TN / NN 64-wide: four stages of two
+  // instead of two of four; WGRAD 128 x 256: four one-chunk stages instead of two of two). H100, 128 x 64 TN / NN tiles, 9-tap
+  // convs: two stages of four chunks ran 1.4-1.8 x slower than four stages of two.
+  const int min_stages = kiters > chunks_fit ? 3 : 2;
   p.kch = 1;
   if (force_kch > 0) p.kch = force_kch;
   else if (g_force_kch > 0) p.kch = g_force_kch;
-  else if (kiters >= 4 && chunks_fit >= 8) p.kch = 4;
-  else if (kiters >= 2 && chunks_fit >= 4) p.kch = 2;
+  else if (kiters >= 4 && chunks_fit >= 4 * min_stages) p.kch = 4;
+  else if (kiters >= 2 && chunks_fit >= 2 * min_stages) p.kch = 2;
   if (p.kch > kiters) p.kch = kiters;
   if (p.kch > 1 && chunks_fit / p.kch < 2) p.kch = 1;
   p.stages = chunks_fit / p.kch;
