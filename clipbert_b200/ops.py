@@ -119,10 +119,9 @@ def set_mn3d(on):
 
 
 def set_occ2(mode, max_gflop=0.0):
-    """Two weight-gradient GEMM CTAs per SM (128 x 64 tiles, <= 113 KB smem each): 0 = never, 1 = only launches that ask for it
-    (tuning table / reserved bit 5), 2 = every eligible launch of at most ``max_gflop`` GFLOP (0 = no limit). TN / NN launches
-    always run the one-CTA-per-SM ping-pong kernel, whose two consumer warpgroups already overlap one tile's epilogue with the
-    next tile's main loop."""
+    """Accepted for compatibility and ignored: every GEMM runs one CTA per SM. Weight gradients used to have a two-CTAs-per-SM
+    instantiation (128 x 64 tiles); once their wgmma were pipelined it was slower than one CTA per SM on every weight-gradient
+    shape of the training step, and it was removed."""
     f = L.lib().cb_debug_gemm_occ2
     f.argtypes = [ctypes.c_int, ctypes.c_double]
     f.restype = None

@@ -140,16 +140,15 @@ typedef struct cb_gemm_desc {
   int32_t block_n;  /* 0 = let the library choose (64 / 128; 256 for CB_GEMM_WGRAD). TN / NN run 128 x 64 or 128 x 128 tiles:
                        a 128 x 256 tile would need 256 fp32 accumulators per thread of the warpgroup that owns it, more
                        than its 232 registers, so an explicit 256 for TN / NN runs on 128-wide tiles */
-  int32_t reserved; /* tuning / test knobs: bit5 ask for / bit6 forbid the two-CTAs-per-SM weight-gradient instantiation
-                       (128 x 64 tiles; CB_GEMM_WGRAD only), bits 8-11 k-chunks per pipeline stage (0 = automatic); other
-                       bits ignored */
+  int32_t reserved; /* tuning / test knobs: bits 8-11 k-chunks per pipeline stage (0 = automatic); other bits ignored */
 } cb_gemm_desc;
 
 int cb_gemm(const cb_gemm_desc* desc, void* stream);
 /* n independent CB_GEMM_WGRAD problems in ONE persistent launch: the weight gradients of the four Linear layers of a BertLayer
  * (autograd of transformers.py:238-301,363-381) or of the convs of one bottleneck block. The problems should share their
  * reduction length k (tokens / pixels); 1 <= n <= 8. One prologue and tail instead of n, no K-split when the group fills the SMs.
- * Falls back to n cb_gemm launches for n == 1, n > 8 or very different k. Epilogue fields other than scale / out are ignored. */
+ * Falls back to n cb_gemm launches for n == 1, n > 8 or very different k. descs[0].block_n / split_k, when non-zero, set the tile
+ * width / K-split of the whole group. Other epilogue fields than scale / out are ignored. */
 int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* stream);
 
 /* ------------------------------------------------------------------------------------------
