@@ -6,6 +6,11 @@
 // Sequences on this path are short (L = Lt + 9 .. 521), head_dim is 64, and attention is < 1 % of
 // the layer FLOPs at L = 41, so the kernel is a 64x64-tiled online-softmax CUDA-core kernel that
 // packs a whole (sequence, head) into one or a few CTAs; it is latency- not FLOP-bound.
+//
+// By default every length runs on the tensor-core kernels of attention_tc.cu (L <= 64: one CTA per
+// (sequence, head); longer: the flash forward and the two-kernel backward). The CUDA-core kernels
+// here are the general path that cb_debug_attention_general(1) selects, and the reference the
+// tensor-core kernels are tested against.
 #include "common.cuh"
 #include "host_util.h"
 
@@ -407,6 +412,9 @@ int attention_tc_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, 
                      cudaStream_t stream);
 int attention_tc_fwd_flash(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, void* ctx, int64_t ld_ctx, float* lse, int nseq, int l,
                            int lt, int heads, float dropout_p, uint64_t seed, cudaStream_t stream);
+int attention_tc_bwd_long(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const void* ctx, const void* dctx, int64_t ld_ctx,
+                          const float* lse, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, float dropout_p, uint64_t seed,
+                          cudaStream_t stream);
 void attention_tc_set_flash_pipe(int on);   // 1 (default): cp.async double-buffered key tiles in the long-sequence forward
 void attention_tc_set_rows48(int on);   // 1 (default): sequences of up to 48 tokens on the 48-row / three-warp kernels
 int g_attention_force_general = 0;   // test knob: 1 = always use the general (any L) kernels
@@ -460,6 +468,9 @@ int cb_attention_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, 
   if (l <= 64 && !g_attention_force_general)
     return attention_tc_bwd(qkv, ld_qkv, text_mask, ctx, dctx, ld_ctx, lse, dqkv, ld_dqkv, nseq, l, lt, heads, dropout_p, seed,
                             static_cast<cudaStream_t>(stream));
+  if (l > 64 && !g_attention_force_general)
+    return attention_tc_bwd_long(qkv, ld_qkv, text_mask, ctx, dctx, ld_ctx, lse, dqkv, ld_dqkv, nseq, l, lt, heads, dropout_p, seed,
+                                 static_cast<cudaStream_t>(stream));
   static bool once = false;
   const int smem_kv = (6 * TILE_FLOATS + 2 * TS) * sizeof(float);
   const int smem_q = (5 * TILE_FLOATS + 2 * TS) * sizeof(float);

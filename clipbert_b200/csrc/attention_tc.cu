@@ -3,7 +3,9 @@
 // tiles live in shared memory as bf16, the 64x64x64 products run on mma.sync.m16n8k16 (bf16 in, fp32 accumulate)
 // with ldmatrix operand fetches, softmax / dropout / dS stay in the accumulator registers (the S accumulator
 // layout is reused as the A operand of the next product). Same math, masks, dropout stream and lse convention as
-// csrc/attention.cu, which remains the path for L > 64 (448 px frames, 512-token inference).
+// csrc/attention.cu, whose CUDA-core kernels remain the general path (cb_debug_attention_general) and the test reference.
+// Sequences longer than 64 tokens (448 / 768 px frames, 512-token inference) run the multi-tile kernels further down: the
+// online-softmax forward (attn_tc_fwd_flash_kernel) and the backward pair attn_tc_bwd_kv_kernel / attn_tc_bwd_q_kernel.
 //
 // Why mma.sync and not wgmma here: a (sequence, head) problem is 41x41x64 - 0.9 % of the layer FLOPs; it is
 // latency-bound, and a wgmma pipeline (warpgroup-wide 64-row tiles, TMA staging, mbarrier hand-offs) costs more than
@@ -479,6 +481,276 @@ __global__ void __launch_bounds__(RT * 32) attn_tc_bwd_kernel(const __nv_bfloat1
   tc_store_tile<R>(dSs, dk + row0 * ld_dqkv + h * 64, ld_dqkv, L);
 }
 
+// ------------------------------------------------------------------------------------------------ backward, any L
+// The tensor-core backward for sequences longer than one tile (448 px: L = 69 .. 149; 768 px: L = 130 .. 169; paragraph
+// retrieval: L = 521). Two kernels, 4 warps each, grid (ceil(L / 64), heads, nseq), the split of attn_bwd_kv_kernel /
+// attn_bwd_q_kernel (attention.cu): attn_tc_bwd_kv_kernel owns a 64-key tile and loops over query tiles (dK, dV), attn_tc_bwd_q_kernel
+// owns a 64-query tile and loops over key tiles (dQ). Every output row is written by exactly one CTA, in a fixed order: no atomics,
+// no workspace, bit-identical from run to run. Per (query tile, key tile) pair the math is phase 1 of attn_tc_bwd_kernel.
+//
+// Tail tiles: a 16-row slab that lies entirely beyond L costs no MMA. The helpers below are tc_mm_abt / tc_mm_ab_reg / tc_mm_atb
+// with the output column pairs (abt) or the contraction slabs (ab_reg, atb) cut at a run-time count of live slabs; at L = 69 the
+// second tile holds 5 live rows, and its products run over one slab instead of four.
+__device__ __forceinline__ int tc_live_slabs(int nrows) { return min(4, (nrows + 15) >> 4); }
+
+// acc = A(16 x 64 rows r0.. of As) * B^T, output columns [0, 16 njp) only (the others stay zero)
+__device__ __forceinline__ void tc_mm_abt_live(float (&acc)[8][4], const __nv_bfloat16* As, const __nv_bfloat16* Bs, int r0, int lane, int njp) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    uint32_t a[4];
+    ldsm_x4(a, As + (r0 + (lane & 15)) * TC_LD + ks * 16 + (lane >> 4) * 8);
+#pragma unroll
+    for (int jp = 0; jp < 4; ++jp) {
+      if (jp < njp) {
+        uint32_t b[4];
+        ldsm_x4(b, Bs + (jp * 16 + (lane & 7) + (lane >> 4) * 8) * TC_LD + ks * 16 + ((lane >> 3) & 1) * 8);
+        mma16816(acc[2 * jp], a, b[0], b[1]);
+        mma16816(acc[2 * jp + 1], a, b[2], b[3]);
+      }
+    }
+  }
+}
+// acc += A(16 x 64, register fragments afrag[ks]) * B ([k][n] row-major), contracted over the slabs ks < nks of Bs
+__device__ __forceinline__ void tc_mm_ab_reg_live(float (&acc)[8][4], const uint32_t (&afrag)[4][4], const __nv_bfloat16* Bs, int lane, int nks) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    if (ks < nks) {
+#pragma unroll
+      for (int jp = 0; jp < 4; ++jp) {
+        uint32_t b[4];
+        ldsm_x4_t(b, Bs + (ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * TC_LD + jp * 16 + (lane >> 4) * 8);
+        mma16816(acc[2 * jp], afrag[ks], b[0], b[1]);
+        mma16816(acc[2 * jp + 1], afrag[ks], b[2], b[3]);
+      }
+    }
+  }
+}
+// acc += A^T-stored (As holds [k][m]) * B ([k][n] row-major), contracted over the slabs ks < nks; accumulates (no zeroing), so
+// dV / dK build up across query tiles
+__device__ __forceinline__ void tc_mm_atb_live(float (&acc)[8][4], const __nv_bfloat16* As, const __nv_bfloat16* Bs, int m0, int lane, int nks) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    if (ks < nks) {
+      uint32_t a[4];
+      const int mi = lane >> 3;
+      ldsm_x4_t(a, As + (ks * 16 + (lane & 7) + (mi >> 1) * 8) * TC_LD + m0 + (mi & 1) * 8);
+#pragma unroll
+      for (int jp = 0; jp < 4; ++jp) {
+        uint32_t b[4];
+        ldsm_x4_t(b, Bs + (ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * TC_LD + jp * 16 + (lane >> 4) * 8);
+        mma16816(acc[2 * jp], a, b[0], b[1]);
+        mma16816(acc[2 * jp + 1], a, b[2], b[3]);
+      }
+    }
+  }
+}
+
+// additive key mask of the 64 keys k0.. (-10000 for masked text keys, -inf beyond L), and, for the 64 queries q0.., the saved
+// log-sum-exp and D_i = sum_d dO[i][d] O[i][d] (8 threads per row, 16 rows per pass, 4 passes); rows beyond L get 0
+__device__ __forceinline__ void tc_key_mask(float* madd, const int64_t* text_mask, int b, int k0, int L, int Lt) {
+  if (threadIdx.x < 64) {
+    const int j = k0 + threadIdx.x;
+    float m = -INFINITY;
+    if (j < L) m = (j < Lt && text_mask[static_cast<int64_t>(b) * Lt + j] == 0) ? -10000.f : 0.f;
+    madd[threadIdx.x] = m;
+  }
+}
+__device__ __forceinline__ void tc_row_stats(float* Dv, float* lses, const __nv_bfloat16* ctx_h, const __nv_bfloat16* dctx_h, int64_t ld_ctx,
+                                             const float* lse_bh, int q0, int L) {
+  if (threadIdx.x < 64) lses[threadIdx.x] = q0 + threadIdx.x < L ? lse_bh[q0 + threadIdx.x] : 0.f;
+#pragma unroll
+  for (int pass = 0; pass < 4; ++pass) {
+    const int r = pass * 16 + (threadIdx.x >> 3), c = (threadIdx.x & 7) * 8;
+    float acc = 0.f;
+    if (q0 + r < L) {
+      const uint4 uo = *reinterpret_cast<const uint4*>(ctx_h + static_cast<int64_t>(q0 + r) * ld_ctx + c);
+      const uint4 ud = *reinterpret_cast<const uint4*>(dctx_h + static_cast<int64_t>(q0 + r) * ld_ctx + c);
+      const uint32_t ov[4] = {uo.x, uo.y, uo.z, uo.w}, dvv[4] = {ud.x, ud.y, ud.z, ud.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 a = unpack_bf16x2(ov[e]), d = unpack_bf16x2(dvv[e]);
+        acc += a.x * d.x + a.y * d.y;
+      }
+    }
+    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+    if ((threadIdx.x & 7) == 0) Dv[r] = acc;
+  }
+}
+
+// P (dropped probabilities) and dS of a warp's 16 query rows against one 64-key tile, from the S and dP accumulators, in place:
+// s[j] becomes P * dropout multiplier, dp[j] becomes dS. qrow = index of row rq within the sequence; rows >= L give P = dS = 0.
+__device__ __forceinline__ void tc_p_ds(float (&s)[8][4], float (&dp)[8][4], const float* madd, float l0, float l1, float D0, float D1,
+                                        bool ok0, bool ok1, int b, int h, int H, int L, int qrow, int k0, int cq, float scale, const TcDrop& dc) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float m0 = madd[j * 8 + cq], m1 = madd[j * 8 + cq + 1];
+    float p0 = ok0 ? __expf(s[j][0] * scale + m0 - l0) : 0.f, p1 = ok0 ? __expf(s[j][1] * scale + m1 - l0) : 0.f;
+    float p2 = ok1 ? __expf(s[j][2] * scale + m0 - l1) : 0.f, p3 = ok1 ? __expf(s[j][3] * scale + m1 - l1) : 0.f;
+    float r_0 = 1.f, r_1 = 1.f, r_2 = 1.f, r_3 = 1.f;
+    if (dc.thresh) {
+      const uint64_t base0 = ((static_cast<uint64_t>(b) * H + h) * L + qrow) * L + k0 + j * 8 + cq;
+      const uint64_t base1 = base0 + static_cast<uint64_t>(8) * L;
+      dropout_mult2(dc.seed, base0, dc.thresh, dc.inv_keep, r_0, r_1);
+      dropout_mult2(dc.seed, base1, dc.thresh, dc.inv_keep, r_2, r_3);
+    }
+    dp[j][0] = p0 * (dp[j][0] * r_0 - D0); dp[j][1] = p1 * (dp[j][1] * r_1 - D0);
+    dp[j][2] = p2 * (dp[j][2] * r_2 - D1); dp[j][3] = p3 * (dp[j][3] * r_3 - D1);
+    s[j][0] = p0 * r_0; s[j][1] = p1 * r_1; s[j][2] = p2 * r_2; s[j][3] = p3 * r_3;
+  }
+}
+
+// dK, dV of one 64-key tile. K, V and the key mask stay in smem; per query tile: phase 1 (each warp: 16 query rows x 64 keys)
+// forms P and dS and writes them to smem, phase 2 (each warp: 16 key rows) accumulates dV += Pd^T dO and dK += dS^T Q in registers.
+__global__ void __launch_bounds__(TC_THREADS) attn_tc_bwd_kv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                                    const __nv_bfloat16* __restrict__ v, int64_t ld_qkv,
+                                                                    const int64_t* __restrict__ text_mask, const __nv_bfloat16* __restrict__ ctx,
+                                                                    const __nv_bfloat16* __restrict__ dctx, int64_t ld_ctx,
+                                                                    const float* __restrict__ lse, __nv_bfloat16* __restrict__ dk,
+                                                                    __nv_bfloat16* __restrict__ dv, int64_t ld_dqkv, int L, int Lt, int H,
+                                                                    float scale, TcDrop dc_in) {
+  pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
+  const TcDrop dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
+  pdl_trigger();
+  extern __shared__ __align__(16) uint8_t tc_smem[];
+  __nv_bfloat16* Ks = reinterpret_cast<__nv_bfloat16*>(tc_smem);
+  __nv_bfloat16* Vs = Ks + TC_TILE;
+  __nv_bfloat16* Qs = Vs + TC_TILE;
+  __nv_bfloat16* dOs = Qs + TC_TILE;
+  __nv_bfloat16* Ps = dOs + TC_TILE;     // dropped probabilities [query][key]
+  __nv_bfloat16* dSs = Ps + TC_TILE;     // dS [query][key]
+  float* madd = reinterpret_cast<float*>(dSs + TC_TILE);
+  float* Dv = madd + 64;
+  float* lses = Dv + 64;
+  const int kb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int k0 = kb * 64;
+  const int64_t row0 = static_cast<int64_t>(b) * L;
+  const int nks = tc_live_slabs(L - k0);          // live 16-key slabs of this tile
+  tc_load_tile(Ks, k + (row0 + k0) * ld_qkv + h * 64, ld_qkv, L - k0);
+  tc_load_tile(Vs, v + (row0 + k0) * ld_qkv + h * 64, ld_qkv, L - k0);
+  tc_key_mask(madd, text_mask, b, k0, L, Lt);
+  const int r0 = warp * 16;
+  const int rq = r0 + (lane >> 2), cq = 2 * (lane & 3);
+  float dvacc[8][4], dkacc[8][4];
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) dvacc[j][e] = dkacc[j][e] = 0.f;
+  const int nqb = (L + 63) / 64;
+  for (int qb = 0; qb < nqb; ++qb) {
+    const int q0 = qb * 64;
+    const int nqs = tc_live_slabs(L - q0);        // live 16-query slabs of this tile
+    __syncthreads();                               // phase 2 of the previous query tile is done with Qs, dOs, Ps, dSs
+    tc_load_tile(Qs, q + (row0 + q0) * ld_qkv + h * 64, ld_qkv, L - q0);
+    tc_load_tile(dOs, dctx + (row0 + q0) * ld_ctx + h * 64, ld_ctx, L - q0);
+    tc_row_stats(Dv, lses, ctx + row0 * ld_ctx + h * 64, dctx + row0 * ld_ctx + h * 64, ld_ctx, lse + (static_cast<int64_t>(b) * H + h) * L, q0, L);
+    __syncthreads();
+    // ---- phase 1: this warp's 16 query rows against the 64 keys: P, dS -> smem ----
+    if (warp < nqs) {
+      float s[8][4], dp[8][4];
+      tc_mm_abt_live(s, Qs, Ks, r0, lane, nks);
+      tc_mm_abt_live(dp, dOs, Vs, r0, lane, nks);
+      tc_p_ds(s, dp, madd, lses[rq], lses[rq + 8], Dv[rq], Dv[rq + 8], q0 + rq < L, q0 + rq + 8 < L, b, h, H, L, q0 + rq, k0, cq, scale, dc);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        *reinterpret_cast<uint32_t*>(Ps + rq * TC_LD + j * 8 + cq) = pack_bf16x2(s[j][0], s[j][1]);
+        *reinterpret_cast<uint32_t*>(Ps + (rq + 8) * TC_LD + j * 8 + cq) = pack_bf16x2(s[j][2], s[j][3]);
+        *reinterpret_cast<uint32_t*>(dSs + rq * TC_LD + j * 8 + cq) = pack_bf16x2(dp[j][0], dp[j][1]);
+        *reinterpret_cast<uint32_t*>(dSs + (rq + 8) * TC_LD + j * 8 + cq) = pack_bf16x2(dp[j][2], dp[j][3]);
+      }
+    } else {                                       // all 16 query rows beyond L: no products, P = dS = 0
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        *reinterpret_cast<uint32_t*>(Ps + rq * TC_LD + j * 8 + cq) = 0u;
+        *reinterpret_cast<uint32_t*>(Ps + (rq + 8) * TC_LD + j * 8 + cq) = 0u;
+        *reinterpret_cast<uint32_t*>(dSs + rq * TC_LD + j * 8 + cq) = 0u;
+        *reinterpret_cast<uint32_t*>(dSs + (rq + 8) * TC_LD + j * 8 + cq) = 0u;
+      }
+    }
+    __syncthreads();
+    // ---- phase 2: this warp's 16 key rows: dV += Pd^T dO, dK += dS^T Q over the live query slabs ----
+    if (warp < nks) {
+      tc_mm_atb_live(dvacc, Ps, dOs, r0, lane, nqs);
+      tc_mm_atb_live(dkacc, dSs, Qs, r0, lane, nqs);
+    }
+  }
+  __syncthreads();                                 // P, dS fully consumed: stage dV / dK in their tiles
+  tc_acc_to_smem(dvacc, Ps, r0, lane, 1.0f);
+  tc_acc_to_smem(dkacc, dSs, r0, lane, scale);
+  __syncthreads();
+  tc_store_tile(Ps, dv + (row0 + k0) * ld_dqkv + h * 64, ld_dqkv, L - k0);
+  tc_store_tile(dSs, dk + (row0 + k0) * ld_dqkv + h * 64, ld_dqkv, L - k0);
+}
+
+// dQ of one 64-query tile. Q, dO, lse and D stay in smem; per key tile each warp forms S and dP for its 16 query rows, turns them
+// into dS in registers, and accumulates dQ += dS K with dS as the register-fragment A operand (dS never goes through smem).
+__global__ void __launch_bounds__(TC_THREADS) attn_tc_bwd_q_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                                   const __nv_bfloat16* __restrict__ v, int64_t ld_qkv,
+                                                                   const int64_t* __restrict__ text_mask, const __nv_bfloat16* __restrict__ ctx,
+                                                                   const __nv_bfloat16* __restrict__ dctx, int64_t ld_ctx,
+                                                                   const float* __restrict__ lse, __nv_bfloat16* __restrict__ dq,
+                                                                   int64_t ld_dqkv, int L, int Lt, int H, float scale, TcDrop dc_in) {
+  pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
+  const TcDrop dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
+  pdl_trigger();
+  extern __shared__ __align__(16) uint8_t tc_smem[];
+  __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(tc_smem);
+  __nv_bfloat16* dOs = Qs + TC_TILE;
+  __nv_bfloat16* Ks = dOs + TC_TILE;
+  __nv_bfloat16* Vs = Ks + TC_TILE;
+  float* madd = reinterpret_cast<float*>(Vs + TC_TILE);
+  float* Dv = madd + 64;
+  float* lses = Dv + 64;
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = qb * 64;
+  const int64_t row0 = static_cast<int64_t>(b) * L;
+  const bool live = warp < tc_live_slabs(L - q0);  // this warp holds at least one query row < L
+  tc_load_tile(Qs, q + (row0 + q0) * ld_qkv + h * 64, ld_qkv, L - q0);
+  tc_load_tile(dOs, dctx + (row0 + q0) * ld_ctx + h * 64, ld_ctx, L - q0);
+  tc_row_stats(Dv, lses, ctx + row0 * ld_ctx + h * 64, dctx + row0 * ld_ctx + h * 64, ld_ctx, lse + (static_cast<int64_t>(b) * H + h) * L, q0, L);
+  const int r0 = warp * 16;
+  const int rq = r0 + (lane >> 2), cq = 2 * (lane & 3);
+  float acc[8][4];
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
+  const int nkb = (L + 63) / 64;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int k0 = kb * 64;
+    const int nks = tc_live_slabs(L - k0);        // live 16-key slabs of this tile
+    __syncthreads();                               // every warp is done with the previous key tile
+    tc_load_tile(Ks, k + (row0 + k0) * ld_qkv + h * 64, ld_qkv, L - k0);
+    tc_load_tile(Vs, v + (row0 + k0) * ld_qkv + h * 64, ld_qkv, L - k0);
+    tc_key_mask(madd, text_mask, b, k0, L, Lt);
+    __syncthreads();
+    if (live) {
+      float s[8][4], dp[8][4];
+      tc_mm_abt_live(s, Qs, Ks, r0, lane, nks);
+      tc_mm_abt_live(dp, dOs, Vs, r0, lane, nks);
+      tc_p_ds(s, dp, madd, lses[rq], lses[rq + 8], Dv[rq], Dv[rq + 8], q0 + rq < L, q0 + rq + 8 < L, b, h, H, L, q0 + rq, k0, cq, scale, dc);
+      uint32_t dsf[4][4];                          // dS in the accumulator layout = the A fragments of dS K
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        dsf[j >> 1][(j & 1) * 2] = pack_bf16x2(dp[j][0], dp[j][1]);
+        dsf[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(dp[j][2], dp[j][3]);
+      }
+      tc_mm_ab_reg_live(acc, dsf, Ks, lane, nks);  // dQ += dS K
+    }
+  }
+  __syncthreads();                                 // everyone is done reading Qs: reuse it to stage dQ
+  tc_acc_to_smem(acc, Qs, r0, lane, scale);
+  __syncthreads();
+  tc_store_tile(Qs, dq + (row0 + q0) * ld_dqkv + h * 64, ld_dqkv, L - q0);
+}
+
 static TcDrop make_tc_drop(float p, uint64_t seed) { return make_drop(p, seed); }
 
 // called from cb_attention_fwd / cb_attention_bwd (attention.cu) when l <= 64
@@ -564,6 +836,36 @@ int attention_tc_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, 
   if (l <= 48 && g_tc_rows48)
     return launch_tc_bwd<3>(qkv, ld_qkv, text_mask, ctx, dctx, ld_ctx, lse, dqkv, ld_dqkv, nseq, l, lt, heads, dropout_p, seed, stream);
   return launch_tc_bwd<4>(qkv, ld_qkv, text_mask, ctx, dctx, ld_ctx, lse, dqkv, ld_dqkv, nseq, l, lt, heads, dropout_p, seed, stream);
+}
+
+// called from cb_attention_bwd (attention.cu) for l > 64. kv kernel: K, V, Q, dO, P, dS tiles + three 64-float vectors = 55 KB;
+// q kernel: Q, dO, K, V tiles + the same vectors = 37 KB; both leave room for several CTAs per SM.
+int attention_tc_bwd_long(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const void* ctx, const void* dctx, int64_t ld_ctx,
+                          const float* lse, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, float dropout_p, uint64_t seed,
+                          cudaStream_t stream) {
+  const int smem_kv = 6 * TC_TILE * 2 + 3 * 64 * 4;
+  const int smem_q = 4 * TC_TILE * 2 + 3 * 64 * 4;
+  static bool once = false;
+  if (!once) {
+    cudaError_t e = cudaFuncSetAttribute(attn_tc_bwd_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_kv);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_tc_bwd_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_q);
+    if (e != cudaSuccess) { set_error("attention_tc_bwd_long smem: %s", cudaGetErrorString(e)); return CB_ERR_CUDA; }
+    once = true;
+  }
+  const __nv_bfloat16* base = static_cast<const __nv_bfloat16*>(qkv);
+  __nv_bfloat16* dbase = static_cast<__nv_bfloat16*>(dqkv);
+  const int hid = heads * 64;
+  const TcDrop dc = make_tc_drop(dropout_p, seed);
+  const dim3 grid(ceil_div(l, 64), heads, nseq);
+  launch_k(attn_tc_bwd_kv_kernel, grid, TC_THREADS, smem_kv, stream, base, base + hid, base + 2 * hid, ld_qkv, text_mask,
+           static_cast<const __nv_bfloat16*>(ctx), static_cast<const __nv_bfloat16*>(dctx), ld_ctx, lse, dbase + hid, dbase + 2 * hid,
+           ld_dqkv, l, lt, heads, 0.125f, dc);
+  int rc = check_launch("cb_attention_bwd(tc, kv)");
+  if (rc) return rc;
+  launch_k(attn_tc_bwd_q_kernel, grid, TC_THREADS, smem_q, stream, base, base + hid, base + 2 * hid, ld_qkv, text_mask,
+           static_cast<const __nv_bfloat16*>(ctx), static_cast<const __nv_bfloat16*>(dctx), ld_ctx, lse, dbase, ld_dqkv, l, lt, heads,
+           0.125f, dc);
+  return check_launch("cb_attention_bwd(tc, q)");
 }
 
 }  // namespace cb

@@ -202,7 +202,10 @@ int cb_embed_visual_bwd(const void* dh, const void* grid, const int32_t* seq2vid
  * qkv: bf16 [nseq*l, 3*heads*64] (Q | K | V as produced by the fused N=2304 projection);
  * text_mask: int64 [nseq, lt] (visual tokens are always attendable, modeling.py:217-220);
  * ctx: bf16 [nseq*l, heads*64]; lse: fp32 [nseq, heads, l] log-sum-exp saved for the backward.
- * The backward recomputes P tile by tile from Q, K, lse and regenerates the dropout mask.
+ * The backward recomputes P tile by tile from Q, K, lse and regenerates the dropout mask. Every length runs on tensor
+ * cores (mma.sync): l <= 64 in one CTA per (sequence, head); longer sequences in two kernels, one per 64-key tile
+ * (dK, dV) and one per 64-query tile (dQ). Each output row is written by one CTA: no atomics, no workspace, results
+ * bit-identical from run to run. cb_debug_attention_general(1) selects the CUDA-core kernels instead, for every length.
  * ------------------------------------------------------------------------------------------ */
 int cb_attention_fwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, void* ctx, int64_t ld_ctx, float* lse,
                      int nseq, int l, int lt, int heads, int head_dim, float dropout_p, uint64_t seed, void* stream);
