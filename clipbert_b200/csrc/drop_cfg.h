@@ -5,8 +5,8 @@
 namespace cb {
 
 struct DropCfg {
-  uint32_t thresh;          // p * 65536 (0 = no dropout)
-  float inv_keep;           // 1 / (1 - p)
+  uint32_t thresh;          // p * 65536 (0 = no dropout, 65536 = drop everything)
+  float inv_keep;           // 1 / (1 - p), 0 when p >= 1
   uint64_t seed;
   const uint64_t* offset;   // device word added (times an odd constant) to the seed at run time, or nullptr
 };
@@ -18,7 +18,12 @@ inline DropCfg make_drop(float p, uint64_t seed) {
   DropCfg d;
   d.seed = seed;
   d.offset = drop_offset_ptr();
-  if (p > 0.0f) {
+  if (p >= 1.0f) {
+    // nn.Dropout(p=1) returns zeros. No 16-bit lane reaches 65536, so every element is dropped; the multiplier of a kept
+    // element would be 1 / 0 = inf, which turns a kept 0 into NaN.
+    d.thresh = 65536u;
+    d.inv_keep = 0.0f;
+  } else if (p > 0.0f) {
     double t = static_cast<double>(p) * 65536.0 + 0.5;
     d.thresh = t >= 65535.0 ? 65535u : static_cast<uint32_t>(t);
     if (d.thresh == 0) d.thresh = 1;

@@ -1248,7 +1248,8 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
   CB_REQUIRE(d.ntaps == 1 || d.ntaps == 9 || (d.ntaps == 4 && d.mode == CB_GEMM_TN),
              "cb_gemm: ntaps must be 1, 9 (3x3 conv) or 4 (row taps, TN only) (got %d)", d.ntaps);
   CB_REQUIRE(d.mode == CB_GEMM_TN || d.mode == CB_GEMM_WGRAD || d.mode == CB_GEMM_NN, "cb_gemm: bad mode %d", d.mode);
-  CB_REQUIRE(d.dropout_p >= 0.0f && d.dropout_p < 1.0f, "cb_gemm: dropout_p out of range");
+  // [0, 1] as nn.Dropout; p = 1 drops every element (make_drop)
+  CB_REQUIRE(d.dropout_p >= 0.0f && d.dropout_p <= 1.0f, "cb_gemm: dropout_p %g outside [0, 1]", d.dropout_p);
 
   GemmEpi epi;
   epi.scale = d.scale;

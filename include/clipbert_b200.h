@@ -56,7 +56,19 @@ int cb_set_pdl(int enable);
  * next replay sees an advanced word and draws new ones. cb_dropout_offset_advance enqueues a one-thread kernel:
  * ++*counter; if (snapshot) *snapshot = *counter - a step advances the model's counter once and binds the per-step
  * snapshot, so a later step (or a second forward before this one's backward) cannot change the masks of this one.
- * Keep decision of element e: 16-bit lane (e & 3) of splitmix64(seed, e >> 2) >= round(p * 65536). */
+ *
+ * The mask (pinned by tests/dropout_ref.py and tests/test_gpu_dropout.py):
+ *   seed'   = seed + word * 0xD1342543DE82EF95 (mod 2^64) while a word is bound, else seed
+ *   keep(e) = 16-bit lane (e & 3) of splitmix64(seed', e >> 2) >= thresh, thresh = round(p * 65536) clamped to [1, 65535]
+ *             for 0 < p < 1; y = x / (1 - p) where kept, 0 elsewhere. p <= 0: no dropout. p >= 1: thresh = 65536 and a
+ *             multiplier of 0, so every element is dropped (as nn.Dropout(p=1)).
+ *   element index e of each consumer:
+ *     cb_dropout                   i, the flat index into x
+ *     cb_gemm epilogue (TN, NN)    out_row * n + col: n is the descriptor's column count (not out_ld), out_row the row
+ *                                  after the row map
+ *     cb_layernorm_bwd             row * 768 + col (dx_drop, dbias_drop)
+ *     cb_embed_text_* / _visual_*  (seq * l + pos) * 768 + col: text rows at pos = t, visual cell j at pos = lt + j
+ *     cb_attention_fwd / _bwd      ((seq * heads + h) * l + i) * l + j for probability P[i, j] of head h */
 int cb_dropout_offset_bind(const uint64_t* device_word);
 int cb_dropout_offset_advance(uint64_t* counter, uint64_t* snapshot, void* stream);
 

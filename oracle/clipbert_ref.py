@@ -201,7 +201,14 @@ def visual_embeddings(grid, sd, prefix, eps, sample_indices=None):
     return layer_norm(v, sd, prefix + "LayerNorm.", eps)
 
 
-def bert_layer(h, ext_mask, sd, prefix, n_heads, eps, rnd=EXACT):
+def _dropout(drop, site, layer, x):
+    """Train-mode nn.Dropout hook: ``drop(site, layer, x)`` returns x with a mask applied (x unchanged when drop is None).
+    Sites: "text_emb" / "visual_emb" after the embedding LayerNorms, "attn_probs", "attn_out" / "ffn_out" after the dense of
+    BertSelfOutput / BertOutput (before the residual), "pooled" before the classifier; layer = encoder layer index or None."""
+    return x if drop is None else drop(site, layer, x)
+
+
+def bert_layer(h, ext_mask, sd, prefix, n_heads, eps, rnd=EXACT, drop=None, layer=None):
     """BertLayer.forward (transformers.py:394-418) = attention + intermediate + output."""
     b, l, d = h.shape
     hd = d // n_heads
@@ -214,26 +221,28 @@ def bert_layer(h, ext_mask, sd, prefix, n_heads, eps, rnd=EXACT):
     k = split(r(linear(h, sd, prefix + "attention.self.key.", rnd)))
     v = split(r(linear(h, sd, prefix + "attention.self.value.", rnd)))
     s = torch.matmul(q, k.transpose(-1, -2)) / math.sqrt(hd) + ext_mask       # :257-264
-    p = torch.softmax(s, dim=-1)
+    p = _dropout(drop, "attn_probs", layer, torch.softmax(s, dim=-1))                    # :271
     ctx = r(torch.matmul(p, v).permute(0, 2, 1, 3).reshape(b, l, d))
-    a = r(layer_norm(r(linear(ctx, sd, prefix + "attention.output.dense.", rnd) + h), sd,
+    a = r(layer_norm(r(_dropout(drop, "attn_out", layer, linear(ctx, sd, prefix + "attention.output.dense.", rnd)) + h), sd,
                      prefix + "attention.output.LayerNorm.", eps))            # :297-301
     i = r(F.gelu(linear(a, sd, prefix + "intermediate.dense.", rnd)))         # :363-366 (erf gelu)
-    return r(layer_norm(r(linear(i, sd, prefix + "output.dense.", rnd) + a), sd, prefix + "output.LayerNorm.", eps))
+    return r(layer_norm(r(_dropout(drop, "ffn_out", layer, linear(i, sd, prefix + "output.dense.", rnd)) + a), sd,
+                        prefix + "output.LayerNorm.", eps))                         # :377-381
 
 
 def clipbert_base_model(text_input_ids, grid, text_mask, sd, prefix="transformer.bert.", cfg=BERT_CFG,
-                        return_layers=False, rnd=EXACT, sample_indices=None):
-    """ClipBertBaseModel.forward: returns (sequence_output, pooled_output)."""
+                        return_layers=False, rnd=EXACT, sample_indices=None, drop=None):
+    """ClipBertBaseModel.forward: returns (sequence_output, pooled_output). drop: train-mode dropout hook (see _dropout)."""
     eps = cfg["layer_norm_eps"]
-    te = rnd.act(bert_embeddings(text_input_ids, sd, prefix + "embeddings.", eps))
-    ve = rnd.act(visual_embeddings(rnd.act(grid), sd, prefix + "visual_embeddings.", eps, sample_indices))
+    te = rnd.act(_dropout(drop, "text_emb", None, bert_embeddings(text_input_ids, sd, prefix + "embeddings.", eps)))
+    ve = rnd.act(_dropout(drop, "visual_emb", None, visual_embeddings(rnd.act(grid), sd, prefix + "visual_embeddings.", eps,
+                                                                         sample_indices)))
     mask = torch.cat([text_mask, text_mask.new_ones(ve.shape[:2])], dim=-1)      # modeling.py:217-220
     h = torch.cat([te, ve], dim=1)                                               # [text ; visual]
     ext = (1.0 - mask[:, None, None, :].to(h.dtype)) * -10000.0                  # hf get_extended_attention_mask
     layers = [h]
     for i in range(cfg["num_hidden_layers"]):
-        h = bert_layer(h, ext, sd, "%sencoder.layer.%d." % (prefix, i), cfg["num_attention_heads"], eps, rnd)
+        h = bert_layer(h, ext, sd, "%sencoder.layer.%d." % (prefix, i), cfg["num_attention_heads"], eps, rnd, drop, i)
         layers.append(h)
     pooled = rnd.act(torch.tanh(linear(h[:, 0], sd, prefix + "pooler.dense.", rnd)))   # transformers.py:470-476
     if return_layers:
@@ -241,8 +250,9 @@ def clipbert_base_model(text_input_ids, grid, text_mask, sd, prefix="transformer
     return h, pooled
 
 
-def mlp_head(pooled, sd, prefix="transformer.classifier.", rnd=EXACT):
-    """nn.Sequential(Linear(768,1536), ReLU, Linear(1536,num_labels)) (modeling.py:534-539)."""
+def mlp_head(pooled, sd, prefix="transformer.classifier.", rnd=EXACT, drop=None):
+    """dropout (modeling.py:552) -> nn.Sequential(Linear(768,1536), ReLU, Linear(1536,num_labels)) (modeling.py:534-539)."""
+    pooled = _dropout(drop, "pooled", None, pooled)
     return linear(rnd.act(rnd.relu(linear(pooled, sd, prefix + "0.", rnd), prefix + "relu")), sd, prefix + "2.", rnd)
 
 
@@ -255,10 +265,10 @@ def retrieval_loss(logits, labels, loss_type="ce", margin=0.2, sample_size=-1):
 
 
 def video_text_retrieval(text_input_ids, grid, text_mask, sd, labels=None, loss_type="ce", margin=0.2,
-                         sample_size=-1, rnd=EXACT):
-    """ClipBertForVideoTextRetrieval.forward (modeling.py:543-558), eval mode (dropout off)."""
-    _, pooled = clipbert_base_model(text_input_ids, grid, text_mask, sd, rnd=rnd)
-    logits = mlp_head(pooled, sd, rnd=rnd)
+                         sample_size=-1, rnd=EXACT, drop=None):
+    """ClipBertForVideoTextRetrieval.forward (modeling.py:543-558); eval mode (dropout off) unless a drop hook is given."""
+    _, pooled = clipbert_base_model(text_input_ids, grid, text_mask, sd, rnd=rnd, drop=drop)
+    logits = mlp_head(pooled, sd, rnd=rnd, drop=drop)
     loss = retrieval_loss(logits, labels, loss_type, margin, sample_size) if labels is not None else 0
     return dict(logits=logits, loss=loss)
 

@@ -4,7 +4,8 @@ Purpose: run the Python orchestration of clipbert_b200/modeling.py (buffer plann
 epilogue flags, index bookkeeping) on a machine without a GPU and compare it with the oracle. It swaps the functions of
 clipbert_b200.ops for torch code that does what the header says each entry point does (bf16 buffers in, fp32 arithmetic,
 bf16 / fp32 out); nothing in the product imports this file, and the kernels themselves are only ever checked on an H100
-(tests/test_gpu_*.py). Dropout must be off (the counter RNG of the kernels is not restated here).
+(tests/test_gpu_*.py). Dropout draws the kernels' masks (tests/dropout_ref.py) at each consumer's element index, with the
+device word bound by dropout_offset_bind folded into the seed, so the seed plumbing of the model is checked as well.
 """
 import contextlib
 import math
@@ -12,12 +13,18 @@ import math
 import torch
 import torch.nn.functional as F
 
+import dropout_ref as D
+
 F32 = torch.float32
 IGNORE_DROPOUT = False      # emulated_ops(ignore_dropout=True): dropout arguments are accepted and treated as p = 0 (dry runs)
 
 
-def _no_dropout(p):
-    assert IGNORE_DROPOUT or not p, "emulator: dropout must be off"
+def _drop_mult(p, seed, idx):
+    """fp32 multipliers (0 or 1 / (1 - p)) shaped like the index array idx, or None when dropout is off."""
+    if IGNORE_DROPOUT or not p:
+        return None
+    word = None if BOUND_DROPOUT_WORD is None else int(BOUND_DROPOUT_WORD.reshape(-1)[0].item())
+    return torch.from_numpy(D.multipliers(D.effective_seed(seed, word), idx, p))
 
 
 def _mat(t, rows, cols, ld):
@@ -72,7 +79,6 @@ def _out_rows(kw, m):
 def gemm(**kw):
     mode, m, n, k = kw.get("mode", 0), kw["m"], kw["n"], kw["k"]
     ntaps, tap_w, tap_sign = kw.get("ntaps", 1), kw.get("tap_w", 0), kw.get("tap_sign", 1)
-    _no_dropout(kw.get("dropout_p"))
     a, b, out = kw["a"], kw["b"], kw["out"]
     if mode == 1:                                       # WGRAD: out[m, t*N + n] += rowscale[m] * sum_p A[p, m] B[p + shift_t, n]
         A = _mat(a, k, m, kw["a_ld"]).to(F32)
@@ -98,11 +104,14 @@ def gemm(**kw):
         v = v * kw["scale"][:n].to(F32)
     if kw.get("shift") is not None:
         v = v + kw["shift"][:n].to(F32)
+    dst, n_dst = _out_rows(kw, m)
+    keep = dst >= 0
+    mult = _drop_mult(kw.get("dropout_p"), kw.get("dropout_seed", 0), D.gemm_index(dst.clamp(min=0).numpy(), n))
+    if mult is not None:                                # keyed by output row * n + column
+        v = v * mult
     if kw.get("residual") is not None:
         v = v + _mat(kw["residual"], m, n, kw["res_ld"]).to(F32)
     act = kw.get("act", 0)
-    dst, n_dst = _out_rows(kw, m)
-    keep = dst >= 0
     if kw.get("out2") is not None:
         _mat(kw["out2"], n_dst, n, kw["out2_ld"])[dst[keep]] = (_gelu_grad(v) if act == 4 else v)[keep].to(kw["out2"].dtype)
     if act == 1:
@@ -147,30 +156,38 @@ def layernorm_fwd(x, gamma, beta, y, stats, eps):
 
 
 def layernorm_bwd(dy, x, stats, gamma, dx, dx_drop, dgamma, dbeta, dbias_drop, p, seed):
-    _no_dropout(p)
     d, dg, db = _ln_bwd(dy.to(F32), x.to(F32), stats[:, 0], stats[:, 1], gamma)
     dx.copy_(d)
     if dx_drop is not None:
-        dx_drop.copy_(d)
-    dgamma.add_(dg)
-    dbeta.add_(db)
-    if dbias_drop is not None:
-        dbias_drop[: d.shape[1]].add_(dx.to(F32).sum(0))     # column sums of the bf16 tensor the dense's dgrad consumes
+        mult = _drop_mult(p, seed, D.layernorm_index(d.shape[0]))
+        dx_drop.copy_(d if mult is None else d * mult)
+    if dgamma is not None:
+        dgamma.add_(dg)
+    if dbeta is not None:
+        dbeta.add_(db)
+    if dbias_drop is not None:      # column sums of the bf16 tensor the dense's dgrad consumes
+        dbias_drop[: d.shape[1]].add_((dx if dx_drop is None else dx_drop).to(F32).sum(0))
+
+
+def _embed_mult(p, seed, nseq, l, pos):
+    return _drop_mult(p, seed, D.embedding_index(nseq, l, pos).reshape(nseq * len(pos), -1))
 
 
 def embed_text_fwd(ids, word, pos, typ, gamma, beta, out, stats, nseq, lt, l, eps, p, seed):
-    _no_dropout(p)
     v = word[ids] + pos[:lt][None] + typ[0][None, None]
     o, mean, rstd = _ln_fwd(v.reshape(nseq * lt, -1), gamma, beta, eps)
-    out.view(nseq, l, -1)[:, :lt].copy_(o.view(nseq, lt, -1))
+    mult = _embed_mult(p, seed, nseq, l, range(lt))
+    out.view(nseq, l, -1)[:, :lt].copy_((o if mult is None else o * mult).view(nseq, lt, -1))
     stats[:, 0], stats[:, 1] = mean, rstd
 
 
 def embed_text_bwd(dh, ids, word, pos, typ, gamma, stats, dword, dpos, dtyp, dgamma, dbeta, nseq, lt, l, p, seed):
-    _no_dropout(p)
     h = word.shape[1]
     v = (word[ids] + pos[:lt][None] + typ[0][None, None]).reshape(nseq * lt, h)
     dy = dh.view(nseq, l, h)[:, :lt].reshape(nseq * lt, h).to(F32)
+    mult = _embed_mult(p, seed, nseq, l, range(lt))
+    if mult is not None:
+        dy = dy * mult
     d, dg, db = _ln_bwd(dy, v, stats[:, 0], stats[:, 1], gamma)
     dgamma.add_(dg)
     dbeta.add_(db)
@@ -189,20 +206,22 @@ def _visual_pre(grid, seq2vid, n_ex, rowemb, colemb, typ, nseq, t, gh, gw):
 
 
 def embed_visual_fwd(grid, seq2vid, n_ex, rowemb, colemb, typ, gamma, beta, out, stats, nseq, t, gh, gw, lt, l, eps, p, seed):
-    _no_dropout(p)
     v, _, _ = _visual_pre(grid, seq2vid, n_ex, rowemb, colemb, typ, nseq, t, gh, gw)
     o, mean, rstd = _ln_fwd(v, gamma, beta, eps)
-    out.view(nseq, l, -1)[:, lt:].copy_(o.view(nseq, gh * gw, -1))
+    mult = _embed_mult(p, seed, nseq, l, range(lt, l))
+    out.view(nseq, l, -1)[:, lt:].copy_((o if mult is None else o * mult).view(nseq, gh * gw, -1))
     stats[:, 0], stats[:, 1] = mean, rstd
 
 
 def embed_visual_bwd(dh, grid, seq2vid, vid_start, n_ex, rowemb, colemb, typ, gamma, stats, dv_tmp, dgrid, drow, dcol, dtyp,
                      dgamma, dbeta, nseq, nvid, t, gh, gw, lt, l, p, seed):
-    _no_dropout(p)
     h = grid.shape[-1]
     lv = gh * gw
     v, vid, j = _visual_pre(grid, seq2vid, n_ex, rowemb, colemb, typ, nseq, t, gh, gw)
     dy = dh.view(nseq, l, h)[:, lt:].reshape(nseq * lv, h).to(F32)
+    mult = _embed_mult(p, seed, nseq, l, range(lt, l))
+    if mult is not None:
+        dy = dy * mult
     d, dg, db = _ln_bwd(dy, v, stats[:, 0], stats[:, 1], gamma)
     dgamma.add_(dg)
     dbeta.add_(db)
@@ -216,28 +235,29 @@ def embed_visual_bwd(dh, grid, seq2vid, vid_start, n_ex, rowemb, colemb, typ, ga
         dgrid.view(nvid, t, lv, h).copy_(per_vid[:, None].expand(nvid, t, lv, h))
 
 
-def _attention(qkv, text_mask, nseq, l, lt, heads):
+def _attention(qkv, text_mask, nseq, l, lt, heads, p, seed):
     hd = qkv.shape[1] // (3 * heads)
     q, k, v = (x.reshape(nseq, l, heads, hd).permute(0, 2, 1, 3) for x in qkv.view(nseq, l, 3, heads * hd).unbind(2))
     mask = torch.cat([text_mask.to(qkv.dtype), torch.ones(nseq, l - lt, dtype=qkv.dtype)], dim=1)
     s = q @ k.transpose(-1, -2) / math.sqrt(hd) + ((1.0 - mask) * -10000.0)[:, None, None, :]
     pr = torch.softmax(s, dim=-1)
+    mult = _drop_mult(p, seed, D.attention_index(nseq, heads, l))
+    if mult is not None:                                # the log-sum-exp is of the undropped scores
+        pr = pr * mult.to(pr.dtype)
     return (pr @ v).permute(0, 2, 1, 3).reshape(nseq * l, heads * hd), torch.logsumexp(s, dim=-1)
 
 
 def attention_fwd(qkv, text_mask, ctx, lse, nseq, l, lt, heads, p, seed):
-    _no_dropout(p)
-    o, ls = _attention(qkv.double(), text_mask, nseq, l, lt, heads)
+    o, ls = _attention(qkv.double(), text_mask, nseq, l, lt, heads, p, seed)
     ctx.copy_(o)
     if lse is not None:
         lse.copy_(ls)
 
 
 def attention_bwd(qkv, text_mask, ctx, dctx, lse, dqkv, nseq, l, lt, heads, p, seed):
-    _no_dropout(p)
     x = qkv.to(F32).clone().requires_grad_(True)
     with torch.enable_grad():
-        o, _ = _attention(x, text_mask, nseq, l, lt, heads)
+        o, _ = _attention(x, text_mask, nseq, l, lt, heads, p, seed)
         o.backward(dctx.to(F32))
     dqkv.copy_(x.grad)
 
@@ -247,8 +267,8 @@ def colsum(x, out, m, n, ld=None):
 
 
 def dropout(x, y, p, seed):
-    _no_dropout(p)
-    y.copy_(x)
+    mult = _drop_mult(p, seed, D.flat_index(x.numel()))
+    y.copy_(x if mult is None else (x.to(F32).reshape(-1) * mult).view(x.shape))
 
 
 def gelu_bwd(dy, u, dx):
@@ -445,7 +465,7 @@ def cast_bf16_f32(src, dst):
 
 
 def dropout_offset_bind(word):
-    """cb_dropout_offset_bind: process-wide device word folded into the dropout seeds (the emulator draws no masks)."""
+    """cb_dropout_offset_bind: process-wide device word folded into the seeds of the masks drawn afterwards."""
     global BOUND_DROPOUT_WORD
     BOUND_DROPOUT_WORD = word
 

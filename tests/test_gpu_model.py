@@ -3,7 +3,7 @@
 Forward: per stage and end to end, against BOTH the plain fp32 oracle and the bf16-rounding-matched
 oracle (oracle.clipbert_ref.Rounding.bf16). Backward: every trainable parameter gradient and the
 gradient flowing into the CNN, against fp32 autograd on the oracle. Dropout is off (eval-mode
-probabilities, p = 0) because the RNGs differ; dropout consistency is covered in test_gpu_ops.py.
+probabilities, p = 0); training with dropout on is compared with the oracle under the same masks in test_gpu_dropout.py.
 """
 import pytest
 import torch

@@ -6,6 +6,7 @@ regression shows up in the CPU suite; the kernels themselves are only ever check
 import pytest
 import torch
 
+import test_gpu_dropout as GD
 import test_gpu_model as G
 import test_gpu_optim as GO
 from ops_emulator import emulated_ops
@@ -35,6 +36,16 @@ def test_gpu_model_test_body_on_emulated_ops(weights, name, kw):
     with emulated_ops() as calls:
         getattr(G, name)(cuda=CPU, weights=weights, **kw)
     assert calls["gemm"] > 0
+
+
+@pytest.mark.parametrize("case", GD.MODEL_CASES, ids=["L41", "L69-ragged"])
+def test_dropout_training_step_on_emulated_ops(weights, case):
+    """tests/test_gpu_dropout.py's model-level body on CPU: the emulator draws the restated masks at the seeds and device word
+    the model passes to each launch, so a wrong seed in modeling.py (a LayerNorm backward regenerating another site's mask, a
+    forgotten word binding) fails here on any machine."""
+    with emulated_ops() as calls:
+        GD.test_transformer_training_step_with_dropout(cuda=CPU, weights=weights, case=case)
+    assert calls["attention_bwd"] == 12 and calls["dropout"] == 1
 
 
 def test_fused_adamw_gpu_test_body_on_emulated_ops():
