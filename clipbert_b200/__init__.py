@@ -6,5 +6,5 @@ host-side mirrors of the reference module interface (``ClipBert``, ``GridFeatBac
 """
 from .e2e_model import ClipBert, clip_lse_loss, clip_pool_loss  # noqa: F401
 from .grid_feat import GridFeatBackbone  # noqa: F401
-from .modeling import (ClipBertForMultipleChoice, ClipBertForPreTraining, ClipBertForRegression,  # noqa: F401
+from .modeling import (ClipBertBaseModel, ClipBertForMultipleChoice, ClipBertForPreTraining, ClipBertForRegression,  # noqa: F401
                        ClipBertForSequenceClassification, ClipBertForVideoTextRetrieval)

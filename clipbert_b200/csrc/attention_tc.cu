@@ -751,6 +751,92 @@ __global__ void __launch_bounds__(TC_THREADS) attn_tc_bwd_q_kernel(const __nv_bf
   tc_store_tile(Qs, dq + (row0 + q0) * ld_dqkv + h * 64, ld_dqkv, L - q0);
 }
 
+// ------------------------------------------------------------------------------------------------ probabilities
+// attention_probs of BertSelfAttention (transformers.py:257-285), written to memory for output_attentions: P[i, j] =
+// exp(S[i, j] - lse[i]) x dropout multiplier, from the log-sum-exp the forward saved (the P the backward kernels rebuild in
+// tc_p_ds). One CTA = 64 query rows of one (sequence, head); per 64-key tile each warp forms S for its 16 rows on mma.sync.
+// The kernel is bound by the bytes it writes (4 l^2 per (sequence, head)): each key tile is staged in shared memory as fp32
+// and written out as 16-byte vectors. The output rows of a CTA are one contiguous run of memory, but a row segment starts at
+// any 4-byte alignment (l is odd at 224 px), so each staged row is shifted by (its global element index) & 3: the aligned
+// 16-byte groups of the segment are then aligned in shared memory too, and only the up to three elements at either end of a
+// segment go out as scalar stores. Streaming stores (st.global.cs): P is written once and read by the host, not by a kernel.
+constexpr int PR_LD = 72;                 // fp32 elements per staged row: 64 keys + up to 3 of shift, 16-byte aligned rows
+
+__global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                                   int64_t ld_qkv, const int64_t* __restrict__ text_mask,
+                                                                   const float* __restrict__ lse, float* __restrict__ probs, int L, int Lt,
+                                                                   int H, float scale, TcDrop dc_in) {
+  pdl_wait();
+  const TcDrop dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
+  pdl_trigger();
+  extern __shared__ __align__(16) uint8_t tc_smem[];
+  __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(tc_smem);
+  __nv_bfloat16* Ks = Qs + TC_TILE;
+  float* Ps = reinterpret_cast<float*>(Ks + TC_TILE);       // [64][PR_LD] staged probabilities of one key tile
+  float* madd = Ps + 64 * PR_LD;
+  float* lses = madd + 64;
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = qb * 64;
+  const int nq = min(64, L - q0);
+  const int64_t row0 = static_cast<int64_t>(b) * L;
+  const uint64_t prow0 = (static_cast<uint64_t>(b) * H + h) * L + q0;   // row index of query q0 in probs viewed as [nseq*H*L, L]
+  const bool live = warp < tc_live_slabs(nq);                          // this warp holds at least one query row < L
+  tc_load_tile(Qs, q + (row0 + q0) * ld_qkv + h * 64, ld_qkv, nq);
+  if (threadIdx.x < 64) lses[threadIdx.x] = threadIdx.x < nq ? lse[prow0 + threadIdx.x] : 0.f;
+  const int r0 = warp * 16;
+  const int rq = r0 + (lane >> 2), cq = 2 * (lane & 3);
+  const int nkb = (L + 63) / 64;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int k0 = kb * 64, nk = min(64, L - k0);
+    __syncthreads();                     // the previous tile has been written out: Ks, Ps and the mask are free
+    tc_load_tile(Ks, k + (row0 + k0) * ld_qkv + h * 64, ld_qkv, nk);
+    tc_key_mask(madd, text_mask, b, k0, L, Lt);
+    __syncthreads();
+    if (live) {
+      float s[8][4];
+      tc_mm_abt_live(s, Qs, Ks, r0, lane, tc_live_slabs(nk));
+      const float l0 = lses[rq], l1 = lses[rq + 8];
+      const uint64_t e0 = (prow0 + rq) * L + k0, e1 = e0 + static_cast<uint64_t>(8) * L;   // element index of (row, k0)
+      float* d0 = Ps + rq * PR_LD + static_cast<int>(e0 & 3) + cq;
+      float* d1 = Ps + (rq + 8) * PR_LD + static_cast<int>(e1 & 3) + cq;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float m0 = madd[j * 8 + cq], m1 = madd[j * 8 + cq + 1];
+        float p0 = __expf(s[j][0] * scale + m0 - l0), p1 = __expf(s[j][1] * scale + m1 - l0);
+        float p2 = __expf(s[j][2] * scale + m0 - l1), p3 = __expf(s[j][3] * scale + m1 - l1);
+        if (dc.thresh) {
+          float r_0, r_1, r_2, r_3;
+          dropout_mult2(dc.seed, e0 + j * 8 + cq, dc.thresh, dc.inv_keep, r_0, r_1);
+          dropout_mult2(dc.seed, e1 + j * 8 + cq, dc.thresh, dc.inv_keep, r_2, r_3);
+          p0 *= r_0; p1 *= r_1; p2 *= r_2; p3 *= r_3;
+        }
+        d0[j * 8] = p0; d0[j * 8 + 1] = p1;
+        d1[j * 8] = p2; d1[j * 8 + 1] = p3;
+      }
+    }
+    __syncthreads();
+    // 16 threads per row, 8 rows per pass; rows >= nq and keys >= nk are never written
+    for (int r = threadIdx.x >> 4; r < nq; r += TC_THREADS / 16) {
+      const uint64_t e = (prow0 + r) * L + k0;
+      const int sh = static_cast<int>(e & 3), end = sh + nk;
+      float* dst = probs + (e - sh);     // 16-byte aligned
+      const float* src = Ps + r * PR_LD;
+      for (int c = (threadIdx.x & 15) * 4; c < end; c += 64) {
+        const float4 v = *reinterpret_cast<const float4*>(src + c);
+        if (c >= sh && c + 4 <= end) {
+          __stcs(reinterpret_cast<float4*>(dst + c), v);
+        } else {
+          const float w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            if (c + i >= sh && c + i < end) __stcs(dst + c + i, w[i]);
+        }
+      }
+    }
+  }
+}
+
 static TcDrop make_tc_drop(float p, uint64_t seed) { return make_drop(p, seed); }
 
 // called from cb_attention_fwd / cb_attention_bwd (attention.cu) when l <= 64
@@ -869,3 +955,20 @@ int attention_tc_bwd_long(const void* qkv, int64_t ld_qkv, const int64_t* text_m
 }
 
 }  // namespace cb
+
+extern "C" int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, float* probs, int nseq, int l,
+                                  int lt, int heads, int head_dim, float dropout_p, uint64_t seed, void* stream) {
+  using namespace cb;
+  CB_REQUIRE(head_dim == 64, "cb_attention_probs: head_dim %d unsupported (built for 64)", head_dim);
+  CB_REQUIRE(qkv && text_mask && lse && probs && nseq > 0 && l > 0 && lt >= 0 && lt <= l && heads > 0 && nseq <= 65535 && heads <= 65535,
+             "cb_attention_probs: bad arguments");
+  CB_REQUIRE(ld_qkv % 8 == 0 && ld_qkv >= 3 * heads * 64, "cb_attention_probs: qkv row pitch must be a multiple of 8 and hold Q | K | V");
+  CB_REQUIRE(reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(probs) % 16 == 0,
+             "cb_attention_probs: qkv and probs must be 16-byte aligned");
+  const int smem = 2 * TC_TILE * 2 + (64 * PR_LD + 2 * 64) * 4;   // Q, K tiles (bf16) + staged P, key mask, lse (fp32): 37 KB
+  const __nv_bfloat16* base = static_cast<const __nv_bfloat16*>(qkv);
+  const int hid = heads * 64;
+  launch_k(attn_tc_probs_kernel, dim3(ceil_div(l, 64), heads, nseq), TC_THREADS, smem, static_cast<cudaStream_t>(stream), base, base + hid,
+           ld_qkv, text_mask, lse, probs, l, lt, heads, 0.125f, make_tc_drop(dropout_p, seed));
+  return check_launch("cb_attention_probs");
+}

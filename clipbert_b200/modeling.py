@@ -115,13 +115,42 @@ class BertPooler(nn.Module):
 
 
 class ClipBertBaseModel(nn.Module):
-    def __init__(self, config):
+    """src/modeling/modeling.py:156-238: embeddings + 12 BertLayers + pooler, the building block every head calls as
+    ``self.bert(...)``.
+
+    ``forward(text_input_ids, visual_inputs, attention_mask)`` returns ``(sequence_output, pooled_output)``, then
+    ``(all_hidden_states,)`` and ``(all_attentions,)`` when ``config.output_hidden_states`` / ``config.output_attentions``
+    are set (read at construction, as BertEncoder does; missing = False). ``visual_inputs`` is (B', T, h, w, 768) with one
+    row per text example (repeat_tensor_rows already applied).
+
+    Inside a head (``head.bert``) the call runs the head's engine: the parameters are views into the head's flat storage and
+    their gradients land in its flat gradient buffer. Constructed on its own, the model gets an engine and flat storage of
+    its own and initialises its weights as BertPreTrainedModel.init_weights does.
+
+    Dtypes: sequence_output, pooled_output and the 13 hidden states are bf16 - the engine's own activation buffers, no copy
+    (the reference's amp-O2 runs hand out fp16 here). The attentions are fp32 (B', heads, L, L), one per layer, the
+    post-dropout probabilities. Autograd flows from sequence_output, pooled_output and every hidden state into every
+    parameter and into ``visual_inputs``; the attention probabilities are returned non-differentiable, the one departure
+    from the reference (whose attentions are ordinary autograd tensors).
+    """
+
+    def __init__(self, config, _engine=None):
         super().__init__()
         self.config = config
         self.embeddings = BertEmbeddings(config)
         self.visual_embeddings = VisualInputEmbedding(config)
         self.encoder = BertEncoder(config)
         self.pooler = BertPooler(config)
+        self.output_hidden_states = bool(_cfg(config, "output_hidden_states", False))
+        self.output_attentions = bool(_cfg(config, "output_attentions", False))
+        if _engine is None:
+            _init_bert_weights(self, _cfg(config, "initializer_range", 0.02))
+            _engine = _BaseModelEngine(config, self)
+        # a back-reference, not a submodule: state_dict keys stay the reference's, and a head keeps one flat storage
+        self.__dict__["_engine"] = _engine
+
+    def forward(self, text_input_ids, visual_inputs, attention_mask):
+        return self._engine._run_base(text_input_ids, visual_inputs, attention_mask, self.output_hidden_states, self.output_attentions)
 
 
 def _require_cuda(t):
@@ -170,19 +199,41 @@ class _TransformerFn(torch.autograd.Function):
         stash, ctx.stash = ctx.stash, None
         m = ctx.module
         dgrid = m._backward_impl(stash, douts if len(douts) > 1 else douts[0], ctx.grid_needs_grad)
-        m._pending_backward = max(0, m._pending_backward - 1)
-        if m._pending_backward == 0 and m._grad_ready_hook is not None:
-            m._grad_ready_hook(m._flat.grad)          # every clip's contribution is in: the exchange may start
+        m._backward_done()
+        return None, dgrid, None, None, None, None
+
+
+class _BaseModelFn(torch.autograd.Function):
+    """ClipBertBaseModel.forward as one autograd node: outputs (sequence_output, pooled_output, *hidden_states, *attentions)."""
+
+    @staticmethod
+    def forward(ctx, module, grid, anchor, ids, mask, flags):
+        (seq, pooled, hidden, attn), stash = module._forward_impl(ids, grid, mask, (1, None, None), need_backward=True, base=flags)
+        module._pending_backward += 1
+        ctx.module, ctx.stash = module, stash
+        ctx.grid_needs_grad = grid.requires_grad
+        ctx.n_hidden = len(hidden)
+        ctx.mark_non_differentiable(*attn)
+        ctx.set_materialize_grads(False)        # unused outputs arrive as None and cost nothing in the backward
+        return (seq, pooled) + tuple(hidden) + tuple(attn)
+
+    @staticmethod
+    def backward(ctx, dseq, dpooled, *rest):
+        stash, ctx.stash = ctx.stash, None
+        m = ctx.module
+        stash["base_grads"] = (dseq, dpooled, rest[:ctx.n_hidden])
+        dgrid = m._backward_impl(stash, None, ctx.grid_needs_grad)
+        m._backward_done()
         return None, dgrid, None, None, None, None
 
 
 class _ClipBertHeadModel(nn.Module):
     """Shared engine: ClipBertBaseModel + an MLP head; subclasses set the head and the loss."""
 
-    def __init__(self, config):
+    def __init__(self, config, bert=None):
         super().__init__()
         self.config = config
-        self.bert = ClipBertBaseModel(config)
+        self.bert = ClipBertBaseModel(config, _engine=self) if bert is None else bert
         self.dropout = nn.Dropout(_cfg(config, "hidden_dropout_prob"))
         self._flat = None
         self._dirty = True
@@ -364,26 +415,57 @@ class _ClipBertHeadModel(nn.Module):
             return _TransformerFn.apply(self, grid, anchor, ids, mask, repeat)
         return self._forward_impl(ids, grid, mask, repeat, need_backward=False)[0]
 
+    def _run_base(self, text_input_ids, visual_inputs, attention_mask, want_hidden, want_attn):
+        """ClipBertBaseModel.forward on this engine (the head itself is not run). visual_inputs: (B', T, h, w, 768)."""
+        _require_cuda(text_input_ids)
+        self._ensure_ready(text_input_ids.device)
+        assert visual_inputs.shape[0] == text_input_ids.shape[0], "visual_inputs must have one row per text example"
+        grid = visual_inputs if visual_inputs.dtype == torch.bfloat16 else visual_inputs.to(torch.bfloat16)
+        grid = grid.contiguous()
+        ids = text_input_ids.contiguous()
+        mask = attention_mask.to(torch.int64).contiguous()
+        flags = (bool(want_hidden), bool(want_attn))
+        if torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters())):
+            outs = _BaseModelFn.apply(self, grid, self.bert.pooler.dense.weight, ids, mask, flags)
+            n_hidden = len(self.bert.encoder.layer) + 1 if flags[0] else 0
+            seq, pooled, hidden, attn = outs[0], outs[1], outs[2:2 + n_hidden], outs[2 + n_hidden:]
+        else:
+            seq, pooled, hidden, attn = self._forward_impl(ids, grid, mask, (1, None, None), need_backward=False, base=flags)[0]
+        out = (seq, pooled)
+        if flags[0]:
+            out = out + (tuple(hidden),)
+        if flags[1]:
+            out = out + (tuple(attn),)
+        return out
+
+    def _backward_done(self):
+        self._pending_backward = max(0, self._pending_backward - 1)
+        if self._pending_backward == 0 and self._grad_ready_hook is not None:
+            self._grad_ready_hook(self._flat.grad)          # every clip's contribution is in: the exchange may start
+
     def _gemm_fwd(self, x, m, li, out, **kw):
         ops.gemm(mode=ops.CB_GEMM_TN, m=m, n=li.n, k=li.k, a=x, a_rows=m, a_ld=kw.pop("a_ld", li.k), b=li.w, b_rows=li.n, b_ld=li.k,
                  shift=li.b, out=out, out_ld=li.n, **kw)
 
-    def _forward_impl(self, ids, grid, mask, repeat, need_backward):
+    def _forward_impl(self, ids, grid, mask, repeat, need_backward, base=None):
         """Binds the per-call dropout word for the duration of the pass and unbinds it on the way out: the binding is process-wide
         state of the library, and a word that outlives its tensor would be a dangling device pointer for every later launch that
         draws masks (found by the autotuner: cb_gemm launches with dropout after the recording step's tensors had been freed)."""
         try:
-            return self._forward_body(ids, grid, mask, repeat, need_backward)
+            return self._forward_body(ids, grid, mask, repeat, need_backward, base)
         finally:
             ops.dropout_offset_bind(None)
 
-    def _forward_body(self, ids, grid, mask, repeat, need_backward):
+    def _forward_body(self, ids, grid, mask, repeat, need_backward, base=None):
+        """base = None: the head's forward, returns its outputs. base = (want_hidden, want_attn): ClipBertBaseModel.forward,
+        returns (sequence_output, pooled_output, hidden_states, attentions) without running the head."""
         dev = ids.device
         cfg = self.config
         H = _cfg(cfg, "hidden_size")
         heads = _cfg(cfg, "num_attention_heads")
         eps = float(_cfg(cfg, "layer_norm_eps"))
-        train = self.training
+        want_hidden, want_attn = base if base is not None else (False, False)
+        train = self.bert.training if base is not None else self.training
         p_h = float(_cfg(cfg, "hidden_dropout_prob")) if train else 0.0
         p_a = float(_cfg(cfg, "attention_probs_dropout_prob")) if train else 0.0
         seed = self._next_seed()
@@ -430,18 +512,25 @@ class _ClipBertHeadModel(nn.Module):
         if self._capture is not None:
             self._capture["embeddings"] = x.view(nseq, L, H).clone()
         # ---- encoder ----
+        hidden, attn = [], []
         for i in range(len(self.bert.encoder.layer)):
             ls = seed + 16 * (i + 1)
             if self._inject is not None and i in self._inject:      # test hook: layer-local parity (same input on both sides)
                 x = self._inject[i].to(device=dev, dtype=bf16).reshape(M, H).contiguous()
+            if want_hidden:
+                hidden.append(x.view(nseq, L, H))
             qkv_l, ao_l, in_l, out_l = (self._lin["l%d.%s" % (i, k)] for k in ("qkv", "ao", "inter", "out"))
             g1, b1, _, _ = self._ln("l%d.ln1" % i)
             g2, b2, _, _ = self._ln("l%d.ln2" % i)
             qkv = new(M, 3 * H)
             self._gemm_fwd(x, M, qkv_l, qkv)
             ctx = new(M, H)
-            lse = new(nseq, heads, L, dtype=f32) if need_backward else None
+            lse = new(nseq, heads, L, dtype=f32) if (need_backward or want_attn) else None
             ops.attention_fwd(qkv, mask, ctx, lse, nseq, L, lt, heads, p_a, ls + 1)
+            if want_attn:       # same seed and bound word as the forward: the probabilities its context was made from
+                probs = new(nseq, heads, L, L, dtype=f32)
+                ops.attention_probs(qkv, mask, lse, probs, nseq, L, lt, heads, p_a, ls + 1)
+                attn.append(probs)
             s1 = new(M, H)
             self._gemm_fwd(ctx, M, ao_l, s1, residual=x, res_ld=H, dropout_p=p_h, dropout_seed=ls + 2)
             a = new(M, H)
@@ -472,7 +561,12 @@ class _ClipBertHeadModel(nn.Module):
         st["pooled"] = pooled
         if self._capture is not None:
             self._capture["pooled"] = pooled
-        out = self._head_forward(pooled, st, nseq, p_h, seed, need_backward)
+        if base is not None:
+            if want_hidden:
+                hidden.append(x.view(nseq, L, H))
+            out = (x.view(nseq, L, H), pooled, hidden, attn)
+        else:
+            out = self._head_forward(pooled, st, nseq, p_h, seed, need_backward)
         return out, (st if need_backward else None)
 
     # generic 2-layer MLP head: dropout -> Linear -> ReLU -> Linear (modeling.py:534-539,552-553)
@@ -553,17 +647,26 @@ class _ClipBertHeadModel(nn.Module):
 
         ops.dropout_offset_bind(st.get("drop_word"))       # regenerate exactly this forward's masks
         sq = ops.SideQueue()                               # wgrad GEMMs / bias sums run beside the dgrad chain
-        dpre = self._head_backward(st, dout, nseq, H)      # grad w.r.t. pooler pre-activation
+        base = st.get("base_grads")                        # ClipBertBaseModel.forward: (d sequence, d pooled, d hidden states)
+        dhidden = None
+        if base is None:
+            dpre = self._head_backward(st, dout, nseq, H)  # grad w.r.t. pooler pre-activation
+        else:
+            dpre, dseq, dhidden = self._base_output_grads(st, base, M, H)
         pl = self._lin["pooler"]
         x_last = st["x_last"]
-        self._wgrad(pl, dpre, x_last, nseq, x_ld=L * H)
-        ops.colsum(dpre, pl.gb, nseq, H)
+        if dpre is not None:
+            self._wgrad(pl, dpre, x_last, nseq, x_ld=L * H)
+            ops.colsum(dpre, pl.gb, nseq, H)
         dx = torch.zeros(M, H, dtype=bf16, device=dev)
-        self._dgrad(pl, dpre, nseq, dx, out_ld=L * H)      # scatters into the [CLS] rows
-        extra = self._extra_sequence_grad(st)
+        if dpre is not None:
+            self._dgrad(pl, dpre, nseq, dx, out_ld=L * H)  # scatters into the [CLS] rows
+        extra = self._extra_sequence_grad(st) if base is None else dseq
         if extra is not None:
             dx += extra
         for i in reversed(range(len(st["layers"]))):
+            if dhidden is not None and dhidden[i + 1] is not None:     # output of layer i = hidden_states[i + 1]
+                dx += dhidden[i + 1]
             ly = st["layers"][i]
             ls = ly["seed"]
             qkv_l, ao_l, in_l, out_l = (self._lin["l%d.%s" % (i, k)] for k in ("qkv", "ao", "inter", "out"))
@@ -613,6 +716,8 @@ class _ClipBertHeadModel(nn.Module):
             self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
             dx = dxn
             st["layers"][i] = None     # free this layer's stash
+        if dhidden is not None and dhidden[0] is not None:                 # hidden_states[0] = the embedding output
+            dx += dhidden[0]
         # ---- embeddings ----
         g_t, _, dg_t, db_t = self._ln("emb.ln")
         g_v, _, dg_v, db_v = self._ln("vis.ln")
@@ -646,12 +751,39 @@ class _ClipBertHeadModel(nn.Module):
     def _extra_sequence_grad(self, st):
         return None
 
+    def _base_output_grads(self, st, grads, M, H):
+        """Upstream gradients of ClipBertBaseModel.forward -> (d pooler pre-activation or None, dense d sequence_output or None,
+        [d hidden_states[k] or None] or None), all bf16. d pooled goes through tanh' = 1 - pooled^2 (BertPooler,
+        transformers.py:470-476) as the heads' dpre does, here as one product on the (B', 768) rows."""
+        dseq, dpooled, dh = grads
+        bf16 = torch.bfloat16
+
+        def dense(g):
+            return None if g is None else g.reshape(M, H).to(bf16).contiguous()
+
+        dpre = None
+        if dpooled is not None:
+            pooled = st["pooled"].float()
+            dpre = (dpooled.float() * (1.0 - pooled * pooled)).to(bf16)
+        return dpre, dense(dseq), ([dense(g) for g in dh] if dh else None)
+
     # ---- misc -------------------------------------------------------------------------------------
     def zero_grad(self, set_to_none=False):
         if self._flat is not None and self._flat.grad is not None:
             self._flat.zero_grad()
         else:
             super().zero_grad(set_to_none=set_to_none)
+
+
+class _BaseModelEngine(_ClipBertHeadModel):
+    """The engine of a ClipBertBaseModel constructed on its own: flat storage for the base model's parameters, no head. It is
+    reached through the base model's back-reference only, so its own training flag is never read (base passes use bert's)."""
+
+    def __init__(self, config, bert):
+        super().__init__(config, bert=bert)
+
+    def _head_linears(self):
+        return []
 
 
 class _MlpHeadMixin:

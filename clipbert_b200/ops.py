@@ -37,6 +37,7 @@ _SIGS = {
     "cb_cross_entropy_bwd": [_vp, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _i, _i64, _vp],
     "cb_attention_fwd": [_vp, _i64, _vp, _vp, _i64, _vp, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_attention_bwd": [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
+    "cb_attention_probs": [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_stem_im2col": [_vp, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp],
     "cb_maxpool3x3s2": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool3x3s2_strided": [_vp, _vp, _i, _i, _i, _i, _i64, _i64, _vp],
@@ -420,6 +421,12 @@ def attention_fwd(qkv, text_mask, ctx, lse, nseq, l, lt, heads, p, seed):
 def attention_bwd(qkv, text_mask, ctx, dctx, lse, dqkv, nseq, l, lt, heads, p, seed):
     _call("cb_attention_bwd", _p(qkv), qkv.shape[1], _p(text_mask), _p(ctx), _p(dctx), ctx.shape[1], _p(lse), _p(dqkv),
           dqkv.shape[1], nseq, l, lt, heads, 64, p, seed, _s())
+
+
+def attention_probs(qkv, text_mask, lse, probs, nseq, l, lt, heads, p, seed):
+    """probs: fp32 [nseq, heads, l, l] contiguous, from the lse cb_attention_fwd wrote for the same arguments."""
+    assert probs.dtype == torch.float32 and probs.is_contiguous() and probs.numel() == nseq * heads * l * l
+    _call("cb_attention_probs", _p(qkv), qkv.shape[1], _p(text_mask), _p(lse), _p(probs), nseq, l, lt, heads, 64, p, seed, _s())
 
 
 # ------------------------------------------------------------------------------------------------

@@ -68,7 +68,7 @@ int cb_set_pdl(int enable);
  *                                  after the row map
  *     cb_layernorm_bwd             row * 768 + col (dx_drop, dbias_drop)
  *     cb_embed_text_* / _visual_*  (seq * l + pos) * 768 + col: text rows at pos = t, visual cell j at pos = lt + j
- *     cb_attention_fwd / _bwd      ((seq * heads + h) * l + i) * l + j for probability P[i, j] of head h */
+ *     cb_attention_fwd / _bwd / _probs  ((seq * heads + h) * l + i) * l + j for probability P[i, j] of head h */
 int cb_dropout_offset_bind(const uint64_t* device_word);
 int cb_dropout_offset_advance(uint64_t* counter, uint64_t* snapshot, void* stream);
 
@@ -224,6 +224,16 @@ int cb_attention_fwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, 
 int cb_attention_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const void* ctx, const void* dctx,
                      int64_t ld_ctx, const float* lse, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads,
                      int head_dim, float dropout_p, uint64_t seed, void* stream);
+/* The attention probabilities themselves, for output_attentions (transformers.py:257-285: the attention_probs returned at
+ * :284, after the dropout of :271): probs fp32 [nseq, heads, l, l], contiguous, 16-byte aligned;
+ *   P[s, h, i, j] = exp(Q_i . K_j / 8 + madd_j - lse[s, h, i]) x dropout multiplier
+ * with madd_j = -10000 for a text key whose mask entry is 0, else 0, and lse what cb_attention_fwd wrote for the same qkv,
+ * mask and l (every forward kernel writes the same convention: max_j + log sum_j exp(S_ij - max_j) over the masked scores).
+ * The mask is the forward's (same seed, same bound device word, element index above), so with dropout_p = 0 each row sums
+ * to 1 and with dropout it is exactly the P the forward multiplied V by. Tensor cores (mma.sync), one CTA per (64-query
+ * tile, head, sequence); rows and columns beyond l are never written. */
+int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, float* probs, int nseq,
+                       int l, int lt, int heads, int head_dim, float dropout_p, uint64_t seed, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Small helpers on the transformer side.
