@@ -34,6 +34,7 @@ class GemmDesc(ctypes.Structure):
         ("rowmap", ctypes.c_int32), ("map_h", ctypes.c_int32), ("map_w", ctypes.c_int32),
         ("dropout_p", ctypes.c_float), ("dropout_seed", ctypes.c_uint64),
         ("block_n", ctypes.c_int32), ("reserved", ctypes.c_int32),
+        ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_int64),
     ]
 
 
@@ -62,6 +63,12 @@ def lib():
     L.cb_gemm.restype = ctypes.c_int
     L.cb_gemm_wgrad_group.argtypes = [ctypes.POINTER(GemmDesc), ctypes.c_int, ctypes.c_void_p]
     L.cb_gemm_wgrad_group.restype = ctypes.c_int
+    L.cb_gemm_workspace_bytes.argtypes = [ctypes.POINTER(GemmDesc)]
+    L.cb_gemm_workspace_bytes.restype = ctypes.c_int64
+    L.cb_gemm_wgrad_group_workspace_bytes.argtypes = [ctypes.POINTER(GemmDesc), ctypes.c_int]
+    L.cb_gemm_wgrad_group_workspace_bytes.restype = ctypes.c_int64
+    L.cb_set_deterministic.argtypes = [ctypes.c_int]
+    L.cb_set_deterministic.restype = ctypes.c_int
     _lib = L
     return L
 

@@ -17,6 +17,7 @@ static int pdl_default() {
   return (e && e[0] == '1') ? 1 : ((e && e[0] == '2') ? 2 : 0);
 }
 std::atomic<int> g_pdl{pdl_default()};
+std::atomic<int> g_det{0};
 static std::atomic<const uint64_t*> g_drop_offset{nullptr};
 const uint64_t* drop_offset_ptr() { return g_drop_offset.load(std::memory_order_relaxed); }
 
@@ -168,6 +169,7 @@ int cb_version(void) { return 100; }
 int cb_sm_arch(void) { return 90; }
 int64_t cb_launch_count(void) { return cb::g_launches.load(std::memory_order_relaxed); }
 int cb_set_pdl(int enable) { return cb::g_pdl.exchange(enable == 2 ? 2 : (enable ? 1 : 0), std::memory_order_relaxed); }
+int cb_set_deterministic(int enable) { return cb::g_det.exchange(enable ? 1 : 0, std::memory_order_relaxed); }
 int cb_dropout_offset_bind(const uint64_t* device_word) {
   cb::g_drop_offset.store(device_word, std::memory_order_relaxed);
   return CB_OK;

@@ -138,6 +138,33 @@ __device__ __forceinline__ void block_accumulate(float (&acc)[CH][8], float* sme
   __syncthreads();
 }
 
+// Deterministic mode: the block's reduced vector (its warps summed in warp order, as above) is stored to its own scratch row
+// `part` instead; ordered_colsum_kernel adds the rows into the destination in a fixed order afterwards.
+__device__ __forceinline__ void block_store(float (&acc)[CH][8], float* smem_buf, float* part, int warp, int lane) {
+  store_row_f32(smem_buf + warp * HID, lane, acc);
+  __syncthreads();
+  for (int i = threadIdx.x * 4; i < HID; i += blockDim.x * 4) {
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int w = 0; w < ROWS_PER_BLOCK; ++w) {
+      const float4 v = *reinterpret_cast<const float4*>(smem_buf + w * HID + i);
+      s.x += v.x, s.y += v.y, s.z += v.z, s.w += v.w;
+    }
+    *reinterpret_cast<float4*>(part + i) = s;
+  }
+  __syncthreads();
+}
+// partial `slot` of this block in a scratch laid out [slot][block][768], blocks numbered x-fastest over the grid
+__device__ __forceinline__ float* part_row(float* part, int slot) {
+  const int nb = gridDim.x * gridDim.y, b = blockIdx.y * gridDim.x + blockIdx.x;
+  return part + (static_cast<int64_t>(slot) * nb + b) * HID;
+}
+template <bool DET>
+__device__ __forceinline__ void accumulate(float (&acc)[CH][8], float* smem_buf, float* gdst, float* part, int slot, int warp, int lane) {
+  if constexpr (DET) block_store(acc, smem_buf, part_row(part, slot), warp, lane);
+  else block_accumulate(acc, smem_buf, gdst, warp, lane);
+}
+
 // ------------------------------------------------------------------------------------------------
 // LayerNorm over rows of a [M, 768] bf16 matrix
 // ------------------------------------------------------------------------------------------------
@@ -161,11 +188,13 @@ __global__ void __launch_bounds__(128) ln_fwd_kernel(const __nv_bfloat16* __rest
 }
 
 // grid-stride over rows; per-warp dgamma / dbeta / dbias partials, reduced per block
+template <bool DET>
 __global__ void __launch_bounds__(128) ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
                                                      const __nv_bfloat16* __restrict__ x,
                                                      const float* __restrict__ stats, const float* gamma,
                                                      __nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dx_drop,
-                                                     float* dgamma, float* dbeta, float* dbias_drop, int M, DropCfg dc_in) {
+                                                     float* dgamma, float* dbeta, float* dbias_drop, int M, DropCfg dc_in,
+                                                     float* part) {
   pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
   const DropCfg dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
   pdl_trigger();
@@ -213,9 +242,9 @@ __global__ void __launch_bounds__(128) ln_bwd_kernel(const __nv_bfloat16* __rest
         for (int j = 0; j < 8; ++j) ad[c][j] += __bfloat162float(__float2bfloat16(g[c][j]));
     }
   }
-  if (dgamma) block_accumulate(ag, red, dgamma, warp, lane);
-  if (dbeta) block_accumulate(ab, red, dbeta, warp, lane);
-  if (dbias_drop) block_accumulate(ad, red, dbias_drop, warp, lane);
+  if (dgamma) accumulate<DET>(ag, red, dgamma, part, 0, warp, lane);
+  if (dbeta) accumulate<DET>(ab, red, dbeta, part, 1, warp, lane);
+  if (dbias_drop) accumulate<DET>(ad, red, dbias_drop, part, 2, warp, lane);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -257,12 +286,15 @@ __global__ void __launch_bounds__(128) embed_text_fwd_kernel(const int64_t* __re
 // grid = (blocks per position, Lt): every block works on ONE text position t, so the position-embedding gradient is summed in
 // registers / shared memory and leaves the block as 768 atomics (it was one atomic per element per row: 64-way contention on the
 // Lt rows of dpos made this kernel 82 us at 64 sequences); the word rows go out as 16-byte reductions.
+// DET: the parameter partials go to scratch (slots dgamma, dbeta, d type/pos) and row r's word gradient to drows[r] (fp32), which
+// word_scatter_ordered_kernel adds into the table afterwards.
+template <bool DET>
 __global__ void __launch_bounds__(128) embed_text_bwd_kernel(const __nv_bfloat16* __restrict__ dh,
                                                              const int64_t* __restrict__ ids, const float* word,
                                                              const float* pos, const float* type0, const float* gamma,
                                                              const float* __restrict__ stats, float* dword, float* dpos,
                                                              float* dtype0, float* dgamma, float* dbeta, int nseq, int Lt,
-                                                             int L, int vocab, DropCfg dc_in) {
+                                                             int L, int vocab, DropCfg dc_in, float* part, float* drows) {
   pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
   const DropCfg dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
   pdl_trigger();
@@ -310,15 +342,50 @@ __global__ void __launch_bounds__(128) embed_text_bwd_kernel(const __nv_bfloat16
         ag[c][j] += gsave[c][j] * e[c][j];
         at[c][j] += g[c][j];
       }
-      float* wrow = dword + id * HID + c * 256 + lane * 8;
-      red_add_f32x4(wrow, make_float4(g[c][0], g[c][1], g[c][2], g[c][3]));
-      red_add_f32x4(wrow + 4, make_float4(g[c][4], g[c][5], g[c][6], g[c][7]));
+      if constexpr (!DET) {
+        float* wrow = dword + id * HID + c * 256 + lane * 8;
+        red_add_f32x4(wrow, make_float4(g[c][0], g[c][1], g[c][2], g[c][3]));
+        red_add_f32x4(wrow + 4, make_float4(g[c][4], g[c][5], g[c][6], g[c][7]));
+      }
     }
+    if constexpr (DET) store_row_f32(drows + r * HID, lane, g);
   }
-  block_accumulate(ag, red, dgamma, warp, lane);
-  block_accumulate(ab, red, dbeta, warp, lane);
-  block_accumulate(at, red, dtype0, warp, lane);
-  block_accumulate(at, red, dpos + static_cast<int64_t>(t) * HID, warp, lane);      // d pos[t] = d type[0] restricted to this position
+  if constexpr (DET) {      // one partial of d type[0] serves d type[0] and d pos[t] (see ordered reduction in cb_embed_text_bwd_det)
+    block_store(ag, red, part_row(part, 0), warp, lane);
+    block_store(ab, red, part_row(part, 1), warp, lane);
+    block_store(at, red, part_row(part, 2), warp, lane);
+  } else {
+    block_accumulate(ag, red, dgamma, warp, lane);
+    block_accumulate(ab, red, dbeta, warp, lane);
+    block_accumulate(at, red, dtype0, warp, lane);
+    block_accumulate(at, red, dpos + static_cast<int64_t>(t) * HID, warp, lane);      // d pos[t] = d type[0] restricted to this position
+  }
+}
+
+// Deterministic word-table scatter: the block of row r returns unless r is the FIRST row carrying its (clamped) token id; that
+// block sums the fp32 rows drows[r'] of every row r' >= r with the same id in row order and adds the sum to dword[id]. So every
+// table row has one writer and one summation order, whatever the schedule.
+__global__ void __launch_bounds__(HID / 4) word_scatter_ordered_kernel(const int64_t* __restrict__ ids, const float* __restrict__ drows,
+                                                                        float* dword, int R, int vocab) {
+  pdl_wait();
+  pdl_trigger();
+  const int r = blockIdx.x;
+  auto clamp_id = [vocab](int64_t id) { return id < 0 ? 0 : (id >= vocab ? static_cast<int64_t>(vocab - 1) : id); };
+  const int64_t id = clamp_id(ids[r]);
+  int seen = 0;
+  for (int q = threadIdx.x; q < r; q += blockDim.x) seen |= clamp_id(ids[q]) == id;
+  if (__syncthreads_or(seen)) return;
+  const int c = threadIdx.x * 4;
+  float4 s = *reinterpret_cast<const float4*>(drows + static_cast<int64_t>(r) * HID + c);
+  for (int q = r + 1; q < R; ++q) {
+    if (clamp_id(ids[q]) != id) continue;
+    const float4 v = *reinterpret_cast<const float4*>(drows + static_cast<int64_t>(q) * HID + c);
+    s.x += v.x, s.y += v.y, s.z += v.z, s.w += v.w;
+  }
+  float4* o = reinterpret_cast<float4*>(dword + id * HID + c);
+  float4 d = *o;
+  d.x += s.x, d.y += s.y, d.z += s.z, d.w += s.w;
+  *o = d;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -374,7 +441,8 @@ __global__ void __launch_bounds__(128) embed_visual_fwd_kernel(const __nv_bfloat
   }
 }
 
-// pass 1: LN backward per (b', j); writes dv (fp32) to tmp and accumulates parameter gradients
+// pass 1: LN backward per (b', j); writes dv (fp32) to tmp and accumulates parameter gradients (DET: stores their partials)
+template <bool DET>
 __global__ void __launch_bounds__(128) embed_visual_bwd_kernel(const __nv_bfloat16* __restrict__ dh,
                                                                const __nv_bfloat16* __restrict__ grid,
                                                                const int32_t* __restrict__ seq2vid, int n_ex,
@@ -383,7 +451,7 @@ __global__ void __launch_bounds__(128) embed_visual_bwd_kernel(const __nv_bfloat
                                                                const float* __restrict__ stats, float* __restrict__ dv_tmp,
                                                                float* drow, float* dcol, float* dtype0, float* dgamma,
                                                                float* dbeta, int nseq, int T, int gh, int gw, int Lt, int L,
-                                                               DropCfg dc_in) {
+                                                               DropCfg dc_in, float* part) {
   pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
   const DropCfg dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
   pdl_trigger();
@@ -443,11 +511,17 @@ __global__ void __launch_bounds__(128) embed_visual_bwd_kernel(const __nv_bfloat
         at[c][q] += g[c][q];
       }
   }
-  block_accumulate(ag, red, dgamma, warp, lane);
-  block_accumulate(ab, red, dbeta, warp, lane);
-  block_accumulate(at, red, dtype0, warp, lane);
-  block_accumulate(at, red, drow + static_cast<int64_t>(j / gw) * HID, warp, lane);
-  block_accumulate(at, red, dcol + static_cast<int64_t>(j % gw) * HID, warp, lane);
+  if constexpr (DET) {
+    block_store(ag, red, part_row(part, 0), warp, lane);
+    block_store(ab, red, part_row(part, 1), warp, lane);
+    block_store(at, red, part_row(part, 2), warp, lane);
+  } else {
+    block_accumulate(ag, red, dgamma, warp, lane);
+    block_accumulate(ab, red, dbeta, warp, lane);
+    block_accumulate(at, red, dtype0, warp, lane);
+    block_accumulate(at, red, drow + static_cast<int64_t>(j / gw) * HID, warp, lane);
+    block_accumulate(at, red, dcol + static_cast<int64_t>(j % gw) * HID, warp, lane);
+  }
 }
 
 // pass 2: dgrid[vid, t, j] = (1/T) * sum_{b' -> vid} dv[b', j]   (backward of repeat_tensor_rows + frame mean)
@@ -488,9 +562,11 @@ __global__ void __launch_bounds__(128) embed_visual_bwd_reduce_kernel(const floa
 // column sums (bias gradients): db[n] += sum_m dY[m, n]
 // ------------------------------------------------------------------------------------------------
 // block = 8 warps x 32 lanes: a lane owns 8 columns (one 128-bit load per row), warps stride the rows of a
-// 128-row slab; partials are combined across warps in smem so that each block issues ONE atomic per column
+// 128-row slab; partials are combined across warps in smem so that each block issues ONE atomic per column (DET: stores the
+// slab's sums to part[slab][n] for ordered_colsum_kernel)
+template <bool DET>
 __global__ void __launch_bounds__(256) colsum_kernel(const __nv_bfloat16* __restrict__ x, int64_t ld, float* __restrict__ out, int M,
-                                                     int N) {
+                                                     int N, float* part) {
   pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
   pdl_trigger();
   __shared__ float red[8][256 + 8];
@@ -518,8 +594,79 @@ __global__ void __launch_bounds__(256) colsum_kernel(const __nv_bfloat16* __rest
     float s = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) s += red[w][c];
-    atomicAdd(out + blockIdx.x * 256 + c, s);
+    if constexpr (DET) part[static_cast<int64_t>(blockIdx.y) * N + blockIdx.x * 256 + c] = s;
+    else atomicAdd(out + blockIdx.x * 256 + c, s);
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// ordered reductions of the deterministic mode
+// ------------------------------------------------------------------------------------------------
+// Job: for every row r < rows and column c < width
+//   dst[r * dst_rs + c] += sum_{a < na} sum_{b < nb} src[r * src_rs + a * sa + b * sb + c]
+// summed into a register starting at 0, a-major then b, one thread per (r, c). The partial rows a kernel stored are thereby
+// added in one fixed order whatever the grid or the schedule.
+struct ColRedJob {
+  float* dst;
+  const float* src;
+  int rows;
+  int64_t dst_rs, src_rs;
+  int na;
+  int64_t sa;
+  int nb;
+  int64_t sb;
+};
+constexpr int COLRED_MAX_JOBS = 5;
+struct ColRed {
+  int width, njobs;
+  ColRedJob j[COLRED_MAX_JOBS];
+};
+__global__ void __launch_bounds__(256) ordered_colsum_kernel(const __grid_constant__ ColRed r) {
+  pdl_wait();
+  pdl_trigger();
+  const ColRedJob& J = r.j[blockIdx.z];
+  const int c = blockIdx.x * 256 + threadIdx.x;
+  if (c >= r.width) return;
+  for (int row = blockIdx.y; row < J.rows; row += gridDim.y) {
+    const float* p = J.src + row * J.src_rs + c;
+    float s = 0.f;
+    for (int a = 0; a < J.na; ++a) {
+#pragma unroll 8
+      for (int b = 0; b < J.nb; ++b) s += p[a * J.sa + b * J.sb];
+    }
+    J.dst[row * J.dst_rs + c] += s;
+  }
+}
+static int launch_ordered_colsum(const ColRed& r, cudaStream_t stream, const char* what) {
+  int rows = 1;
+  for (int i = 0; i < r.njobs; ++i) rows = max(rows, r.j[i].rows);
+  launch_k(ordered_colsum_kernel, dim3(ceil_div(r.width, 256), min(rows, 1024), r.njobs), 256, 0, stream, r);
+  return check_launch(what);
+}
+// job summing `n` consecutive partial rows (stride `stride` floats) into one destination row
+static ColRedJob colred_all(float* dst, const float* src, int n, int64_t stride) { return {dst, src, 1, 0, 0, 1, 0, n, stride}; }
+
+// out[0] += the n partials, in a fixed order: thread t sums part[t], part[t + 256], ... ; then the warps' xor butterflies and the
+// eight warp sums in warp order
+__global__ void __launch_bounds__(256) ordered_sum_kernel(const float* __restrict__ part, int n, float* out) {
+  pdl_wait();
+  pdl_trigger();
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n; i += 256) s += part[i];
+  s = warp_sum(s);
+  __shared__ float w[8];
+  if ((threadIdx.x & 31) == 0) w[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) t += w[k];
+    out[0] += t;
+  }
+}
+int launch_ordered_sum(const float* part, int n, float* out, cudaStream_t stream, const char* what) {
+  launch_k(ordered_sum_kernel, 1, 256, 0, stream, part, n, out);
+  return check_launch(what);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -653,6 +800,18 @@ __global__ void cast_scale_segments_kernel(const float* __restrict__ master, __n
 // ================================================================================================
 using namespace cb;
 
+// deterministic mode: the entry points that accumulate with atomics refuse (never a silent fall-back to an order that depends on
+// the schedule); their _det variants take the scratch of the ordered reductions
+#define CB_REQUIRE_NONDET(name) \
+  CB_REQUIRE(!cb::g_det.load(std::memory_order_relaxed), "%s: deterministic mode is on; call %s_det with its scratch", name, name)
+#define CB_REQUIRE_SCRATCH(name, scratch, bytes, need)                                                                   \
+  CB_REQUIRE((scratch) != nullptr && (bytes) >= (need) && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0,                \
+             "%s: needs a 16-byte aligned scratch of %lld bytes, got %lld", name, static_cast<long long>(need),              \
+             static_cast<long long>((scratch) ? (bytes) : 0))
+
+static int ln_bwd_blocks(int m) { return max(1, min(ceil_div(m, ROWS_PER_BLOCK), 132 * 2)); }   // two CTAs per H100 SM
+static int embed_bwd_per_pos(int nseq) { return max(1, min(ceil_div(nseq, 2 * ROWS_PER_BLOCK), 32)); }   // two (up to five) rows per warp
+
 extern "C" {
 
 int cb_layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats, int m, int hidden,
@@ -669,13 +828,36 @@ int cb_layernorm_bwd(const void* dy, const void* x, const float* stats, const fl
                      uint64_t dropout_seed, void* stream) {
   CB_REQUIRE(hidden == HID, "cb_layernorm_bwd: hidden size %d unsupported", hidden);
   CB_REQUIRE(dy && x && stats && gamma && dx && m > 0, "cb_layernorm_bwd: bad arguments");
+  if (dgamma || dbeta || dbias_drop) CB_REQUIRE_NONDET("cb_layernorm_bwd");
   // the dgamma / dbeta / dbias atomics contend once per block and column: a few rows per warp, not one
-  const int blocks = max(1, min(ceil_div(m, ROWS_PER_BLOCK), 132 * 2));   // two CTAs per H100 SM
-  launch_k(ln_bwd_kernel, blocks, 128, 0, static_cast<cudaStream_t>(stream), 
+  const int blocks = ln_bwd_blocks(m);
+  launch_k(ln_bwd_kernel<false>, blocks, 128, 0, static_cast<cudaStream_t>(stream), 
       static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x), stats, gamma,
       static_cast<__nv_bfloat16*>(dx), static_cast<__nv_bfloat16*>(dx_drop), dgamma, dbeta, dbias_drop, m,
-      make_drop(dropout_p, dropout_seed));
+      make_drop(dropout_p, dropout_seed), static_cast<float*>(nullptr));
   return check_launch("cb_layernorm_bwd");
+}
+
+int64_t cb_layernorm_bwd_scratch_bytes(int m) { return m > 0 ? 3ll * ln_bwd_blocks(m) * HID * 4 : 0; }
+
+int cb_layernorm_bwd_det(const void* dy, const void* x, const float* stats, const float* gamma, void* dx, void* dx_drop,
+                         float* dgamma, float* dbeta, float* dbias_drop, int m, int hidden, float dropout_p,
+                         uint64_t dropout_seed, float* scratch, int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(hidden == HID, "cb_layernorm_bwd_det: hidden size %d unsupported", hidden);
+  CB_REQUIRE(dy && x && stats && gamma && dx && m > 0, "cb_layernorm_bwd_det: bad arguments");
+  CB_REQUIRE_SCRATCH("cb_layernorm_bwd_det", scratch, scratch_bytes, cb_layernorm_bwd_scratch_bytes(m));
+  const int blocks = ln_bwd_blocks(m);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  launch_k(ln_bwd_kernel<true>, blocks, 128, 0, st, static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(x),
+           stats, gamma, static_cast<__nv_bfloat16*>(dx), static_cast<__nv_bfloat16*>(dx_drop), dgamma, dbeta, dbias_drop, m,
+           make_drop(dropout_p, dropout_seed), scratch);
+  int rc = check_launch("cb_layernorm_bwd_det");
+  ColRed r = {HID, 0, {}};
+  float* dst[3] = {dgamma, dbeta, dbias_drop};
+  for (int k = 0; k < 3; ++k)
+    if (dst[k]) r.j[r.njobs++] = colred_all(dst[k], scratch + static_cast<int64_t>(k) * blocks * HID, blocks, HID);
+  if (rc != CB_OK || r.njobs == 0) return rc;
+  return launch_ordered_colsum(r, st, "cb_layernorm_bwd_det(reduce)");
 }
 
 int cb_embed_text_fwd(const int64_t* ids, const float* word, const float* pos, const float* type0, const float* gamma,
@@ -696,11 +878,45 @@ int cb_embed_text_bwd(const void* dh, const int64_t* ids, const float* word, con
   CB_REQUIRE(hidden == HID, "cb_embed_text_bwd: hidden size %d unsupported", hidden);
   CB_REQUIRE(dh && ids && dword && dpos && dtype0 && dgamma && dbeta, "cb_embed_text_bwd: bad arguments");
   CB_REQUIRE(nseq > 0 && lt > 0 && lt <= 65535, "cb_embed_text_bwd: bad sizes");
-  const int per_pos = max(1, min(ceil_div(nseq, 2 * ROWS_PER_BLOCK), 32));      // two (up to five at 640 sequences) rows per warp
-  launch_k(embed_text_bwd_kernel, dim3(per_pos, lt), 128, 0, static_cast<cudaStream_t>(stream), 
+  CB_REQUIRE_NONDET("cb_embed_text_bwd");
+  const int per_pos = embed_bwd_per_pos(nseq);      // two (up to five at 640 sequences) rows per warp
+  launch_k(embed_text_bwd_kernel<false>, dim3(per_pos, lt), 128, 0, static_cast<cudaStream_t>(stream), 
       static_cast<const __nv_bfloat16*>(dh), ids, word, pos, type0, gamma, stats, dword, dpos, dtype0, dgamma, dbeta,
-      nseq, lt, l, vocab, make_drop(dropout_p, seed));
+      nseq, lt, l, vocab, make_drop(dropout_p, seed), static_cast<float*>(nullptr), static_cast<float*>(nullptr));
   return check_launch("cb_embed_text_bwd");
+}
+
+int64_t cb_embed_text_bwd_scratch_bytes(int nseq, int lt) {
+  if (nseq <= 0 || lt <= 0) return 0;
+  return (3ll * embed_bwd_per_pos(nseq) * lt + static_cast<int64_t>(nseq) * lt) * HID * 4;
+}
+
+int cb_embed_text_bwd_det(const void* dh, const int64_t* ids, const float* word, const float* pos, const float* type0,
+                          const float* gamma, const float* stats, float* dword, float* dpos, float* dtype0, float* dgamma,
+                          float* dbeta, int nseq, int lt, int l, int vocab, int hidden, float dropout_p, uint64_t seed,
+                          float* scratch, int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(hidden == HID, "cb_embed_text_bwd_det: hidden size %d unsupported", hidden);
+  CB_REQUIRE(dh && ids && dword && dpos && dtype0 && dgamma && dbeta, "cb_embed_text_bwd_det: bad arguments");
+  CB_REQUIRE(nseq > 0 && lt > 0 && lt <= 65535, "cb_embed_text_bwd_det: bad sizes");
+  CB_REQUIRE_SCRATCH("cb_embed_text_bwd_det", scratch, scratch_bytes, cb_embed_text_bwd_scratch_bytes(nseq, lt));
+  const int per_pos = embed_bwd_per_pos(nseq);
+  const int64_t nb = static_cast<int64_t>(per_pos) * lt;
+  float* drows = scratch + 3 * nb * HID;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  launch_k(embed_text_bwd_kernel<true>, dim3(per_pos, lt), 128, 0, st, static_cast<const __nv_bfloat16*>(dh), ids, word, pos, type0,
+           gamma, stats, dword, dpos, dtype0, dgamma, dbeta, nseq, lt, l, vocab, make_drop(dropout_p, seed), scratch, drows);
+  int rc = check_launch("cb_embed_text_bwd_det");
+  if (rc != CB_OK) return rc;
+  // partial of block (x, t) at slot k: scratch[(k * nb + t * per_pos + x) * 768]. dgamma / dbeta / d type[0]: every block in
+  // block order; d pos[t]: the per_pos blocks of position t in x order.
+  ColRed r = {HID, 4, {colred_all(dgamma, scratch, static_cast<int>(nb), HID), colred_all(dbeta, scratch + nb * HID, static_cast<int>(nb), HID),
+                       colred_all(dtype0, scratch + 2 * nb * HID, static_cast<int>(nb), HID),
+                       {dpos, scratch + 2 * nb * HID, lt, HID, static_cast<int64_t>(per_pos) * HID, 1, 0, per_pos, HID}}};
+  rc = launch_ordered_colsum(r, st, "cb_embed_text_bwd_det(reduce)");
+  if (rc != CB_OK) return rc;
+  launch_k(word_scatter_ordered_kernel, static_cast<int>(static_cast<int64_t>(nseq) * lt), HID / 4, 0, st, ids, drows, dword,
+           nseq * lt, vocab);
+  return check_launch("cb_embed_text_bwd_det(word scatter)");
 }
 
 int cb_embed_visual_fwd(const void* grid, const int32_t* seq2vid, int n_ex, const float* rowemb, const float* colemb,
@@ -726,10 +942,12 @@ int cb_embed_visual_bwd(const void* dh, const void* grid, const int32_t* seq2vid
   CB_REQUIRE((seq2vid && vid_start) || n_ex > 0, "cb_embed_visual_bwd: need seq2vid+vid_start or uniform n_ex");
   const int Lv = gh * gw;
   CB_REQUIRE(Lv <= 65535, "cb_embed_visual_bwd: grid of %d cells unsupported", Lv);
-  const int per_pos = max(1, min(ceil_div(nseq, 2 * ROWS_PER_BLOCK), 32));
-  launch_k(embed_visual_bwd_kernel, dim3(per_pos, Lv), 128, 0, static_cast<cudaStream_t>(stream), 
+  CB_REQUIRE_NONDET("cb_embed_visual_bwd");
+  const int per_pos = embed_bwd_per_pos(nseq);
+  launch_k(embed_visual_bwd_kernel<false>, dim3(per_pos, Lv), 128, 0, static_cast<cudaStream_t>(stream), 
       static_cast<const __nv_bfloat16*>(dh), static_cast<const __nv_bfloat16*>(grid), seq2vid, n_ex, rowemb, colemb,
-      type0, gamma, stats, dv_tmp, drow, dcol, dtype0, dgamma, dbeta, nseq, t, gh, gw, lt, l, make_drop(dropout_p, seed));
+      type0, gamma, stats, dv_tmp, drow, dcol, dtype0, dgamma, dbeta, nseq, t, gh, gw, lt, l, make_drop(dropout_p, seed),
+      static_cast<float*>(nullptr));
   int rc = check_launch("cb_embed_visual_bwd");
   if (rc != CB_OK) return rc;
   if (dgrid) {
@@ -740,11 +958,68 @@ int cb_embed_visual_bwd(const void* dh, const void* grid, const int32_t* seq2vid
   return rc;
 }
 
+int64_t cb_embed_visual_bwd_scratch_bytes(int nseq, int gh, int gw) {
+  if (nseq <= 0 || gh <= 0 || gw <= 0) return 0;
+  return 3ll * embed_bwd_per_pos(nseq) * gh * gw * HID * 4;
+}
+
+int cb_embed_visual_bwd_det(const void* dh, const void* grid, const int32_t* seq2vid, const int32_t* vid_start, int n_ex,
+                            const float* rowemb, const float* colemb, const float* type0, const float* gamma,
+                            const float* stats, float* dv_tmp, void* dgrid, float* drow, float* dcol, float* dtype0,
+                            float* dgamma, float* dbeta, int nseq, int nvid, int t, int gh, int gw, int lt, int l, int hidden,
+                            float dropout_p, uint64_t seed, float* scratch, int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(hidden == HID, "cb_embed_visual_bwd_det: hidden size %d unsupported", hidden);
+  CB_REQUIRE(dh && grid && dv_tmp && drow && dcol && dtype0 && dgamma && dbeta, "cb_embed_visual_bwd_det: bad arguments");
+  CB_REQUIRE((seq2vid && vid_start) || n_ex > 0, "cb_embed_visual_bwd_det: need seq2vid+vid_start or uniform n_ex");
+  CB_REQUIRE(nseq > 0 && t > 0 && gh > 0 && gw > 0, "cb_embed_visual_bwd_det: bad sizes");
+  const int Lv = gh * gw;
+  CB_REQUIRE(Lv <= 65535, "cb_embed_visual_bwd_det: grid of %d cells unsupported", Lv);
+  CB_REQUIRE_SCRATCH("cb_embed_visual_bwd_det", scratch, scratch_bytes, cb_embed_visual_bwd_scratch_bytes(nseq, gh, gw));
+  const int per_pos = embed_bwd_per_pos(nseq);
+  const int64_t nb = static_cast<int64_t>(per_pos) * Lv;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  launch_k(embed_visual_bwd_kernel<true>, dim3(per_pos, Lv), 128, 0, st, static_cast<const __nv_bfloat16*>(dh),
+           static_cast<const __nv_bfloat16*>(grid), seq2vid, n_ex, rowemb, colemb, type0, gamma, stats, dv_tmp, drow, dcol, dtype0,
+           dgamma, dbeta, nseq, t, gh, gw, lt, l, make_drop(dropout_p, seed), scratch);
+  int rc = check_launch("cb_embed_visual_bwd_det");
+  if (rc != CB_OK) return rc;
+  // partial of block (x, cell j = rr * gw + cc) at slot k: scratch[(k * nb + j * per_pos + x) * 768]. dgamma / dbeta / d type[0]:
+  // every block in block order; d row[rr]: cells of row rr in column order, each cell's blocks in x order; d col[cc]: cells of
+  // column cc in row order, each cell's blocks in x order.
+  const float* at = scratch + 2 * nb * HID;
+  const int64_t cell = static_cast<int64_t>(per_pos) * HID;
+  ColRed r = {HID, 5, {colred_all(dgamma, scratch, static_cast<int>(nb), HID), colred_all(dbeta, scratch + nb * HID, static_cast<int>(nb), HID),
+                       colred_all(dtype0, at, static_cast<int>(nb), HID),
+                       {drow, at, gh, HID, gw * cell, gw, cell, per_pos, HID},
+                       {dcol, at, gw, HID, cell, gh, gw * cell, per_pos, HID}}};
+  rc = launch_ordered_colsum(r, st, "cb_embed_visual_bwd_det(reduce)");
+  if (rc != CB_OK || !dgrid) return rc;
+  launch_k(embed_visual_bwd_reduce_kernel, ceil_div(static_cast<int64_t>(nvid) * Lv, ROWS_PER_BLOCK), 128, 0, st, dv_tmp, vid_start, n_ex,
+           static_cast<__nv_bfloat16*>(dgrid), nvid, t, Lv);
+  return check_launch("cb_embed_visual_bwd_det(dgrid)");
+}
+
 int cb_colsum(const void* x, int64_t ld, float* out, int m, int n, void* stream) {
   CB_REQUIRE(x && out && m > 0 && n > 0 && n % 8 == 0 && ld % 8 == 0, "cb_colsum: bad arguments (n, ld must be multiples of 8)");
+  CB_REQUIRE_NONDET("cb_colsum");
   dim3 grid(ceil_div(n, 256), ceil_div(m, 128));
-  launch_k(colsum_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), static_cast<const __nv_bfloat16*>(x), ld, out, m, n);
+  launch_k(colsum_kernel<false>, grid, 256, 0, static_cast<cudaStream_t>(stream), static_cast<const __nv_bfloat16*>(x), ld, out, m, n,
+           static_cast<float*>(nullptr));
   return check_launch("cb_colsum");
+}
+
+int64_t cb_colsum_scratch_bytes(int m, int n) { return m > 0 && n > 0 ? static_cast<int64_t>(ceil_div(m, 128)) * n * 4 : 0; }
+
+int cb_colsum_det(const void* x, int64_t ld, float* out, int m, int n, float* scratch, int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(x && out && m > 0 && n > 0 && n % 8 == 0 && ld % 8 == 0, "cb_colsum_det: bad arguments (n, ld must be multiples of 8)");
+  CB_REQUIRE_SCRATCH("cb_colsum_det", scratch, scratch_bytes, cb_colsum_scratch_bytes(m, n));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int slabs = ceil_div(m, 128);
+  launch_k(colsum_kernel<true>, dim3(ceil_div(n, 256), slabs), 256, 0, st, static_cast<const __nv_bfloat16*>(x), ld, out, m, n, scratch);
+  const int rc = check_launch("cb_colsum_det");
+  if (rc != CB_OK) return rc;
+  ColRed r = {n, 1, {colred_all(out, scratch, slabs, n)}};     // out[c] += slab 0 + slab 1 + ... (in slab order)
+  return launch_ordered_colsum(r, st, "cb_colsum_det(reduce)");
 }
 
 int cb_dropout(const void* x, void* y, int64_t n, float p, uint64_t seed, void* stream) {

@@ -36,6 +36,8 @@
 //   warpgroups that multiply rows 64g .. 64g+63 of one 128 x BN tile (BN up to 256) with wgmma m64nBNk16, hand every ring stage
 //   back as soon as the products that read it have retired (one stage of wgmma stays in flight), then add the tile into the fp32
 //   output with red.global.add.v2.f32 straight from the fragment (four lanes cover 32 contiguous bytes of a row). One CTA per SM.
+#include <algorithm>
+
 #include "common.cuh"
 #include "host_util.h"
 
@@ -408,7 +410,9 @@ __device__ __forceinline__ void mma_tile_pp(float (&acc)[2][BN / 2], uint32_t sm
 // ---- weight-gradient epilogue: out[tap * N + n] of rows m += acc * scale[m], straight from the wgmma fragment ----------------------
 // Fragment layout of m64nNk16 (f32): warp w of the warpgroup holds rows 16w + lane/4 (d[4j], d[4j+1]) and 16w + lane/4 + 8
 // (d[4j+2], d[4j+3]) at columns 8j + 2 (lane % 4) + {0, 1}.
-template <int BN>
+// STORE (deterministic mode, K split): the scaled partial goes to the split's own workspace plane with plain stores instead; the
+// planes are added into out in split order by wgrad_split_reduce_kernel.
+template <int BN, bool STORE = false>
 __device__ __forceinline__ void wgrad_epilogue(const float (&acc)[BN / 2], float* obase, int64_t out_ld, const float* scale, int M, int N, int r0,
                                                int n0, int lane) {
   const int r1 = r0 + 8;
@@ -418,8 +422,13 @@ __device__ __forceinline__ void wgrad_epilogue(const float (&acc)[BN / 2], float
   for (int j = 0; j < BN / 8; ++j) {
     const int n = n0 + j * 8 + 2 * (lane & 3);
     if (n < N) {     // N % 8 == 0: the pair n, n + 1 is inside
-      if (r0 < M) red_add_f32x2(obase + static_cast<int64_t>(r0) * out_ld + n, acc[4 * j] * rs0, acc[4 * j + 1] * rs0);
-      if (r1 < M) red_add_f32x2(obase + static_cast<int64_t>(r1) * out_ld + n, acc[4 * j + 2] * rs1, acc[4 * j + 3] * rs1);
+      if constexpr (STORE) {
+        if (r0 < M) *reinterpret_cast<float2*>(obase + static_cast<int64_t>(r0) * out_ld + n) = make_float2(acc[4 * j] * rs0, acc[4 * j + 1] * rs0);
+        if (r1 < M) *reinterpret_cast<float2*>(obase + static_cast<int64_t>(r1) * out_ld + n) = make_float2(acc[4 * j + 2] * rs1, acc[4 * j + 3] * rs1);
+      } else {
+        if (r0 < M) red_add_f32x2(obase + static_cast<int64_t>(r0) * out_ld + n, acc[4 * j] * rs0, acc[4 * j + 1] * rs0);
+        if (r1 < M) red_add_f32x2(obase + static_cast<int64_t>(r1) * out_ld + n, acc[4 * j + 2] * rs1, acc[4 * j + 3] * rs1);
+      }
     }
   }
 }
@@ -745,10 +754,12 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
 }
 
 // ===================================== WGRAD =====================================
-template <int BN>
+// DET: every tile writes its scaled partial into plane `split` of the workspace ws (fp32 [splits][M][ntaps * N]) with plain
+// stores; the planes are added into out afterwards in split order (deterministic mode with a K-split; unused otherwise).
+template <int BN, bool DET = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K, int ntaps, int tap_w,
-                int tap_sign, int iters_per_split, int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, GemmEpi epi) {
+                int tap_sign, int iters_per_split, int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, GemmEpi epi, float* ws) {
   using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -830,8 +841,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 4);
     mma_tile<BN, 1, 1>(acc, smem0, stage_bytes, KCH, STAGES, t.n_iters, wg, lane, s, ph, full_bar, empty_bar);
     if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 5);
-    wgrad_epilogue<BN>(acc, reinterpret_cast<float*>(epi.out) + static_cast<int64_t>(t.tap) * N, epi.out_ld, epi.scale, M, N,
-                       t.m0 + wrow + (lane >> 2), t.n0, lane);
+    if constexpr (DET)
+      wgrad_epilogue<BN, true>(acc, ws + static_cast<int64_t>(t.it_begin / iters_per_split) * M * ntaps * N + static_cast<int64_t>(t.tap) * N,
+                               static_cast<int64_t>(ntaps) * N, epi.scale, M, N, t.m0 + wrow + (lane >> 2), t.n0, lane);
+    else
+      wgrad_epilogue<BN>(acc, reinterpret_cast<float*>(epi.out) + static_cast<int64_t>(t.tap) * N, epi.out_ld, epi.scale, M, N,
+                         t.m0 + wrow + (lane >> 2), t.n0, lane);
     if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 8);
   }
   if (threadIdx.x == 0) dbg_stamp(epi, 11);
@@ -841,7 +856,7 @@ static int g_sm_limit = 0;    // tuning hook: cap on the persistent grid (0 = ev
                               // all-reduce overlapped with the backward pass) pins some SMs for its whole duration; with the static
                               // round-robin tile schedule the CTAs that cannot be placed run as a second wave. Capping the grid at
                               // the SM count minus the co-resident kernel's CTAs avoids the second wave.
-static int sm_count() {
+static int sm_count_device() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
@@ -849,8 +864,15 @@ static int sm_count() {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     if (n <= 0) n = 132;
   }
+  return n;
+}
+static int sm_count() {
+  const int n = sm_count_device();
   return (g_sm_limit > 0 && g_sm_limit < n) ? g_sm_limit : n;
 }
+// SMs the launch plan (tile width, K-split) is chosen for. In deterministic mode the split decides the summation order, so it
+// depends on the problem shape and the device only, never on the grid cap; the grid itself may still be capped.
+static int plan_sm_count() { return g_det.load(std::memory_order_relaxed) ? sm_count_device() : sm_count(); }
 
 static long long* g_gemm_timeline = nullptr;
 static int g_force_kch = 0;   // tuning hook: chunks per stage (0 = automatic)
@@ -912,15 +934,61 @@ static int epi_in_bytes(const cb_gemm_desc& d, int bn) {
   return d.mode == CB_GEMM_WGRAD ? 0 : ((d.residual != nullptr) + (d.aux != nullptr)) * (bn / 64) * IN_BOX_BYTES;
 }
 
+// K-splits a launch asked for `want` splits of kc k-chunks runs: every split non-empty
+static int real_splits(int kc, int want) {
+  const int sp = want < 1 ? 1 : (want > kc ? kc : want);
+  return ceil_div(kc, ceil_div(kc, sp));
+}
+
+// Deterministic weight gradients with a K-split: out[m, c] += ws[0][m, c] + ws[1][m, c] + ... + ws[S-1][m, c], added one plane
+// at a time into a register copy of out (so the order is the split order whatever the grid), 4 columns per thread.
+struct SplitReduceJob {
+  float* out;
+  const float* ws;            // [S][M][W]
+  int64_t out_ld;
+  int M, W, S;                // W = ntaps * N, a multiple of 8
+};
+struct SplitReduce {
+  int njobs;
+  SplitReduceJob j[8];
+};
+__global__ void __launch_bounds__(256) wgrad_split_reduce_kernel(const __grid_constant__ SplitReduce r) {
+  pdl_wait();
+  pdl_trigger();
+  const SplitReduceJob& J = r.j[blockIdx.y];
+  const int w4 = J.W / 4;
+  const int64_t total = static_cast<int64_t>(J.M) * w4, plane = static_cast<int64_t>(J.M) * J.W;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x; i < total; i += static_cast<int64_t>(gridDim.x) * 256) {
+    const int64_t m = i / w4;
+    const int c = static_cast<int>(i - m * w4) * 4;
+    float4* o = reinterpret_cast<float4*>(J.out + m * J.out_ld + c);
+    float4 v = *o;
+    const float* p = J.ws + m * J.W + c;
+    for (int s = 0; s < J.S; ++s) {
+      const float4 a = *reinterpret_cast<const float4*>(p + s * plane);
+      v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
+    }
+    *o = v;
+  }
+}
+static int launch_split_reduce(const SplitReduce& r, cudaStream_t stream, const char* what) {
+  int64_t most = 0;
+  for (int i = 0; i < r.njobs; ++i) most = std::max(most, static_cast<int64_t>(r.j[i].M) * (r.j[i].W / 4));
+  const int gx = static_cast<int>(std::min<int64_t>(1024, (most + 255) / 256));
+  launch_k(wgrad_split_reduce_kernel, dim3(gx, r.njobs), 256, 0, stream, r);
+  return check_launch(what);
+}
+
 // MODE 0 / 2 (TN / NN): gemm_pingpong_kernel, BN = 64 / 128. MODE 1 (WGRAD): gemm_kernel. One CTA per SM.
-template <int BN, int MODE>
-static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_t stream) {
+template <int BN, int MODE, bool DET = false>
+static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_t stream, float* ws = nullptr) {
   static_assert(MODE == 1 || BN <= 128, "TN / NN: 128 x 64 or 128 x 128 tiles");
+  static_assert(MODE == 1 || !DET, "only the weight gradients have a deterministic instantiation");
   GemmEpi epi = epi_in;
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   auto kern = [] {
-    if constexpr (MODE == 1) return gemm_kernel<BN>;
+    if constexpr (MODE == 1) return gemm_kernel<BN, DET>;
     else return gemm_pingpong_kernel<BN, MODE>;
   }();
   if (!attr_set) {
@@ -955,11 +1023,8 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
            get_tmap_3d_mn(&tb, d.b, d.n, d.b_rows, d.b_ld, BK, BN / 64);
     ok = mn3d || (get_tmap_2d(&ta, d.a, d.m, d.a_rows, d.a_ld, 64, BK) && get_tmap_2d(&tb, d.b, d.n, d.b_rows, d.b_ld, 64, BK));
     const int kc = ceil_div(d.k, BK);
-    int splits = d.split_k < 1 ? 1 : d.split_k;
-    if (splits > kc) splits = kc;
-    iters_per_split = ceil_div(kc, splits);
-    splits = ceil_div(kc, iters_per_split);   // every split is non-empty
-    total *= splits * d.ntaps;
+    iters_per_split = ceil_div(kc, real_splits(kc, d.split_k));
+    total *= real_splits(kc, d.split_k) * d.ntaps;
     kiters = iters_per_split;
   }
   // epilogue inputs (TN / NN): residual / aux [M, N] at the tile's A rows, 128 x 64 boxes; unused map slots carry a copy of ta
@@ -982,7 +1047,7 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
   const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + sp.n_in * in_bytes + sp.epi_bytes + Cfg::BAR_BYTES + 1024;
   if constexpr (MODE == 1)
     launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, iters_per_split,
-                  tiles_m, tiles_n, total, stages, kch, epi);
+                  tiles_m, tiles_n, total, stages, kch, epi, ws);
   else
     launch_gemm_k(kern, grid, PP_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, tiles_m,
                   tiles_n, total, stages, kch, sp.n_in, epi);
@@ -1000,8 +1065,7 @@ struct LaunchCfg {
   int bn, splits;
 };
 
-static LaunchCfg choose_config(const cb_gemm_desc& d) {
-  const int units = sm_count();
+static LaunchCfg choose_config(const cb_gemm_desc& d, int units) {
   const int kc = ceil_div(d.k, BK);
   const bool wgrad = d.mode == CB_GEMM_WGRAD;
   // TN / NN: 128 x 256 would need 256 fp32 accumulators per consumer thread, more than its 232 registers; an explicit
@@ -1072,6 +1136,11 @@ struct WgradGroup {
   int nprob, total_tiles;
   WgradProblem p[WG_MAX_PROBLEMS];
 };
+// DET: problem i's split planes (fp32 [splits][M][ntaps * N]), nullptr when it has one split. A trailing kernel parameter of its
+// own, so that the parameters of the default instantiation keep their offsets.
+struct WgradWorkspace {
+  float* p[WG_MAX_PROBLEMS];
+};
 struct WgTile {
   int pi, m0, n0, tap, it_begin, n_iters;
 };
@@ -1096,9 +1165,9 @@ __device__ __forceinline__ WgTile wg_decode(const WgradGroup& g, int tile) {
   return t;
 }
 
-template <int BN>
+template <int BN, bool DET = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-    wgrad_group_kernel(const __grid_constant__ WgradGroup g, int STAGES, int KCH) {
+    wgrad_group_kernel(const __grid_constant__ WgradGroup g, int STAGES, int KCH, const __grid_constant__ WgradWorkspace ws) {
   using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -1171,15 +1240,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const WgTile t = wg_decode(g, tile);
     const WgradProblem& P = g.p[t.pi];
     mma_tile<BN, 1, 1>(acc, smem0, stage_bytes, KCH, STAGES, t.n_iters, wg, lane, s, ph, full_bar, empty_bar);
-    wgrad_epilogue<BN>(acc, P.out + static_cast<int64_t>(t.tap) * P.N, P.out_ld, P.scale, P.M, P.N, t.m0 + wrow + (lane >> 2), t.n0 * BN, lane);
+    if (DET && ws.p[t.pi] != nullptr)
+      wgrad_epilogue<BN, true>(acc, ws.p[t.pi] + static_cast<int64_t>(t.it_begin / P.iters_per_split) * P.M * P.ntaps * P.N +
+                                        static_cast<int64_t>(t.tap) * P.N,
+                               static_cast<int64_t>(P.ntaps) * P.N, P.scale, P.M, P.N, t.m0 + wrow + (lane >> 2), t.n0 * BN, lane);
+    else
+      wgrad_epilogue<BN>(acc, P.out + static_cast<int64_t>(t.tap) * P.N, P.out_ld, P.scale, P.M, P.N, t.m0 + wrow + (lane >> 2), t.n0 * BN, lane);
   }
 }
 
-template <int BN>
-static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cudaStream_t stream) {
+template <int BN, bool DET = false>
+static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cudaStream_t stream, float* ws = nullptr) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
-  auto kern = wgrad_group_kernel<BN>;
+  auto kern = wgrad_group_kernel<BN, DET>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
@@ -1190,6 +1264,9 @@ static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cuda
   }
   alignas(64) WgradGroup g;
   g.nprob = n;
+  SplitReduce red;
+  red.njobs = 0;
+  WgradWorkspace wsp;
   int total = 0, max_iters = 0;
   for (int i = 0; i < n; ++i) {
     const cb_gemm_desc& d = descs[i];
@@ -1205,9 +1282,14 @@ static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cuda
     P.M = d.m; P.N = d.n; P.K = d.k;
     P.ntaps = d.ntaps; P.tap_w = d.tap_w; P.tap_sign = d.tap_sign;
     const int kc = ceil_div(d.k, BK);
-    int sp = splits < 1 ? 1 : (splits > kc ? kc : splits);
+    const int sp = real_splits(kc, splits);
     P.iters_per_split = ceil_div(kc, sp);
-    sp = ceil_div(kc, P.iters_per_split);
+    wsp.p[i] = nullptr;
+    if (DET && sp > 1) {     // this problem's planes follow the previous problems' in the workspace
+      wsp.p[i] = ws;
+      red.j[red.njobs++] = {static_cast<float*>(d.out), ws, d.out_ld, d.m, d.ntaps * d.n, sp};
+      ws += static_cast<int64_t>(sp) * d.m * d.ntaps * d.n;
+    }
     P.tiles_m = ceil_div(d.m, BM);
     P.tiles_n = ceil_div(d.n, BN);
     P.tile_begin = total;
@@ -1222,8 +1304,61 @@ static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cuda
   }
   const int smem_bytes = sp.stages * sp.kch * Cfg::STAGE_BYTES + Cfg::BAR_BYTES + 1024;
   const int units = sm_count();
-  launch_gemm_k(kern, total < units ? total : units, GEMM_THREADS, smem_bytes, stream, g, sp.stages, sp.kch);
-  return check_launch("cb_gemm_wgrad_group");
+  launch_gemm_k(kern, total < units ? total : units, GEMM_THREADS, smem_bytes, stream, g, sp.stages, sp.kch, wsp);
+  const int rc = check_launch("cb_gemm_wgrad_group");
+  if (rc != CB_OK || red.njobs == 0) return rc;
+  return launch_split_reduce(red, stream, "cb_gemm_wgrad_group(split reduce)");
+}
+
+// Tile width and K-split of a grouped launch (groupable = false: the problems run as separate cb_gemm launches).
+struct GroupPlan {
+  bool groupable;
+  int bn, split;
+};
+static GroupPlan group_plan(const cb_gemm_desc* descs, int n, int sms) {
+  GroupPlan gp = {n >= 2 && n <= WG_MAX_PROBLEMS, 64, 1};
+  // one schedule for all: reduction lengths within 2 x of each other, otherwise the round-robin tiles are unbalanced
+  for (int i = 0; i < n; ++i)
+    if (descs[i].k * 2 < descs[0].k || descs[0].k * 2 < descs[i].k) gp.groupable = false;
+  if (!gp.groupable) return gp;
+  // tile width: the widest that does not mostly pad, unless descs[0].block_n sets it; K-split: descs[0].split_k, or the one with
+  // the least time per CTA
+  int min_n = descs[0].n;
+  for (int i = 1; i < n; ++i) min_n = descs[i].n < min_n ? descs[i].n : min_n;
+  gp.bn = descs[0].block_n ? descs[0].block_n : (min_n >= 192 ? 256 : (min_n >= 96 ? 128 : 64));
+  int64_t base = 0;
+  int kc_min = 1 << 30, kc_max = 0;
+  for (int i = 0; i < n; ++i) {
+    base += static_cast<int64_t>(ceil_div(descs[i].m, BM)) * ceil_div(descs[i].n, gp.bn) * descs[i].ntaps;
+    const int kc = ceil_div(descs[i].k, BK);
+    kc_min = kc < kc_min ? kc : kc_min;
+    kc_max = kc > kc_max ? kc : kc_max;
+  }
+  double best_cost = 1e30;
+  for (int sp = 1; sp <= 8 && sp <= kc_min; ++sp) {
+    const double waves = static_cast<double>((base * sp + sms - 1) / sms);
+    // per wave: the tile's k-chunks, then its red.add epilogue, which takes about as long as 8 chunks of the main loop. Fitted
+    // on an H100 to the BertLayer group (2624 tokens, 41 chunks; 128 x 256 tiles, 216 per split), 1 / 2 / 3 splits: 76 / 95 / 90 us
+    const double cost = waves * (ceil_div(kc_max, sp) + 8.0);
+    if (cost < best_cost) { best_cost = cost; gp.split = sp; }
+  }
+  if (descs[0].split_k > 0) gp.split = descs[0].split_k;
+  return gp;
+}
+
+// workspace of one deterministic weight gradient run with `splits` K-splits (none for one split)
+static int64_t wgrad_ws_bytes(const cb_gemm_desc& d, int splits) {
+  return splits > 1 ? static_cast<int64_t>(splits) * d.m * d.ntaps * d.n * 4 : 0;
+}
+static int64_t group_ws_bytes(const cb_gemm_desc* descs, int n) {
+  const GroupPlan gp = group_plan(descs, n, sm_count_device());
+  int64_t bytes = 0;
+  for (int i = 0; i < n; ++i) {
+    const int64_t b = gp.groupable ? wgrad_ws_bytes(descs[i], real_splits(ceil_div(descs[i].k, BK), gp.split))
+                                   : wgrad_ws_bytes(descs[i], choose_config(descs[i], sm_count_device()).splits);
+    bytes = gp.groupable ? bytes + b : std::max(bytes, b);     // separate launches run one after another: one workspace for all
+  }
+  return bytes;
 }
 
 }  // namespace cb
@@ -1291,7 +1426,7 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
     CB_REQUIRE(d.ntaps == 1 || d.tap_w > 2, "cb_gemm: tap modes need tap_w (padded row pitch in pixels)");
     CB_REQUIRE(d.block_n == 0 || d.block_n == 64 || d.block_n == 128 || d.block_n == 256, "cb_gemm: block_n must be 0, 64, 128 or 256 (got %d)",
                d.block_n);
-    const LaunchCfg lc = choose_config(d);
+    const LaunchCfg lc = choose_config(d, sm_count());
     switch (lc.bn) {
       case 64: return nn ? launch_gemm<64, 2>(d, epi, stream) : launch_gemm<64, 0>(d, epi, stream);
       case 128: return nn ? launch_gemm<128, 2>(d, epi, stream) : launch_gemm<128, 0>(d, epi, stream);
@@ -1302,9 +1437,28 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
     CB_REQUIRE(d.m % 8 == 0 && d.n % 8 == 0, "cb_gemm(WGRAD): m, n must be multiples of 8 (got %d, %d)", d.m, d.n);
     CB_REQUIRE(d.out_ld % 4 == 0, "cb_gemm(WGRAD): out_ld must be a multiple of 4");
     CB_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "cb_gemm(WGRAD): out must be 16-byte aligned");
-    const LaunchCfg lc = choose_config(d);
+    const LaunchCfg lc = choose_config(d, plan_sm_count());
     cb_gemm_desc d2 = d;
     d2.split_k = lc.splits;
+    if (g_det.load(std::memory_order_relaxed) && lc.splits > 1) {
+      const int64_t need = wgrad_ws_bytes(d, lc.splits);
+      CB_REQUIRE(d.workspace != nullptr && d.workspace_bytes >= need && (reinterpret_cast<uintptr_t>(d.workspace) & 15) == 0,
+                 "cb_gemm(WGRAD): deterministic mode needs a 16-byte aligned workspace of %lld bytes (cb_gemm_workspace_bytes), got %lld",
+                 static_cast<long long>(need), static_cast<long long>(d.workspace ? d.workspace_bytes : 0));
+      float* ws = static_cast<float*>(d.workspace);
+      int rc = CB_ERR_INVALID;
+      switch (lc.bn) {
+        case 64: rc = launch_gemm<64, 1, true>(d2, epi, stream, ws); break;
+        case 128: rc = launch_gemm<128, 1, true>(d2, epi, stream, ws); break;
+        case 256: rc = launch_gemm<256, 1, true>(d2, epi, stream, ws); break;
+        default: CB_REQUIRE(false, "cb_gemm(WGRAD): block_n must be 0, 64, 128 or 256 (got %d)", lc.bn);
+      }
+      if (rc != CB_OK) return rc;
+      SplitReduce red;
+      red.njobs = 1;
+      red.j[0] = {static_cast<float*>(d.out), ws, d.out_ld, d.m, d.ntaps * d.n, lc.splits};
+      return launch_split_reduce(red, stream, "cb_gemm(split reduce)");
+    }
     switch (lc.bn) {
       case 64: return launch_gemm<64, 1>(d2, epi, stream);
       case 128: return launch_gemm<128, 1>(d2, epi, stream);
@@ -1320,7 +1474,6 @@ extern "C" int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* strea
   using namespace cb;
   CB_REQUIRE(descs != nullptr && n >= 1, "cb_gemm_wgrad_group: no problems");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  bool groupable = n >= 2 && n <= WG_MAX_PROBLEMS;
   for (int i = 0; i < n; ++i) {
     const cb_gemm_desc& d = descs[i];
     CB_REQUIRE(d.mode == CB_GEMM_WGRAD && d.out_fp32 == 1, "cb_gemm_wgrad_group: problem %d is not an fp32 WGRAD descriptor", i);
@@ -1328,43 +1481,50 @@ extern "C" int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* strea
     CB_REQUIRE(d.m % 8 == 0 && d.n % 8 == 0 && d.out_ld % 4 == 0 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0,
                "cb_gemm_wgrad_group: problem %d: m, n multiples of 8, out 16-byte aligned, out_ld a multiple of 4", i);
     CB_REQUIRE(d.ntaps == 1 || d.ntaps == 9, "cb_gemm_wgrad_group: problem %d: ntaps must be 1 or 9", i);
-    // one schedule for all: reduction lengths within 2 x of each other, otherwise the round-robin tiles are unbalanced
-    if (d.k * 2 < descs[0].k || descs[0].k * 2 < d.k) groupable = false;
   }
-  if (!groupable) {      // a single problem, too many, or very different reduction lengths: the ordinary launches
+  const bool det = g_det.load(std::memory_order_relaxed);
+  int64_t need = 0;
+  if (det) {
+    need = group_ws_bytes(descs, n);
+    CB_REQUIRE(need == 0 || (descs[0].workspace != nullptr && descs[0].workspace_bytes >= need &&
+                             (reinterpret_cast<uintptr_t>(descs[0].workspace) & 15) == 0),
+               "cb_gemm_wgrad_group: deterministic mode needs a 16-byte aligned workspace of %lld bytes in descs[0] "
+               "(cb_gemm_wgrad_group_workspace_bytes), got %lld",
+               static_cast<long long>(need), static_cast<long long>(descs[0].workspace ? descs[0].workspace_bytes : 0));
+  }
+  const GroupPlan gp = group_plan(descs, n, plan_sm_count());
+  if (!gp.groupable) {      // a single problem, too many, or very different reduction lengths: the ordinary launches
     for (int i = 0; i < n; ++i) {
-      const int rc = cb_gemm(&descs[i], stream_v);
+      cb_gemm_desc d = descs[i];
+      d.workspace = descs[0].workspace;       // stream-ordered launches: one workspace serves them all
+      d.workspace_bytes = descs[0].workspace_bytes;
+      const int rc = cb_gemm(&d, stream_v);
       if (rc != CB_OK) return rc;
     }
     return CB_OK;
   }
-  // tile width: the widest that does not mostly pad, unless descs[0].block_n sets it; K-split: descs[0].split_k, or the one with
-  // the least time per CTA
-  CB_REQUIRE(descs[0].block_n == 0 || descs[0].block_n == 64 || descs[0].block_n == 128 || descs[0].block_n == 256,
-             "cb_gemm_wgrad_group: block_n must be 0, 64, 128 or 256 (got %d)", descs[0].block_n);
-  int min_n = descs[0].n;
-  for (int i = 1; i < n; ++i) min_n = descs[i].n < min_n ? descs[i].n : min_n;
-  const int bn = descs[0].block_n ? descs[0].block_n : (min_n >= 192 ? 256 : (min_n >= 96 ? 128 : 64));
-  int64_t base = 0;
-  int kc_min = 1 << 30, kc_max = 0;
-  for (int i = 0; i < n; ++i) {
-    base += static_cast<int64_t>(ceil_div(descs[i].m, BM)) * ceil_div(descs[i].n, bn) * descs[i].ntaps;
-    const int kc = ceil_div(descs[i].k, BK);
-    kc_min = kc < kc_min ? kc : kc_min;
-    kc_max = kc > kc_max ? kc : kc_max;
+  CB_REQUIRE(gp.bn == 64 || gp.bn == 128 || gp.bn == 256, "cb_gemm_wgrad_group: block_n must be 0, 64, 128 or 256 (got %d)", gp.bn);
+  if (det && need > 0) {
+    float* ws = static_cast<float*>(descs[0].workspace);
+    if (gp.bn == 256) return launch_wgrad_group<256, true>(descs, n, gp.split, stream, ws);
+    if (gp.bn == 128) return launch_wgrad_group<128, true>(descs, n, gp.split, stream, ws);
+    return launch_wgrad_group<64, true>(descs, n, gp.split, stream, ws);
   }
-  const int sms = sm_count();
-  int best_split = 1;
-  double best_cost = 1e30;
-  for (int sp = 1; sp <= 8 && sp <= kc_min; ++sp) {
-    const double waves = static_cast<double>((base * sp + sms - 1) / sms);
-    // per wave: the tile's k-chunks, then its red.add epilogue, which takes about as long as 8 chunks of the main loop. Fitted
-    // on an H100 to the BertLayer group (2624 tokens, 41 chunks; 128 x 256 tiles, 216 per split), 1 / 2 / 3 splits: 76 / 95 / 90 us
-    const double cost = waves * (ceil_div(kc_max, sp) + 8.0);
-    if (cost < best_cost) { best_cost = cost; best_split = sp; }
-  }
-  if (descs[0].split_k > 0) best_split = descs[0].split_k;
-  if (bn == 256) return launch_wgrad_group<256>(descs, n, best_split, stream);
-  if (bn == 128) return launch_wgrad_group<128>(descs, n, best_split, stream);
-  return launch_wgrad_group<64>(descs, n, best_split, stream);
+  if (gp.bn == 256) return launch_wgrad_group<256>(descs, n, gp.split, stream);
+  if (gp.bn == 128) return launch_wgrad_group<128>(descs, n, gp.split, stream);
+  return launch_wgrad_group<64>(descs, n, gp.split, stream);
+}
+
+extern "C" int64_t cb_gemm_workspace_bytes(const cb_gemm_desc* d) {
+  using namespace cb;
+  if (d == nullptr || d->mode != CB_GEMM_WGRAD || d->m <= 0 || d->n <= 0 || d->k <= 0) return 0;
+  return wgrad_ws_bytes(*d, choose_config(*d, sm_count_device()).splits);
+}
+
+extern "C" int64_t cb_gemm_wgrad_group_workspace_bytes(const cb_gemm_desc* descs, int n) {
+  using namespace cb;
+  if (descs == nullptr || n < 1) return 0;
+  for (int i = 0; i < n; ++i)
+    if (descs[i].mode != CB_GEMM_WGRAD || descs[i].m <= 0 || descs[i].n <= 0 || descs[i].k <= 0) return 0;
+  return group_ws_bytes(descs, n);
 }

@@ -36,6 +36,11 @@ inline int check_launch(const char* what) {
 // overlap, see include/clipbert_b200.h.
 extern std::atomic<int> g_pdl;
 
+// deterministic mode (cb_set_deterministic): accumulations run in a fixed order; see include/clipbert_b200.h
+extern std::atomic<int> g_det;
+// out[0] += sum of part[0, n) in a fixed order (bert_ops.cu: ordered_sum_kernel), one launch on `stream`
+int launch_ordered_sum(const float* part, int n, float* out, cudaStream_t stream, const char* what);
+
 // g_pdl: 0 off, 1 every kernel, 2 every kernel EXCEPT the persistent GEMMs (their early-launched CTAs would hold ~200 KB
 // of shared memory per SM while they wait; an LN / attention / column-sum CTA holds a few KB)
 template <bool kGemm, typename... KArgs, typename... Args>

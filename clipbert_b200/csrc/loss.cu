@@ -12,9 +12,28 @@
 
 namespace cb {
 
+// the block's share of the mean: one atomic per block, or (DET) a plain store to part[blockIdx.x] summed in block order afterwards
+template <bool DET>
+__device__ __forceinline__ void block_loss_sum(float l, float inv_n, float* loss, float* part) {
+  l = warp_sum(l);
+  __shared__ float red[8];
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = l;
+  __syncthreads();
+  if (threadIdx.x < 8) {
+    float v = red[threadIdx.x];
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
+    if (threadIdx.x == 0) {
+      if constexpr (DET) part[blockIdx.x] = v * inv_n;
+      else atomicAdd(loss, v * inv_n);
+    }
+  }
+}
+
+template <bool DET>
 __global__ void __launch_bounds__(256) clip_lse_loss_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels,
                                                             float* __restrict__ loss, float* __restrict__ dlogits, int n_clips,
-                                                            int nseq, int ncls, float inv_n, float grad_scale) {
+                                                            int nseq, int ncls, float inv_n, float grad_scale, float* part) {
   pdl_wait();
   pdl_trigger();
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -48,17 +67,7 @@ __global__ void __launch_bounds__(256) clip_lse_loss_kernel(const float* __restr
         }
     }
   }
-  // block sum -> one atomic per block
-  l = warp_sum(l);
-  __shared__ float red[8];
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = l;
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    float v = red[threadIdx.x];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(loss, v * inv_n);
-  }
+  block_loss_sum<DET>(l, inv_n, loss, part);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -66,9 +75,10 @@ __global__ void __launch_bounds__(256) clip_lse_loss_kernel(const float* __restr
 // logits.mean(0) or logits.max(0)[0], then calc_loss -> F.cross_entropy(reduction="none") -> .mean()), forward + backward.
 //   mean: d z[k, b, c] = (softmax_c(mean_k z) - onehot) / (n_clips * B')      max: the gradient goes to the arg-max clip only
 // ------------------------------------------------------------------------------------------------
+template <bool DET>
 __global__ void __launch_bounds__(256) clip_pool_ce_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels,
                                                            float* __restrict__ loss, float* __restrict__ dlogits, int n_clips, int nseq,
-                                                           int ncls, int pool_max, float inv_n, float grad_scale) {
+                                                           int ncls, int pool_max, float inv_n, float grad_scale, float* part) {
   pdl_wait();
   pdl_trigger();
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -105,16 +115,7 @@ __global__ void __launch_bounds__(256) clip_pool_ce_kernel(const float* __restri
       }
     }
   }
-  l = warp_sum(l);
-  __shared__ float red[8];
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = l;
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    float v = red[threadIdx.x];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(loss, v * inv_n);
-  }
+  block_loss_sum<DET>(l, inv_n, loss, part);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -172,22 +173,6 @@ __global__ void __launch_bounds__(CE_THREADS) ce_bwd_kernel(const float* __restr
 
 using namespace cb;
 
-extern "C" int cb_clip_pool_ce_loss(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq, int ncls,
-                                    int pool, float grad_scale, void* stream) {
-  CB_REQUIRE(logits && labels && loss, "cb_clip_pool_ce_loss: null pointer");
-  CB_REQUIRE(n_clips > 0 && nseq > 0 && ncls > 0, "cb_clip_pool_ce_loss: empty problem (n_clips=%d nseq=%d ncls=%d)", n_clips, nseq, ncls);
-  CB_REQUIRE(pool == 1 || pool == 2, "cb_clip_pool_ce_loss: pool must be 1 (mean) or 2 (max); lse is cb_clip_lse_loss");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(float), st);
-  if (e != cudaSuccess) {
-    set_error("cb_clip_pool_ce_loss: memset failed: %s", cudaGetErrorString(e));
-    return CB_ERR_CUDA;
-  }
-  launch_k(clip_pool_ce_kernel, ceil_div(nseq, 256), 256, 0, st, logits, labels, loss, dlogits, n_clips, nseq, ncls, pool == 2 ? 1 : 0,
-           1.0f / nseq, grad_scale);
-  return check_launch("cb_clip_pool_ce_loss");
-}
-
 extern "C" int cb_cross_entropy_fwd(const float* logits, int64_t ld, const int64_t* labels, float* loss, float* lse, int64_t rows, int ncls,
                                     int64_t ignore_index, void* stream) {
   CB_REQUIRE(logits && labels && loss && lse, "cb_cross_entropy_fwd: null pointer");
@@ -206,17 +191,60 @@ extern "C" int cb_cross_entropy_bwd(const float* logits, int64_t ld, const int64
   return check_launch("cb_cross_entropy_bwd");
 }
 
-extern "C" int cb_clip_lse_loss(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq,
-                                int ncls, float grad_scale, void* stream) {
-  CB_REQUIRE(logits && labels && loss, "cb_clip_lse_loss: null pointer");
-  CB_REQUIRE(n_clips > 0 && nseq > 0 && ncls > 0, "cb_clip_lse_loss: empty problem (n_clips=%d nseq=%d ncls=%d)", n_clips, nseq, ncls);
+// pool 0 = lse (clip_lse_loss_kernel), 1 / 2 = mean / max (clip_pool_ce_kernel); scratch != nullptr: deterministic launch
+static int clip_loss(const char* name, const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq,
+                     int ncls, int pool, float grad_scale, float* scratch, int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(logits && labels && loss, "%s: null pointer", name);
+  CB_REQUIRE(n_clips > 0 && nseq > 0 && ncls > 0, "%s: empty problem (n_clips=%d nseq=%d ncls=%d)", name, n_clips, nseq, ncls);
+  const int blocks = ceil_div(nseq, 256);
+  if (scratch == nullptr)
+    CB_REQUIRE(!g_det.load(std::memory_order_relaxed), "%s: deterministic mode is on; call %s_det with its scratch", name, name);
+  else
+    CB_REQUIRE(scratch_bytes >= 4ll * blocks, "%s: needs a scratch of %lld bytes", name, 4ll * blocks);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(float), st);
   if (e != cudaSuccess) {
-    set_error("cb_clip_lse_loss: memset failed: %s", cudaGetErrorString(e));
+    set_error("%s: memset failed: %s", name, cudaGetErrorString(e));
     return CB_ERR_CUDA;
   }
-  launch_k(clip_lse_loss_kernel, ceil_div(nseq, 256), 256, 0, st, logits, labels, loss, dlogits, n_clips, nseq, ncls, 1.0f / nseq,
-           grad_scale);
-  return check_launch("cb_clip_lse_loss");
+  if (pool == 0) {
+    if (scratch) launch_k(clip_lse_loss_kernel<true>, blocks, 256, 0, st, logits, labels, loss, dlogits, n_clips, nseq, ncls, 1.0f / nseq, grad_scale, scratch);
+    else launch_k(clip_lse_loss_kernel<false>, blocks, 256, 0, st, logits, labels, loss, dlogits, n_clips, nseq, ncls, 1.0f / nseq, grad_scale, scratch);
+  } else {
+    if (scratch) launch_k(clip_pool_ce_kernel<true>, blocks, 256, 0, st, logits, labels, loss, dlogits, n_clips, nseq, ncls, pool == 2 ? 1 : 0,
+                          1.0f / nseq, grad_scale, scratch);
+    else launch_k(clip_pool_ce_kernel<false>, blocks, 256, 0, st, logits, labels, loss, dlogits, n_clips, nseq, ncls, pool == 2 ? 1 : 0,
+                  1.0f / nseq, grad_scale, scratch);
+  }
+  const int rc = check_launch(name);
+  if (rc != CB_OK || scratch == nullptr) return rc;
+  return launch_ordered_sum(scratch, blocks, loss, st, name);
+}
+
+extern "C" int cb_clip_pool_ce_loss(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq, int ncls,
+                                    int pool, float grad_scale, void* stream) {
+  CB_REQUIRE(pool == 1 || pool == 2, "cb_clip_pool_ce_loss: pool must be 1 (mean) or 2 (max); lse is cb_clip_lse_loss");
+  return clip_loss("cb_clip_pool_ce_loss", logits, labels, loss, dlogits, n_clips, nseq, ncls, pool, grad_scale, nullptr, 0, stream);
+}
+
+extern "C" int cb_clip_lse_loss(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq,
+                                int ncls, float grad_scale, void* stream) {
+  return clip_loss("cb_clip_lse_loss", logits, labels, loss, dlogits, n_clips, nseq, ncls, 0, grad_scale, nullptr, 0, stream);
+}
+
+extern "C" int64_t cb_clip_loss_scratch_bytes(int nseq) { return nseq > 0 ? 4ll * ceil_div(nseq, 256) : 0; }
+
+extern "C" int cb_clip_lse_loss_det(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq,
+                                    int ncls, float grad_scale, float* scratch, int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(scratch != nullptr, "cb_clip_lse_loss_det: needs a scratch of %lld bytes", static_cast<long long>(cb_clip_loss_scratch_bytes(nseq)));
+  return clip_loss("cb_clip_lse_loss_det", logits, labels, loss, dlogits, n_clips, nseq, ncls, 0, grad_scale, scratch, scratch_bytes, stream);
+}
+
+extern "C" int cb_clip_pool_ce_loss_det(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq,
+                                        int ncls, int pool, float grad_scale, float* scratch, int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(pool == 1 || pool == 2, "cb_clip_pool_ce_loss_det: pool must be 1 (mean) or 2 (max); lse is cb_clip_lse_loss_det");
+  CB_REQUIRE(scratch != nullptr, "cb_clip_pool_ce_loss_det: needs a scratch of %lld bytes",
+             static_cast<long long>(cb_clip_loss_scratch_bytes(nseq)));
+  return clip_loss("cb_clip_pool_ce_loss_det", logits, labels, loss, dlogits, n_clips, nseq, ncls, pool, grad_scale, scratch, scratch_bytes,
+                   stream);
 }

@@ -20,7 +20,9 @@ constexpr int CHUNK_COLS = 8;
 // hyper table row (floats): lr, step_size, weight_decay, beta1, beta2, eps, 0, 0
 constexpr int HYPER_COLS = 8;
 
-__device__ __forceinline__ void block_atomic_sum(float acc, float* out) {
+// DET: the block's sum goes to part[blockIdx.x] (plain store) and launch_ordered_sum adds the partials in block order
+template <bool DET>
+__device__ __forceinline__ void block_atomic_sum(float acc, float* out, float* part) {
   acc = warp_sum(acc);
   __shared__ float red[8];
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
@@ -29,12 +31,16 @@ __device__ __forceinline__ void block_atomic_sum(float acc, float* out) {
     float v = red[threadIdx.x];
 #pragma unroll
     for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(out, v);
+    if (threadIdx.x == 0) {
+      if constexpr (DET) part[blockIdx.x] = v;
+      else atomicAdd(out, v);
+    }
   }
 }
 
 // out += sum(x^2) over x[0, n): grid-stride float4 loads, warp shuffle + shared reduction, one atomicAdd per block
-__global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x, int64_t n, float* __restrict__ out) {
+template <bool DET>
+__global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x, int64_t n, float* __restrict__ out, float* part) {
   pdl_wait();
   pdl_trigger();
   float acc = 0.f;
@@ -45,12 +51,14 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x,
   }
   if (blockIdx.x == 0 && threadIdx.x == 0)
     for (int64_t i = n4 << 2; i < n; ++i) acc = fmaf(x[i], x[i], acc);
-  block_atomic_sum(acc, out);
+  block_atomic_sum<DET>(acc, out, part);
 }
 
 // out += sum of x^2 over the chunk table's elements only: alignment padding between parameters and the zero-padded
 // classifier rows belong to no parameter and must not enter the gradient norm
-__global__ void __launch_bounds__(256) sumsq_chunks_kernel(const float* __restrict__ x, const int64_t* __restrict__ chunks, float* __restrict__ out) {
+template <bool DET>
+__global__ void __launch_bounds__(256) sumsq_chunks_kernel(const float* __restrict__ x, const int64_t* __restrict__ chunks, float* __restrict__ out,
+                                                           float* part) {
   pdl_wait();
   pdl_trigger();
   const int64_t* ch = chunks + static_cast<int64_t>(blockIdx.x) * CHUNK_COLS;
@@ -64,7 +72,7 @@ __global__ void __launch_bounds__(256) sumsq_chunks_kernel(const float* __restri
       for (int64_t k = i; k < n; ++k) acc = fmaf(x[off + k], x[off + k], acc);
     }
   }
-  block_atomic_sum(acc, out);
+  block_atomic_sum<DET>(acc, out, part);
 }
 
 __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ master, float* __restrict__ grad, float* __restrict__ exp_avg,
@@ -133,17 +141,38 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ master, 
 extern "C" {
 using namespace cb;
 
+static int sumsq_blocks(int64_t n, const int64_t* chunks, int nchunks) {
+  if (chunks) return nchunks;
+  const int64_t want = (n / 4 + 255) / 256;
+  return static_cast<int>(want < 1 ? 1 : (want > 132 * 8 ? 132 * 8 : want));   // 8 resident 256-thread CTAs per H100 SM
+}
+
 int cb_sumsq(const float* x, int64_t n, const int64_t* chunks, int nchunks, float* out, void* stream) {
   CB_REQUIRE(x && out && (chunks ? nchunks > 0 : n > 0), "cb_sumsq: bad arguments");
   CB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "cb_sumsq: x must be 16-byte aligned");
-  if (chunks) {
-    launch_k(sumsq_chunks_kernel, nchunks, 256, 0, static_cast<cudaStream_t>(stream), x, chunks, out);
-    return check_launch("cb_sumsq");
-  }
-  const int64_t want = (n / 4 + 255) / 256;
-  const int grid = static_cast<int>(want < 1 ? 1 : (want > 132 * 8 ? 132 * 8 : want));   // 8 resident 256-thread CTAs per H100 SM
-  launch_k(sumsq_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), x, n, out);
+  CB_REQUIRE(!g_det.load(std::memory_order_relaxed), "cb_sumsq: deterministic mode is on; call cb_sumsq_det with its scratch");
+  const int grid = sumsq_blocks(n, chunks, nchunks);
+  if (chunks) launch_k(sumsq_chunks_kernel<false>, grid, 256, 0, static_cast<cudaStream_t>(stream), x, chunks, out, static_cast<float*>(nullptr));
+  else launch_k(sumsq_kernel<false>, grid, 256, 0, static_cast<cudaStream_t>(stream), x, n, out, static_cast<float*>(nullptr));
   return check_launch("cb_sumsq");
+}
+
+int64_t cb_sumsq_scratch_bytes(int64_t n, const int64_t* chunks, int nchunks) {
+  return (chunks ? nchunks > 0 : n > 0) ? 4ll * sumsq_blocks(n, chunks, nchunks) : 0;
+}
+
+int cb_sumsq_det(const float* x, int64_t n, const int64_t* chunks, int nchunks, float* out, float* scratch, int64_t scratch_bytes,
+                 void* stream) {
+  CB_REQUIRE(x && out && (chunks ? nchunks > 0 : n > 0), "cb_sumsq_det: bad arguments");
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "cb_sumsq_det: x must be 16-byte aligned");
+  const int grid = sumsq_blocks(n, chunks, nchunks);
+  CB_REQUIRE(scratch && scratch_bytes >= 4ll * grid, "cb_sumsq_det: needs a scratch of %lld bytes", 4ll * grid);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (chunks) launch_k(sumsq_chunks_kernel<true>, grid, 256, 0, st, x, chunks, out, scratch);
+  else launch_k(sumsq_kernel<true>, grid, 256, 0, st, x, n, out, scratch);
+  const int rc = check_launch("cb_sumsq_det");
+  if (rc != CB_OK) return rc;
+  return launch_ordered_sum(scratch, grid, out, st, "cb_sumsq_det(reduce)");
 }
 
 int cb_adamw_step(float* master, float* grad, float* exp_avg, float* exp_avg_sq, void* packed, const int64_t* chunks, int nchunks,

@@ -48,6 +48,21 @@ _SIGS = {
     "cb_maxpool2x2_relu_fwd": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool2x2_relu_bwd": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "cb_relu_mask": [_vp, _vp, _vp, _i64, _vp],
+    # deterministic variants: the arguments of the plain entry point, then (scratch, scratch_bytes) before the stream
+    "cb_layernorm_bwd_det": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _u64, _vp, _i64, _vp],
+    "cb_embed_text_bwd_det": [_vp] * 12 + [_i, _i, _i, _i, _i, _f, _u64, _vp, _i64, _vp],
+    "cb_embed_visual_bwd_det": [_vp, _vp, _vp, _vp, _i] + [_vp] * 12 + [_i, _i, _i, _i, _i, _i, _i, _i, _f, _u64, _vp, _i64, _vp],
+    "cb_colsum_det": [_vp, _i64, _vp, _i, _i, _vp, _i64, _vp],
+    "cb_clip_lse_loss_det": [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _i64, _vp],
+    "cb_clip_pool_ce_loss_det": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _i64, _vp],
+    "cb_sumsq_det": [_vp, _i64, _vp, _i, _vp, _vp, _i64, _vp],
+    # scratch-size queries (int64 results)
+    "cb_layernorm_bwd_scratch_bytes": [_i],
+    "cb_embed_text_bwd_scratch_bytes": [_i, _i],
+    "cb_embed_visual_bwd_scratch_bytes": [_i, _i, _i],
+    "cb_colsum_scratch_bytes": [_i, _i],
+    "cb_clip_loss_scratch_bytes": [_i],
+    "cb_sumsq_scratch_bytes": [_i64, _vp, _i],
 }
 _bound = {}
 
@@ -57,7 +72,7 @@ def _fn(name):
     if f is None:
         f = getattr(L.lib(), name)
         f.argtypes = _SIGS[name]
-        f.restype = _c.c_int
+        f.restype = _c.c_int64 if name.endswith("_scratch_bytes") else _c.c_int
         _bound[name] = f
     return f
 
@@ -159,6 +174,41 @@ def set_pdl(enable):
 
 
 # ------------------------------------------------------------------------------------------------
+# deterministic mode: torch.use_deterministic_algorithms(True) makes every accumulation run in a fixed order
+# ------------------------------------------------------------------------------------------------
+_lib_deterministic = False
+
+
+def set_deterministic(on):
+    """cb_set_deterministic: the library's mode (weight-gradient K-split plan and workspace; the atomic entry points refuse).
+    Returns the previous setting. The wrappers below keep it equal to torch's flag; see ``deterministic``."""
+    return bool(L.lib().cb_set_deterministic(int(bool(on))))
+
+
+def deterministic():
+    """torch.are_deterministic_algorithms_enabled(), mirrored into the library when it changes. Every wrapper that accumulates
+    reads it when it issues its launches, so the flag in force while a pass (forward, backward, optimizer step, CUDA-graph
+    capture) issues its launches decides how they accumulate."""
+    global _lib_deterministic
+    on = torch.are_deterministic_algorithms_enabled()
+    if on != _lib_deterministic:
+        set_deterministic(on)
+        _lib_deterministic = on
+    return on
+
+
+def _scratch(nbytes, like):
+    """fp32 scratch of at least nbytes from the caching allocator, on the current (launch) stream: when the caller drops it the
+    allocator hands the block only to later work on that stream, which runs after the launches that use it."""
+    return torch.empty(max(4, (int(nbytes) + 3) // 4), dtype=torch.float32, device=like.device)
+
+
+def _scratch_args(nbytes, like):
+    t = _scratch(nbytes, like)
+    return t, t.numel() * 4
+
+
+# ------------------------------------------------------------------------------------------------
 # side queue: weight-gradient work off the backward critical path
 # ------------------------------------------------------------------------------------------------
 class SideQueue:
@@ -210,7 +260,7 @@ overlap_wgrad = True      # module switch (bench --overlap_wgrad 0 / tests flip 
 # ------------------------------------------------------------------------------------------------
 # tensor-core contraction
 # ------------------------------------------------------------------------------------------------
-_GEMM_PTR_FIELDS = ("a", "b", "scale", "shift", "residual", "aux", "out", "out2")
+_GEMM_PTR_FIELDS = ("a", "b", "scale", "shift", "residual", "aux", "out", "out2", "workspace")
 _gemm_timing = None
 
 
@@ -248,8 +298,64 @@ def _load_tuning():
             _tuning = {}
 
 
+def _gemm_descs(kws):
+    arr = (L.GemmDesc * len(kws))()
+    for d, kw in zip(arr, kws):
+        d.ntaps = 1
+        d.tap_sign = 1
+        d.split_k = 0
+        for k, v in kw.items():
+            if k in _GEMM_PTR_FIELDS:
+                v = _p(v) if isinstance(v, torch.Tensor) else v
+            setattr(d, k, v)
+    return arr
+
+
+def gemm_workspace_bytes(kw):
+    """cb_gemm_workspace_bytes: workspace a weight-gradient descriptor needs in deterministic mode (0: one K-split)."""
+    return int(L.lib().cb_gemm_workspace_bytes(_gemm_descs([kw])))
+
+
+def gemm_wgrad_group_workspace_bytes(kws):
+    """cb_gemm_wgrad_group_workspace_bytes: the whole group's workspace (carried by the first descriptor)."""
+    return int(L.lib().cb_gemm_wgrad_group_workspace_bytes(_gemm_descs(kws), len(kws)))
+
+
+def _with_workspace(kw, nbytes):
+    if nbytes <= 0:
+        return kw
+    ws, nb = _scratch_args(nbytes, kw["out"])
+    return dict(kw, workspace=ws, workspace_bytes=nb)
+
+
+def _launch_gemm(name, kws):
+    """cb_gemm (one descriptor) or cb_gemm_wgrad_group, with the profiling hooks."""
+    arr = _gemm_descs(kws)
+    timing = _gemm_timing is not None or _op_timing is not None
+    if timing:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    if name == "cb_gemm":
+        rc = L.lib().cb_gemm(arr, _s())
+    else:
+        rc = L.lib().cb_gemm_wgrad_group(arr, len(kws), _s())
+    if rc != 0:
+        raise RuntimeError("%s failed (%d): %s" % (name, rc, L.lib().cb_last_error().decode()))
+    if timing:
+        e1.record()
+        if _gemm_timing is not None:
+            _gemm_timing.append((e0, e1))
+        if _op_timing is not None:
+            d = arr[0]
+            label = ("gemm mode=%d m=%d n=%d k=%d taps=%d res=%d aux=%d o2=%d f32=%d rm=%d" % (
+                d.mode, d.m, d.n, d.k, d.ntaps, bool(d.residual), bool(d.aux), bool(d.out2), d.out_fp32, d.rowmap)
+                if name == "cb_gemm" else "gemm wgrad group x%d" % len(kws))
+            _op_timing.append((label, e0, e1))
+
+
 def gemm(**kw):
-    """cb_gemm with keyword fields of cb_gemm_desc; tensor-valued fields are converted to pointers."""
+    """cb_gemm with keyword fields of cb_gemm_desc; tensor-valued fields are converted to pointers. A weight gradient in
+    deterministic mode gets its split workspace here."""
     if _tuning is None:
         _load_tuning()
     if _gemm_record is not None:
@@ -258,28 +364,9 @@ def gemm(**kw):
         t = _tuning.get(gemm_key(kw))
         if t is not None:
             kw = dict(kw, block_n=t[0], split_k=t[1], reserved=(t[2] << 8) | (32 if (len(t) > 3 and t[3]) else 0))
-    d = L.GemmDesc()
-    d.ntaps = 1
-    d.tap_sign = 1
-    d.split_k = 0
-    for k, v in kw.items():
-        if k in _GEMM_PTR_FIELDS:
-            v = _p(v) if isinstance(v, torch.Tensor) else v
-        setattr(d, k, v)
-    timing = _gemm_timing is not None or _op_timing is not None
-    if timing:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-    rc = L.lib().cb_gemm(ctypes.byref(d), _s())
-    if rc != 0:
-        raise RuntimeError("cb_gemm failed (%d): %s" % (rc, L.lib().cb_last_error().decode()))
-    if timing:
-        e1.record()
-        if _gemm_timing is not None:
-            _gemm_timing.append((e0, e1))
-        if _op_timing is not None:
-            _op_timing.append(("gemm mode=%d m=%d n=%d k=%d taps=%d res=%d aux=%d o2=%d f32=%d rm=%d" % (
-                d.mode, d.m, d.n, d.k, d.ntaps, bool(d.residual), bool(d.aux), bool(d.out2), d.out_fp32, d.rowmap), e0, e1))
+    if kw.get("mode", CB_GEMM_TN) == CB_GEMM_WGRAD and deterministic():
+        kw = _with_workspace(kw, gemm_workspace_bytes(kw))
+    _launch_gemm("cb_gemm", [kw])
 
 
 # module switch (bench --group_wgrad): which weight-gradient GEMMs go out as grouped launches. 0 none; 1 BertLayer (4 in one) +
@@ -298,28 +385,10 @@ def gemm_wgrad_group(kws):
         return
     if _gemm_record is not None:
         _gemm_record.append(dict(group=[dict(kw) for kw in kws]))
-    arr = (L.GemmDesc * len(kws))()
-    for d, kw in zip(arr, kws):
-        d.ntaps = 1
-        d.tap_sign = 1
-        d.split_k = 0
-        for k, v in kw.items():
-            if k in _GEMM_PTR_FIELDS:
-                v = _p(v) if isinstance(v, torch.Tensor) else v
-            setattr(d, k, v)
-    timing = _gemm_timing is not None or _op_timing is not None
-    if timing:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-    rc = L.lib().cb_gemm_wgrad_group(arr, len(kws), _s())
-    if rc != 0:
-        raise RuntimeError("cb_gemm_wgrad_group failed (%d): %s" % (rc, L.lib().cb_last_error().decode()))
-    if timing:
-        e1.record()
-        if _gemm_timing is not None:
-            _gemm_timing.append((e0, e1))
-        if _op_timing is not None:
-            _op_timing.append(("gemm wgrad group x%d" % len(kws), e0, e1))
+    kws = list(kws)
+    if deterministic():
+        kws[0] = _with_workspace(kws[0], gemm_wgrad_group_workspace_bytes(kws))
+    _launch_gemm("cb_gemm_wgrad_group", kws)
 
 
 def wgrad_split(m, n, k, ntaps=1, block_n=128):
@@ -335,8 +404,22 @@ def layernorm_fwd(x, gamma, beta, y, stats, eps):
 
 
 def layernorm_bwd(dy, x, stats, gamma, dx, dx_drop, dgamma, dbeta, dbias_drop, p, seed):
+    if (dgamma is not None or dbeta is not None or dbias_drop is not None) and deterministic():
+        layernorm_bwd_det(dy, x, stats, gamma, dx, dx_drop, dgamma, dbeta, dbias_drop, p, seed,
+                          _scratch(layernorm_bwd_scratch_bytes(x.shape[0]), x))
+        return
     _call("cb_layernorm_bwd", _p(dy), _p(x), _p(stats), _p(gamma), _p(dx), _p(dx_drop), _p(dgamma), _p(dbeta),
           _p(dbias_drop), x.shape[0], x.shape[1], p, seed, _s())
+
+
+def layernorm_bwd_scratch_bytes(m):
+    return int(_fn("cb_layernorm_bwd_scratch_bytes")(m))
+
+
+def layernorm_bwd_det(dy, x, stats, gamma, dx, dx_drop, dgamma, dbeta, dbias_drop, p, seed, scratch):
+    """cb_layernorm_bwd_det: parameter gradients summed in block order through ``scratch`` (fp32)."""
+    _call("cb_layernorm_bwd_det", _p(dy), _p(x), _p(stats), _p(gamma), _p(dx), _p(dx_drop), _p(dgamma), _p(dbeta),
+          _p(dbias_drop), x.shape[0], x.shape[1], p, seed, _p(scratch), scratch.numel() * 4, _s())
 
 
 def embed_text_fwd(ids, word, pos, type0, gamma, beta, out, stats, nseq, lt, l, eps, p, seed):
@@ -345,8 +428,23 @@ def embed_text_fwd(ids, word, pos, type0, gamma, beta, out, stats, nseq, lt, l, 
 
 
 def embed_text_bwd(dh, ids, word, pos, type0, gamma, stats, dword, dpos, dtype0, dgamma, dbeta, nseq, lt, l, p, seed):
+    if deterministic():
+        embed_text_bwd_det(dh, ids, word, pos, type0, gamma, stats, dword, dpos, dtype0, dgamma, dbeta, nseq, lt, l, p, seed,
+                           _scratch(embed_text_bwd_scratch_bytes(nseq, lt), dh))
+        return
     _call("cb_embed_text_bwd", _p(dh), _p(ids), _p(word), _p(pos), _p(type0), _p(gamma), _p(stats), _p(dword), _p(dpos),
           _p(dtype0), _p(dgamma), _p(dbeta), nseq, lt, l, word.shape[0], word.shape[1], p, seed, _s())
+
+
+def embed_text_bwd_scratch_bytes(nseq, lt):
+    return int(_fn("cb_embed_text_bwd_scratch_bytes")(nseq, lt))
+
+
+def embed_text_bwd_det(dh, ids, word, pos, type0, gamma, stats, dword, dpos, dtype0, dgamma, dbeta, nseq, lt, l, p, seed, scratch):
+    """cb_embed_text_bwd_det: table gradients in block / row order through ``scratch`` (fp32)."""
+    _call("cb_embed_text_bwd_det", _p(dh), _p(ids), _p(word), _p(pos), _p(type0), _p(gamma), _p(stats), _p(dword), _p(dpos),
+          _p(dtype0), _p(dgamma), _p(dbeta), nseq, lt, l, word.shape[0], word.shape[1], p, seed, _p(scratch), scratch.numel() * 4,
+          _s())
 
 
 def embed_visual_fwd(grid, seq2vid, n_ex, rowemb, colemb, type0, gamma, beta, out, stats, nseq, t, gh, gw, lt, l, eps, p,
@@ -357,9 +455,26 @@ def embed_visual_fwd(grid, seq2vid, n_ex, rowemb, colemb, type0, gamma, beta, ou
 
 def embed_visual_bwd(dh, grid, seq2vid, vid_start, n_ex, rowemb, colemb, type0, gamma, stats, dv_tmp, dgrid, drow, dcol,
                      dtype0, dgamma, dbeta, nseq, nvid, t, gh, gw, lt, l, p, seed):
+    if deterministic():
+        embed_visual_bwd_det(dh, grid, seq2vid, vid_start, n_ex, rowemb, colemb, type0, gamma, stats, dv_tmp, dgrid, drow, dcol,
+                             dtype0, dgamma, dbeta, nseq, nvid, t, gh, gw, lt, l, p, seed,
+                             _scratch(embed_visual_bwd_scratch_bytes(nseq, gh, gw), dh))
+        return
     _call("cb_embed_visual_bwd", _p(dh), _p(grid), _p(seq2vid), _p(vid_start), n_ex, _p(rowemb), _p(colemb), _p(type0),
           _p(gamma), _p(stats), _p(dv_tmp), _p(dgrid), _p(drow), _p(dcol), _p(dtype0), _p(dgamma), _p(dbeta), nseq, nvid, t,
           gh, gw, lt, l, rowemb.shape[1], p, seed, _s())
+
+
+def embed_visual_bwd_scratch_bytes(nseq, gh, gw):
+    return int(_fn("cb_embed_visual_bwd_scratch_bytes")(nseq, gh, gw))
+
+
+def embed_visual_bwd_det(dh, grid, seq2vid, vid_start, n_ex, rowemb, colemb, type0, gamma, stats, dv_tmp, dgrid, drow, dcol,
+                         dtype0, dgamma, dbeta, nseq, nvid, t, gh, gw, lt, l, p, seed, scratch):
+    """cb_embed_visual_bwd_det: table gradients in block order through ``scratch`` (fp32)."""
+    _call("cb_embed_visual_bwd_det", _p(dh), _p(grid), _p(seq2vid), _p(vid_start), n_ex, _p(rowemb), _p(colemb), _p(type0),
+          _p(gamma), _p(stats), _p(dv_tmp), _p(dgrid), _p(drow), _p(dcol), _p(dtype0), _p(dgamma), _p(dbeta), nseq, nvid, t,
+          gh, gw, lt, l, rowemb.shape[1], p, seed, _p(scratch), scratch.numel() * 4, _s())
 
 
 def nvls_allreduce(multicast_ptr, n, rank, world, scale, max_ctas=0):
@@ -368,12 +483,33 @@ def nvls_allreduce(multicast_ptr, n, rank, world, scale, max_ctas=0):
 
 
 def clip_lse_loss(logits, labels, loss, dlogits, n_clips, nseq, ncls, grad_scale=1.0):
+    if deterministic():
+        clip_lse_loss_det(logits, labels, loss, dlogits, n_clips, nseq, ncls, grad_scale, _scratch(clip_loss_scratch_bytes(nseq), logits))
+        return
     _call("cb_clip_lse_loss", _p(logits), _p(labels), _p(loss), _p(dlogits), n_clips, nseq, ncls, grad_scale, _s())
 
 
 def clip_pool_ce_loss(logits, labels, loss, dlogits, n_clips, nseq, ncls, pool, grad_scale=1.0):
     """pool: 1 = mean, 2 = max over the clips, then cross entropy (cb_clip_pool_ce_loss)."""
+    if deterministic():
+        clip_pool_ce_loss_det(logits, labels, loss, dlogits, n_clips, nseq, ncls, pool, grad_scale,
+                              _scratch(clip_loss_scratch_bytes(nseq), logits))
+        return
     _call("cb_clip_pool_ce_loss", _p(logits), _p(labels), _p(loss), _p(dlogits), n_clips, nseq, ncls, pool, grad_scale, _s())
+
+
+def clip_loss_scratch_bytes(nseq):
+    return int(_fn("cb_clip_loss_scratch_bytes")(nseq))
+
+
+def clip_lse_loss_det(logits, labels, loss, dlogits, n_clips, nseq, ncls, grad_scale, scratch):
+    _call("cb_clip_lse_loss_det", _p(logits), _p(labels), _p(loss), _p(dlogits), n_clips, nseq, ncls, grad_scale, _p(scratch),
+          scratch.numel() * 4, _s())
+
+
+def clip_pool_ce_loss_det(logits, labels, loss, dlogits, n_clips, nseq, ncls, pool, grad_scale, scratch):
+    _call("cb_clip_pool_ce_loss_det", _p(logits), _p(labels), _p(loss), _p(dlogits), n_clips, nseq, ncls, pool, grad_scale,
+          _p(scratch), scratch.numel() * 4, _s())
 
 
 def cross_entropy_fwd(logits, labels, loss, lse, ignore_index=-100):
@@ -386,7 +522,28 @@ def cross_entropy_bwd(logits, labels, lse, grad_loss, dlogits, ignore_index=-100
 
 
 def colsum(x, out, m, n, ld=None):
+    if deterministic():
+        colsum_det(x, out, m, n, ld, _scratch(colsum_scratch_bytes(m, n), x))
+        return
     _call("cb_colsum", _p(x), n if ld is None else ld, _p(out), m, n, _s())
+
+
+def colsum_scratch_bytes(m, n):
+    return int(_fn("cb_colsum_scratch_bytes")(m, n))
+
+
+def colsum_det(x, out, m, n, ld, scratch):
+    """cb_colsum_det: column sums added in slab order through ``scratch`` (fp32)."""
+    _call("cb_colsum_det", _p(x), n if ld is None else ld, _p(out), m, n, _p(scratch), scratch.numel() * 4, _s())
+
+
+def sumsq_scratch_bytes(n, chunks, nchunks):
+    return int(_fn("cb_sumsq_scratch_bytes")(n, _p(chunks), nchunks))
+
+
+def sumsq_det(x, n, chunks, nchunks, out, scratch):
+    """cb_sumsq_det: out[0] += sum of x^2 (chunk table or x[0, n)), block partials added in a fixed order."""
+    _call("cb_sumsq_det", _p(x), n, _p(chunks), nchunks, _p(out), _p(scratch), scratch.numel() * 4, _s())
 
 
 def dropout(x, y, p, seed):

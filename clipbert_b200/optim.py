@@ -21,6 +21,7 @@ import torch
 from torch.optim import Optimizer
 
 from . import _lib as L
+from . import ops
 
 CHUNK = 65536
 
@@ -51,7 +52,11 @@ def _p(t):
 
 
 def sumsq(x, chunks, nchunks, out):
-    """cb_sumsq: out[0] += sum of x^2 over the chunk table's elements (include/clipbert_b200.h)."""
+    """cb_sumsq: out[0] += sum of x^2 over the chunk table's elements (include/clipbert_b200.h); cb_sumsq_det under
+    torch.use_deterministic_algorithms(True)."""
+    if ops.deterministic():
+        ops.sumsq_det(x, x.numel(), chunks, nchunks, out, ops._scratch(ops.sumsq_scratch_bytes(x.numel(), chunks, nchunks), x))
+        return
     L.check(_cfn("cb_sumsq")(_p(x), x.numel(), _p(chunks), nchunks, _p(out), torch.cuda.current_stream().cuda_stream), "cb_sumsq")
 
 

@@ -47,6 +47,22 @@ int64_t cb_launch_count(void);
  * ordered cuDNN/cuBLAS/ATen kernels, SURVEY.md section 8 a1). */
 int cb_set_pdl(int enable);
 
+/* Deterministic mode (default OFF; the Python package mirrors torch.are_deterministic_algorithms_enabled() into it). While it is
+ * on, every accumulation of the library runs in a fixed order, so a training step gives the same bits on every run on the same
+ * device model and build, whatever the grid cap (cb_debug_gemm_sm_limit), PDL setting, stream placement or co-running work:
+ *   - CB_GEMM_WGRAD (cb_gemm, cb_gemm_wgrad_group): the K-split is chosen from the problem shape and the device's SM count only.
+ *     With one split every output element gets one red.add (order-free). With S > 1 splits, split s writes its scaled partial
+ *     tile with plain stores to plane s of the caller's workspace (fp32 [S][m][ntaps * n]) and a second launch adds the planes
+ *     to out in split order 0..S-1: out + (p_0 + p_1 + ... + p_{S-1}) evaluated as ((out + p_0) + p_1) + ... . The workspace is
+ *     cb_gemm_desc.workspace / workspace_bytes (cb_gemm_workspace_bytes; for a group descs[0]'s,
+ *     cb_gemm_wgrad_group_workspace_bytes); a call without enough returns CB_ERR_INVALID.
+ *   - the entry points that add into fp32 gradients / scalars with atomics (cb_layernorm_bwd with dgamma / dbeta / dbias_drop,
+ *     cb_embed_text_bwd, cb_embed_visual_bwd, cb_colsum, cb_sumsq, cb_clip_lse_loss, cb_clip_pool_ce_loss) return
+ *     CB_ERR_INVALID; their _det variants below, which take a caller-owned scratch, are used instead. A _det variant sums in
+ *     its stated order whether or not the mode is on.
+ * Returns the previous setting. */
+int cb_set_deterministic(int enable);
+
 /* Dropout stream position in DEVICE memory. The reference draws a fresh mask at every nn.Dropout call
  * (src/modeling/transformers.py:170,222,295,375; modeling.py:57,552). Here a mask is a pure function of
  * (seed, element index) and every mask-drawing entry point takes the seed BY VALUE, so a captured CUDA graph would
@@ -153,15 +169,21 @@ typedef struct cb_gemm_desc {
                        a 128 x 256 tile would need 256 fp32 accumulators per thread of the warpgroup that owns it, more
                        than its 232 registers, so an explicit 256 for TN / NN runs on 128-wide tiles */
   int32_t reserved; /* tuning / test knobs: bits 8-11 k-chunks per pipeline stage (0 = automatic); other bits ignored */
+  void* workspace;  /* deterministic mode, CB_GEMM_WGRAD: fp32 split planes, 16-byte aligned (NULL / ignored otherwise) */
+  int64_t workspace_bytes;
 } cb_gemm_desc;
 
 int cb_gemm(const cb_gemm_desc* desc, void* stream);
+/* bytes of workspace a CB_GEMM_WGRAD descriptor needs in deterministic mode (0: one K-split, or not a weight gradient) */
+int64_t cb_gemm_workspace_bytes(const cb_gemm_desc* desc);
 /* n independent CB_GEMM_WGRAD problems in ONE persistent launch: the weight gradients of the four Linear layers of a BertLayer
  * (autograd of transformers.py:238-301,363-381) or of the convs of one bottleneck block. The problems should share their
  * reduction length k (tokens / pixels); 1 <= n <= 8. One prologue and tail instead of n, no K-split when the group fills the SMs.
  * Falls back to n cb_gemm launches for n == 1, n > 8 or very different k. descs[0].block_n / split_k, when non-zero, set the tile
  * width / K-split of the whole group. Other epilogue fields than scale / out are ignored. */
 int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* stream);
+/* the same for a group; the group reads its whole workspace from descs[0] (the problems' split planes one after another) */
+int64_t cb_gemm_wgrad_group_workspace_bytes(const cb_gemm_desc* descs, int n);
 
 /* ------------------------------------------------------------------------------------------
  * LayerNorm over rows of a bf16 [m, 768] matrix (fp32 statistics, warp-shuffle reductions).
@@ -178,6 +200,12 @@ int cb_layernorm_fwd(const void* x, const float* gamma, const float* beta, void*
 int cb_layernorm_bwd(const void* dy, const void* x, const float* stats, const float* gamma, void* dx, void* dx_drop,
                      float* dgamma, float* dbeta, float* dbias_drop, int m, int hidden, float dropout_p,
                      uint64_t dropout_seed, void* stream);
+/* Deterministic: the same kernel with B = min(ceil(m / 4), 264) blocks; block b stores its column sums (its four warps added in
+ * warp order) to scratch row b of each output, and dgamma[c] += ((row_0[c] + row_1[c]) + ...) + row_{B-1}[c], blocks in order. */
+int64_t cb_layernorm_bwd_scratch_bytes(int m);
+int cb_layernorm_bwd_det(const void* dy, const void* x, const float* stats, const float* gamma, void* dx, void* dx_drop,
+                         float* dgamma, float* dbeta, float* dbias_drop, int m, int hidden, float dropout_p,
+                         uint64_t dropout_seed, float* scratch, int64_t scratch_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Embeddings. out is the bf16 [nseq * l, 768] encoder input; text rows go to positions [0, lt),
@@ -207,6 +235,23 @@ int cb_embed_visual_bwd(const void* dh, const void* grid, const int32_t* seq2vid
                         const float* stats, float* dv_tmp, void* dgrid, float* drow, float* dcol, float* dtype0,
                         float* dgamma, float* dbeta, int nseq, int nvid, int t, int gh, int gw, int lt, int l, int hidden,
                         float dropout_p, uint64_t seed, void* stream);
+/* Deterministic backwards. The blocks of the kernels above (P = min(max(ceil(nseq / 8), 1), 32) per text position / grid cell)
+ * store their parameter partials to scratch instead of adding them; each output is then the sum of its blocks' rows in block
+ * order (cell, then x): dgamma, dbeta and d type[0] over every block, d pos[t] over the blocks of position t, d row[r] over the
+ * cells of grid row r in column order, d col[c] over the cells of grid column c in row order. The text backward also stores
+ * every row's fp32 word gradient; each table row word[id] then receives the sum of the rows carrying id, in row order
+ * (b * lt + t), added once. Scratch: cb_embed_*_bwd_scratch_bytes. */
+int64_t cb_embed_text_bwd_scratch_bytes(int nseq, int lt);
+int cb_embed_text_bwd_det(const void* dh, const int64_t* ids, const float* word, const float* pos, const float* type0,
+                          const float* gamma, const float* stats, float* dword, float* dpos, float* dtype0, float* dgamma,
+                          float* dbeta, int nseq, int lt, int l, int vocab, int hidden, float dropout_p, uint64_t seed,
+                          float* scratch, int64_t scratch_bytes, void* stream);
+int64_t cb_embed_visual_bwd_scratch_bytes(int nseq, int gh, int gw);
+int cb_embed_visual_bwd_det(const void* dh, const void* grid, const int32_t* seq2vid, const int32_t* vid_start, int n_ex,
+                            const float* rowemb, const float* colemb, const float* type0, const float* gamma,
+                            const float* stats, float* dv_tmp, void* dgrid, float* drow, float* dcol, float* dtype0,
+                            float* dgamma, float* dbeta, int nseq, int nvid, int t, int gh, int gw, int lt, int l, int hidden,
+                            float dropout_p, uint64_t seed, float* scratch, int64_t scratch_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Fused self-attention, BertSelfAttention.forward (transformers.py:230-286):
@@ -244,6 +289,10 @@ int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t* text_mask
  *                 conv weight: w'[o, :] = w[o, :] * gamma[o] * rsqrt(var[o] + 1e-5), d2 FrozenBatchNorm2d)
  * ------------------------------------------------------------------------------------------ */
 int cb_colsum(const void* x, int64_t ld, float* out, int m, int n, void* stream);
+/* deterministic: slab s of 128 rows stores its column sums (rows added in the kernel's order) to scratch row s, then
+ * out[c] += ((slab_0[c] + slab_1[c]) + ...), slabs in order */
+int64_t cb_colsum_scratch_bytes(int m, int n);
+int cb_colsum_det(const void* x, int64_t ld, float* out, int m, int n, float* scratch, int64_t scratch_bytes, void* stream);
 int cb_dropout(const void* x, void* y, int64_t n, float p, uint64_t seed, void* stream);
 /* dx = dy * gelu'(u): backward of BertPredictionHeadTransform's activation (transformers.py:486-495) */
 int cb_gelu_bwd(const void* dy, const void* u, void* dx, int64_t n, void* stream);
@@ -308,6 +357,13 @@ int cb_clip_lse_loss(const float* logits, const int64_t* labels, float* loss, fl
  * logits.mean(0) / logits.max(0)[0] followed by F.cross_entropy(reduction="none").mean(); same tensors as cb_clip_lse_loss */
 int cb_clip_pool_ce_loss(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq, int ncls, int pool,
                          float grad_scale, void* stream);
+/* deterministic: block b (256 examples) stores its share of the mean to scratch[b], then loss[0] = the ordered sum of the
+ * ceil(nseq / 256) shares (thread t adds shares t, t + 256, ...; warps by xor butterfly; warp sums in warp order) */
+int64_t cb_clip_loss_scratch_bytes(int nseq);
+int cb_clip_lse_loss_det(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq, int ncls,
+                         float grad_scale, float* scratch, int64_t scratch_bytes, void* stream);
+int cb_clip_pool_ce_loss_det(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq, int ncls,
+                             int pool, float grad_scale, float* scratch, int64_t scratch_bytes, void* stream);
 /* F.cross_entropy(logits, labels, reduction="none") over `rows` rows of `ncls` fp32 logits (row pitch ld), labels int64 with
  * ignore_index (-100: loss 0, no gradient): the masked-LM loss over the vocabulary (src/modeling/modeling.py:286-299), the
  * ITM / multiple-choice / retrieval CE (:560-580, :430-436). fwd: loss[rows], lse[rows] (stash). bwd: dlogits[r, c] =
@@ -344,6 +400,11 @@ int cb_nvls_allreduce_f32(void* multicast_ptr, int64_t n, int rank, int world, f
  *         beta1, beta2, eps, 0, 0  - refreshed by the caller each step, so the launch itself is graph-capturable.
  * ------------------------------------------------------------------------------------------ */
 int cb_sumsq(const float* x, int64_t n, const int64_t* chunks, int nchunks, float* out, void* stream);
+/* deterministic: block b (one per chunk-table row, else min(ceil(n / 1024), 1056) grid-stride blocks) stores its sum to
+ * scratch[b], then out[0] += the ordered sum of the partials (as cb_clip_lse_loss_det) */
+int64_t cb_sumsq_scratch_bytes(int64_t n, const int64_t* chunks, int nchunks);
+int cb_sumsq_det(const float* x, int64_t n, const int64_t* chunks, int nchunks, float* out, float* scratch, int64_t scratch_bytes,
+                 void* stream);
 int cb_adamw_step(float* master, float* grad, float* exp_avg, float* exp_avg_sq, void* packed_bf16, const int64_t* chunks,
                   int nchunks, const float* hyper, const float* scales, const float* grad_sumsq, float max_norm, int zero_grad,
                   void* stream);
