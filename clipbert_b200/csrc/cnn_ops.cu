@@ -148,6 +148,10 @@ __global__ void __launch_bounds__(256) resize_pad_kernel(const TIn* __restrict__
   y[t] = v;
 }
 
+// ATen's max-pool update (max_pool2d_with_indices): a value replaces the running maximum when it is larger or NaN, so NaN
+// propagates (fmaxf would drop it) and, among equal maxima, the first one in window order stays
+__device__ __forceinline__ bool pool_takes(float v, float best) { return v > best || v != v; }
+
 // 3x3 stride-2 pad-1 max pool, NHWC
 __global__ void maxpool3x3s2_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H, int W,
                                     int C, int Ho, int Wo, int64_t row_pitch /* pixels */, int64_t img_pitch /* pixels */) {
@@ -174,7 +178,7 @@ __global__ void maxpool3x3s2_kernel(const __nv_bfloat16* __restrict__ x, __nv_bf
       float f[8];
       unpack8(*reinterpret_cast<const uint4*>(x + (static_cast<int64_t>(n) * img_pitch + iy * row_pitch + ix) * C + c8 * 8), f);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) m[j] = fmaxf(m[j], f[j]);
+      for (int j = 0; j < 8; ++j) m[j] = pool_takes(f[j], m[j]) ? f[j] : m[j];
     }
   }
   *reinterpret_cast<uint4*>(y + pix * C + c8 * 8) = pack8(m);
@@ -235,7 +239,7 @@ __global__ void maxpool2x2_relu_fwd_kernel(const __nv_bfloat16* __restrict__ x, 
   const int n = static_cast<int>(pix / (static_cast<int64_t>(Wo) * Ho));
   float m[8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) m[j] = 0.f;  // ReLU folded: max(0, window max)
+  for (int j = 0; j < 8; ++j) m[j] = 0.f;  // ReLU folded: max(+0, window max); a window of zeros / -0 gives +0, a NaN gives NaN
 #pragma unroll
   for (int r = 0; r < 2; ++r)
 #pragma unroll
@@ -243,7 +247,7 @@ __global__ void maxpool2x2_relu_fwd_kernel(const __nv_bfloat16* __restrict__ x, 
       float f[8];
       unpack8(*reinterpret_cast<const uint4*>(x + ((static_cast<int64_t>(n) * H + 2 * oy + r) * W + 2 * ox + s) * C + c8 * 8), f);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) m[j] = fmaxf(m[j], f[j]);
+      for (int j = 0; j < 8; ++j) m[j] = pool_takes(f[j], m[j]) ? f[j] : m[j];
     }
   *reinterpret_cast<uint4*>(y + pix * C + c8 * 8) = pack8(m);
 }
@@ -279,13 +283,13 @@ __global__ void maxpool2x2_relu_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
           unpack8(*reinterpret_cast<const uint4*>(x + ((static_cast<int64_t>(n) * H + 2 * oy + r) * W + 2 * ox + s) * C + c8 * 8), f);
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            if (f[j] > best[j]) { best[j] = f[j]; arg[j] = r * 2 + s; }  // first maximum wins (ATen semantics)
+            if (pool_takes(f[j], best[j])) { best[j] = f[j]; arg[j] = r * 2 + s; }  // ATen's arg-max: first maximum, last NaN
         }
       const int me = (yy - 2 * oy) * 2 + (xx - 2 * ox);
       float g[8];
       unpack8(*reinterpret_cast<const uint4*>(dy + ((static_cast<int64_t>(n) * Ho + oy) * Wo + ox) * C + c8 * 8), g);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) g[j] = (arg[j] == me && best[j] > 0.f) ? g[j] : 0.f;
+      for (int j = 0; j < 8; ++j) g[j] = (arg[j] == me && best[j] > 0.f) ? g[j] : 0.f;   // ReLU' = (max > 0), as every mask here
       o = pack8(g);
     }
   }

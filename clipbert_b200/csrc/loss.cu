@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restr
   for (int c = threadIdx.x; c < ncls; c += CE_THREADS) {      // online softmax statistics: one pass over the row
     const float v = z[c];
     if (v > m) { s = s * __expf(m - v) + 1.f; m = v; }
-    else s += __expf(v - m);
+    else if (v != -INFINITY) s += __expf(v - m);   // (a -inf logit adds exp(-inf) = 0; while m is still -inf, exp(-inf + inf) is NaN)
   }
   __shared__ float sm[CE_THREADS / 32], ss[CE_THREADS / 32];
   const float wm = warp_max(m);

@@ -287,6 +287,9 @@ int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t* text_mask
  *   cb_pad_cast   fp32 [rows, c] -> bf16 [rows, cpad] zero padded (d logits -> padded head gradient)
  *   cb_cast_scale fp32 -> bf16 operand packing, optional per-row scale (FrozenBN scale folded into the
  *                 conv weight: w'[o, :] = w[o, :] * gamma[o] * rsqrt(var[o] + 1e-5), d2 FrozenBatchNorm2d)
+ * The packed value is the fp32 product rounded to nearest even (as w * s followed by .to(bfloat16)), except that the library
+ * is built with flush-to-zero: a product below 2^-126 in magnitude packs as a zero of its sign (also cb_cast_scale_segments
+ * and the packed copy of cb_adamw_step).
  * ------------------------------------------------------------------------------------------ */
 int cb_colsum(const void* x, int64_t ld, float* out, int m, int n, void* stream);
 /* deterministic: slab s of 128 rows stores its column sums (rows added in the kernel's order) to scratch row s, then
@@ -294,7 +297,9 @@ int cb_colsum(const void* x, int64_t ld, float* out, int m, int n, void* stream)
 int64_t cb_colsum_scratch_bytes(int m, int n);
 int cb_colsum_det(const void* x, int64_t ld, float* out, int m, int n, float* scratch, int64_t scratch_bytes, void* stream);
 int cb_dropout(const void* x, void* y, int64_t n, float p, uint64_t seed, void* stream);
-/* dx = dy * gelu'(u): backward of BertPredictionHeadTransform's activation (transformers.py:486-495) */
+/* dx = dy * gelu'(u): backward of BertPredictionHeadTransform's activation (transformers.py:486-495). erf is fast_erf
+ * (Abramowitz-Stegun 7.1.26, |error| <= 1.5e-7): within 1 bf16 ulp of the exact result plus |dy| * (0.75e-7 + 4 * 2^-24),
+ * the floor that dominates the left tail where gelu' ~ 1e-6. u = +-inf gives NaN, as ATen's gelu backward (inf * pdf = inf * 0). */
 int cb_gelu_bwd(const void* dy, const void* u, void* dx, int64_t n, void* stream);
 int cb_pad_cast(const float* in, int64_t in_ld, void* out, int rows, int c, int cpad, void* stream);
 int cb_cast_scale(const float* in, const float* rowscale, int64_t row_len, void* out, int64_t n, void* stream);
@@ -326,6 +331,13 @@ int cb_cast_scale_segments(const float* master, void* packed, const int64_t* seg
  *   cb_maxpool2x2_relu_fwd  grid_encoder MaxPool2d(2,2) + ReLU (7x7 -> 3x3 at 224 px, 14x14 -> 7x7 at 448)
  *   cb_maxpool2x2_relu_bwd  its backward, written into the zero-bordered layout read by the 3x3 dgrad/wgrad
  *   cb_relu_mask            dx = dy * (act > 0)
+ * The pools follow F.max_pool2d (max_pool2d_with_indices): a value replaces the running maximum when it is larger or NaN, so a
+ * NaN in a window propagates (a NaN / inf from an overflowing bf16 conv reaches the loss as in the reference), equal maxima keep
+ * the first in window order (the sign of a zero maximum is ATen's), and the 2x2 backward sends the gradient to that arg-max
+ * (first maximum; last NaN). Two differences are pinned: the 2x2 forward writes +0 where the window maximum is -0 (ATen's ReLU
+ * keeps -0), and ReLU' is (act > 0) in every ReLU backward of the library (the 2x2 backward on the window maximum,
+ * cb_unsubsample2_mask, cb_relu_mask and CB_AUX_RELU_MASK alike), so a NaN activation gets gradient 0 where ATen's
+ * threshold_backward passes it on. The forward already carries the NaN into the loss; one rule keeps the three paths equal.
  * ------------------------------------------------------------------------------------------ */
 /* Frame resize + pad of the data pipeline (src/datasets/data_utils.py:202-234 ImageResize: F.interpolate(bilinear,
  * align_corners=False) to new_h x new_w, longer side = max_size; :136-160 ImagePad: zeros at the bottom / right up to
@@ -354,7 +366,9 @@ int cb_relu_mask(const void* dy, const void* act, void* dx, int64_t n, void* str
 int cb_clip_lse_loss(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq, int ncls,
                      float grad_scale, void* stream);
 /* pool_method "mean" (pool = 1) / "max" (pool = 2) of the same loops (run_video_retrieval.py:405-408, run_video_qa.py:485-488):
- * logits.mean(0) / logits.max(0)[0] followed by F.cross_entropy(reduction="none").mean(); same tensors as cb_clip_lse_loss */
+ * logits.mean(0) / logits.max(0)[0] followed by F.cross_entropy(reduction="none").mean(); same tensors as cb_clip_lse_loss.
+ * For max, among clips with exactly equal logits the FIRST receives the gradient. Both clip losses clamp a label outside
+ * [0, ncls) to 0 or ncls - 1 instead of raising as torch.gather / F.cross_entropy would. */
 int cb_clip_pool_ce_loss(const float* logits, const int64_t* labels, float* loss, float* dlogits, int n_clips, int nseq, int ncls, int pool,
                          float grad_scale, void* stream);
 /* deterministic: block b (256 examples) stores its share of the mean to scratch[b], then loss[0] = the ordered sum of the
@@ -367,7 +381,8 @@ int cb_clip_pool_ce_loss_det(const float* logits, const int64_t* labels, float* 
 /* F.cross_entropy(logits, labels, reduction="none") over `rows` rows of `ncls` fp32 logits (row pitch ld), labels int64 with
  * ignore_index (-100: loss 0, no gradient): the masked-LM loss over the vocabulary (src/modeling/modeling.py:286-299), the
  * ITM / multiple-choice / retrieval CE (:560-580, :430-436). fwd: loss[rows], lse[rows] (stash). bwd: dlogits[r, c] =
- * grad_loss[r] * (softmax(z)[c] - [c == y]) with row pitch dld. One block per row, one pass over the row each. */
+ * grad_loss[r] * (softmax(z)[c] - [c == y]) with row pitch dld. One block per row, one pass over the row each. A label outside
+ * [0, ncls) is treated as ignore_index (loss 0, no gradient) instead of raising. -inf logits contribute exp(-inf) = 0. */
 int cb_cross_entropy_fwd(const float* logits, int64_t ld, const int64_t* labels, float* loss, float* lse, int64_t rows, int ncls,
                          int64_t ignore_index, void* stream);
 int cb_cross_entropy_bwd(const float* logits, int64_t ld, const int64_t* labels, const float* lse, const float* grad_loss, float* dlogits,

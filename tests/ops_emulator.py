@@ -338,25 +338,27 @@ def unsubsample2_mask(dsub, act, dx, n, h, w, c):
     ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
     full = torch.zeros(n, h, w, c, dtype=F32)
     full[:, ::2, ::2] = dsub.view(n, ho, wo, c).to(F32)
-    dx.view(-1).copy_((full * (act.view(n, h, w, c).to(F32) > 0)).reshape(-1))
+    dx.view(-1).copy_(torch.where(act.view(n, h, w, c).to(F32) > 0, full, torch.zeros_like(full)).reshape(-1))
 
 
 def maxpool2x2_relu_fwd(x, y, n, h, w, c):
     o = F.max_pool2d(x.view(n, h, w, c).to(F32).permute(0, 3, 1, 2), 2, 2).permute(0, 2, 3, 1)
-    y.view(-1).copy_(torch.relu(o).reshape(-1))
+    y.view(-1).copy_((torch.relu(o) + 0.0).reshape(-1))       # + 0.0: a -0 maximum gives +0, as the kernel
 
 
 def maxpool2x2_relu_bwd(dy, x, dx_pad, n, h, w, c):
     xv = x.view(n, h, w, c).to(F32).permute(0, 3, 1, 2).clone().requires_grad_(True)
     with torch.enable_grad():
-        torch.relu(F.max_pool2d(xv, 2, 2)).backward(dy.view(n, h // 2, w // 2, c).to(F32).permute(0, 3, 1, 2))
+        o = F.max_pool2d(xv, 2, 2)          # ReLU' = (max > 0): a NaN maximum gets no gradient, as every mask of the library
+        up = dy.view(n, h // 2, w // 2, c).to(F32).permute(0, 3, 1, 2)
+        o.backward(torch.where(o.detach() > 0, up, torch.zeros_like(up)))
     pad = torch.zeros(n, h + 2, w + 2, c, dtype=F32)
     pad[:, 1:-1, 1:-1] = xv.grad.permute(0, 2, 3, 1)
     dx_pad.view(-1).copy_(pad.reshape(-1))
 
 
 def relu_mask(dy, act, dx):
-    dx.view(-1).copy_((dy.to(F32) * (act.to(F32) > 0)).reshape(-1))
+    dx.view(-1).copy_(torch.where(act.to(F32) > 0, dy.to(F32), torch.zeros((), dtype=F32)).reshape(-1))
 
 
 def clip_lse_loss(logits, labels, loss, dlogits, n_clips, nseq, ncls, grad_scale=1.0):
@@ -364,7 +366,7 @@ def clip_lse_loss(logits, labels, loss, dlogits, n_clips, nseq, ncls, grad_scale
     with torch.enable_grad():
         lg = z.permute(1, 0, 2)
         out = torch.logsumexp(lg.reshape(nseq, -1), dim=-1, keepdim=True) - torch.logsumexp(lg, dim=1)
-        val = torch.gather(out, -1, labels.view(-1, 1)).mean()
+        val = torch.gather(out, -1, labels.clamp(0, ncls - 1).view(-1, 1)).mean()
         if dlogits is not None:
             val.backward()
             dlogits.copy_(z.grad * grad_scale)
@@ -430,8 +432,12 @@ def opt_adamw_step(master, grad, exp_avg, exp_avg_sq, packed, chunks, nchunks, h
 
 def clip_pool_ce_loss(logits, labels, loss, dlogits, n_clips, nseq, ncls, pool, grad_scale=1.0):
     z = logits.detach().double().requires_grad_(True)
-    pooled = z.mean(0) if pool == 1 else z.max(0)[0]
-    v = torch.nn.functional.cross_entropy(pooled, labels, reduction="none").mean()
+    if pool == 1:
+        pooled = z.mean(0)
+    else:                                   # the first maximal clip takes the gradient (torch.argmax returns the first)
+        first = (z == z.max(0, keepdim=True)[0]).double().argmax(0, keepdim=True)
+        pooled = z.gather(0, first)[0]
+    v = torch.nn.functional.cross_entropy(pooled, labels.clamp(0, ncls - 1), reduction="none").mean()
     v.backward()
     loss.copy_(v.detach().float().reshape(1))
     if dlogits is not None:
@@ -440,8 +446,11 @@ def clip_pool_ce_loss(logits, labels, loss, dlogits, n_clips, nseq, ncls, pool, 
 
 def cross_entropy_fwd(logits, labels, loss, lse, ignore_index=-100):
     z = logits.double()
-    lse.copy_(torch.logsumexp(z, -1).float())
-    loss.copy_(torch.nn.functional.cross_entropy(z, labels, reduction="none", ignore_index=ignore_index).float())
+    ls = torch.logsumexp(z, -1)
+    lse.copy_(ls.float())
+    ok = (labels != ignore_index) & (labels >= 0) & (labels < z.shape[1])      # ignored and out-of-range labels: loss 0
+    zy = z.gather(1, labels.clamp(0, z.shape[1] - 1).view(-1, 1))[:, 0]
+    loss.copy_(torch.where(ok, ls - zy, torch.zeros_like(ls)).float())
 
 
 def cross_entropy_bwd(logits, labels, lse, grad_loss, dlogits, ignore_index=-100):
