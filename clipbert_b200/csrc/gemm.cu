@@ -4,7 +4,7 @@
 //                    (3x3 conv over a zero-bordered NHWC activation); fused epilogue.
 //   MODE 2 (NN)    : as TN but B [K, ntaps*N] is read MN-major (dgrad straight from the forward weight).
 //   MODE 1 (WGRAD) : dW = dY^T X with both operands read MN-major from the activation layout,
-//                    split over the pixel/token dimension, fp32 red.global accumulation.
+//                    optionally split over the pixel/token dimension, fp32 red.global accumulation.
 //
 // Every kernel is persistent (grid = min(#tiles, #SMs x CTAs per SM), static round-robin tile schedule) and fills a shared-memory
 // ring of STAGES x KCH x (A 128x64 | B BNx64) bf16 k-chunks, 128B swizzle, from ONE elected TMA producer lane.
@@ -32,10 +32,11 @@
 //                 tile's operands (plan_smem). Reading them with per-lane global loads inside the epilogue left four dependent
 //                 HBM round trips per tile and warp exposed on the one-chunk main loops of the HBM-bound 1x1 convs.
 //
-// WGRAD: gemm_kernel (and wgrad_group_kernel below), 288 threads: warp 8 is the TMA producer, warps 0..7 two consumer
-//   warpgroups that multiply rows 64g .. 64g+63 of one 128 x BN tile (BN up to 256) with wgmma m64nBNk16, hand every ring stage
-//   back as soon as the products that read it have retired (one stage of wgmma stays in flight), then add the tile into the fp32
-//   output with red.global.add.v2.f32 straight from the fragment (four lanes cover 32 contiguous bytes of a row). One CTA per SM.
+// WGRAD: wgrad_group_kernel, 288 threads, one CTA per SM. It walks the tiles of a group of problems; a single weight gradient
+//   (cb_gemm) is a group of one. Warp 8 is the TMA producer, warps 0..7 two consumer warpgroups that multiply rows
+//   64g .. 64g+63 of one 128 x BN tile (BN up to 256) with wgmma m64nBNk16, hand every ring stage back as soon as the products
+//   that read it have retired (one stage of wgmma stays in flight), then add the tile into the fp32 output with
+//   red.global.add.v2.f32 straight from the fragment (four lanes cover 32 contiguous bytes of a row).
 #include <algorithm>
 
 #include "common.cuh"
@@ -77,8 +78,8 @@ struct GemmEpi {
   float drop_inv_keep;
   uint64_t seed;
   const uint64_t* seed_off;   // device word folded into the seed at run time (cb_dropout_offset_bind), or nullptr
-  int mn3d;         // MN-major operands (B of NN mode, A and B of WGRAD mode) arrive as ONE 3-D TMA box per k-chunk instead of
-                    // BN/64 (BM/64) 2-D boxes: tmA / tmB are then the {64, rows, cols/64} maps of get_tmap_3d_mn
+  int mn3d;         // the MN-major B operand of NN mode arrives as ONE 3-D TMA box per k-chunk instead of BN/64 2-D boxes:
+                    // tmB is then the {64, rows, cols/64} map of get_tmap_3d_mn
   long long* dbg;   // optional in-kernel clock64 timeline, 32 slots per CTA (bring-up / tuning only; NULL in production)
 };
 
@@ -281,31 +282,15 @@ __device__ __forceinline__ void epilogue_math(float (&f)[NC], const GemmEpi& epi
 }
 
 struct TileInfo {
-  int m0, n0, nb0, tap, it_begin, n_iters;
+  int m0, n0;
 };
 
-// tile index -> coordinates; n-tiles are fastest so that concurrently running CTAs share the A rows.
-template <int BN, int MODE>
-__device__ __forceinline__ TileInfo decode_tile(int tile, int tiles_m, int tiles_n, int K, int ntaps, int iters_per_split) {
+// TN / NN tile index -> coordinates; n-tiles are fastest so that concurrently running CTAs share the A rows.
+template <int BN>
+__device__ __forceinline__ TileInfo decode_tile(int tile, int tiles_m, int tiles_n) {
   TileInfo t;
-  const int nt = tile % tiles_n;
-  int r = tile / tiles_n;
-  const int mt = r % tiles_m;
-  r /= tiles_m;
-  t.m0 = mt * BM;
-  t.n0 = nt * BN;
-  t.nb0 = t.n0;
-  const int kc = (K + BK - 1) / BK;
-  if (MODE == 1) {
-    t.tap = r % ntaps;
-    const int split = r / ntaps;
-    t.it_begin = split * iters_per_split;
-    t.n_iters = min(kc, t.it_begin + iters_per_split) - t.it_begin;
-  } else {
-    t.tap = 0;
-    t.it_begin = 0;
-    t.n_iters = ntaps * kc;
-  }
+  t.m0 = (tile / tiles_n) % tiles_m * BM;
+  t.n0 = tile % tiles_n * BN;
   return t;
 }
 
@@ -503,7 +488,7 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
       // residual / aux boxes of a tile into its input buffer, or into the next ring stage (N_IN = 0); rows and columns outside
       // [M, N] arrive as zeros
       auto load_inputs = [&](int tile) {
-        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, 0);
+        const TileInfo t = decode_tile<BN>(tile, tiles_m, tiles_n);
         uint64_t* bar;
         uint8_t* dst;
         if (N_IN) {
@@ -532,7 +517,7 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
       };
       int pend = -1;    // tile whose inputs wait for the next tile's operands
       for (int tile = unit; tile < total_tiles; tile += n_units) {
-        const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, 0);
+        const TileInfo t = decode_tile<BN>(tile, tiles_m, tiles_n);
         // A CTA's first N_IN tiles find their input buffer free: their inputs go out ahead of the operands. A later tile's
         // inputs wait for the buffer (the epilogue N_IN tiles back), so they go out after the NEXT tile's operands: that wait
         // never holds back operands the ring has room for, and the inputs still land under the tile's own main loop. In the
@@ -554,12 +539,12 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
             else if (ntaps > 1) shift = tap_sign * tp * tap_w;        // row taps (space-to-depth stem): tap t reads row m + t * tap_w
             tma_load_2d(sa, &tmA, &full_bar[s], kc * BK, t.m0 + shift);
             if (MODE == 0) {
-              tma_load_2d(sb, &tmB, &full_bar[s], tp * K + kc * BK, t.nb0);
+              tma_load_2d(sb, &tmB, &full_bar[s], tp * K + kc * BK, t.n0);
             } else if (epi.mn3d) {
-              tma_load_3d(sb, &tmB, &full_bar[s], 0, kc * BK, (tp * N + t.nb0) >> 6);
+              tma_load_3d(sb, &tmB, &full_bar[s], 0, kc * BK, (tp * N + t.n0) >> 6);
             } else {
 #pragma unroll
-              for (int j = 0; j < B_BOXES; ++j) tma_load_2d(sb + j * (BK * 128), &tmB, &full_bar[s], tp * N + t.nb0 + j * 64, kc * BK);
+              for (int j = 0; j < B_BOXES; ++j) tma_load_2d(sb + j * (BK * 128), &tmB, &full_bar[s], tp * N + t.n0 + j * 64, kc * BK);
             }
             if (++kc == kc_per_tap) { kc = 0; ++tp; }
           }
@@ -614,7 +599,7 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
   const bool guard = (N & 15) != 0;                 // ragged last 16 columns: per-vector column checks in the generic epilogue
 
   for (int local = wg, tile = unit + wg * n_units; tile < total_tiles; local += 2, tile += 2 * n_units) {
-    const TileInfo t = decode_tile<BN, MODE>(tile, tiles_m, tiles_n, K, ntaps, 0);
+    const TileInfo t = decode_tile<BN>(tile, tiles_m, tiles_n);
     if (local > 0) named_bar_sync(PP_BAR_TURN + wg, 2 * 128);         // the other consumer has issued tile local - 1
     const int pass = tile + n_units < total_tiles ? PP_BAR_TURN + (wg ^ 1) : 0;
     mma_tile_pp<BN, MODE != 0>(acc, smem0, stage_bytes, KCH, STAGES, n_iters, lane, s, ph, full_bar, empty_bar, pass, in_stage);
@@ -753,105 +738,6 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
   if (threadIdx.x == 4 * 32) dbg_stamp(epi, 11);
 }
 
-// ===================================== WGRAD =====================================
-// DET: every tile writes its scaled partial into plane `split` of the workspace ws (fp32 [splits][M][ntaps * N]) with plain
-// stores; the planes are added into out afterwards in split order (deterministic mode with a K-split; unused otherwise).
-template <int BN, bool DET = false>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-    gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K, int ntaps, int tap_w,
-                int tap_sign, int iters_per_split, int tiles_m, int tiles_n, int total_tiles, int STAGES, int KCH, GemmEpi epi, float* ws) {
-  using Cfg = GemmCfg<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  const int stage_bytes = KCH * Cfg::STAGE_BYTES;           // a stage holds KCH consecutive 64-deep k-chunks (one barrier round trip)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
-  uint64_t* empty_bar = full_bar + MAX_STAGES;
-
-  // warp-uniform for the compiler: with a plain threadIdx.x >> 5 ptxas takes the consumer path for divergent and serialises
-  // every wgmma behind the warpgroup arrive it inserts (advisory C7520), which leaves one m64nBNk16 in flight per warpgroup
-  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const int unit = blockIdx.x;                                          // persistent work unit
-  const int n_units = gridDim.x;
-  if (threadIdx.x == 0) dbg_stamp(epi, 0);   // (debug-only buffer, not produced by any kernel: safe before pdl_wait)
-  pdl_trigger();   // PDL: let the next kernel's CTAs take this SM as soon as this CTA leaves it
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CONSUMER_WARPS);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  // PDL: barrier init and descriptor prefetch above overlapped the previous kernel's tail; from here on this kernel touches
-  // global memory, so its producers must have completed.
-  pdl_wait();
-  if (threadIdx.x == 0) dbg_stamp(epi, 1);
-
-  if (warp >= CONSUMER_WARPS) {
-    // ===================== TMA producer =====================
-    // One elected lane owns the barriers and issues the TMA boxes of a stage (KCH chunks x {A boxes, B boxes}).
-    if (warp == CONSUMER_WARPS && lane == 0) {
-      int s = 0;        // smem ring position / phase, carried across tiles
-      uint32_t ph = 0;
-      for (int tile = unit; tile < total_tiles; tile += n_units) {
-        const TileInfo t = decode_tile<BN, 1>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-        int shift = 0;
-        if (ntaps == 9) shift = tap_sign * ((t.tap / 3 - 1) * tap_w + (t.tap % 3 - 1));
-        for (int i = 0; i < t.n_iters; i += KCH) {
-          const int nch = min(KCH, t.n_iters - i);
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          mbar_expect_tx(&full_bar[s], nch * Cfg::STAGE_BYTES);
-          int kit = t.it_begin + i;
-          for (int ch = 0; ch < nch; ++ch, ++kit) {
-            uint8_t* sa = smem + s * stage_bytes + ch * Cfg::STAGE_BYTES;
-            uint8_t* sb = sa + Cfg::A_BYTES;
-            const int p = kit * BK;
-            if (epi.mn3d) {
-              tma_load_3d(sa, &tmA, &full_bar[s], 0, p, t.m0 >> 6);
-              tma_load_3d(sb, &tmB, &full_bar[s], 0, p + shift, t.nb0 >> 6);
-            } else {
-#pragma unroll
-              for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), &tmA, &full_bar[s], t.m0 + j * 64, p);
-#pragma unroll
-              for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), &tmB, &full_bar[s], t.nb0 + j * 64, p + shift);
-            }
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-          if (i == 0 && tile == unit) dbg_stamp(epi, 2);
-        }
-      }
-      dbg_stamp(epi, 3);
-    }
-    return;
-  }
-
-  // ===================== consumer warpgroups: wgmma main loop + red.add epilogue =====================
-  const int wg = warp >> 2;                 // rows wg * 64 .. wg * 64 + 63 of the tile
-  const int wrow = wg * 64 + (warp & 3) * 16;   // first of this warp's 16 rows
-  const uint32_t smem0 = smem_u32(smem);
-  float acc[BN / 2];
-  int s = 0;
-  uint32_t ph = 0;
-  int local = 0;
-  for (int tile = unit; tile < total_tiles; tile += n_units, ++local) {
-    const TileInfo t = decode_tile<BN, 1>(tile, tiles_m, tiles_n, K, ntaps, iters_per_split);
-    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 4);
-    mma_tile<BN, 1, 1>(acc, smem0, stage_bytes, KCH, STAGES, t.n_iters, wg, lane, s, ph, full_bar, empty_bar);
-    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 5);
-    if constexpr (DET)
-      wgrad_epilogue<BN, true>(acc, ws + static_cast<int64_t>(t.it_begin / iters_per_split) * M * ntaps * N + static_cast<int64_t>(t.tap) * N,
-                               static_cast<int64_t>(ntaps) * N, epi.scale, M, N, t.m0 + wrow + (lane >> 2), t.n0, lane);
-    else
-      wgrad_epilogue<BN>(acc, reinterpret_cast<float*>(epi.out) + static_cast<int64_t>(t.tap) * N, epi.out_ld, epi.scale, M, N,
-                         t.m0 + wrow + (lane >> 2), t.n0, lane);
-    if (local == 0 && warp == 0 && lane == 0) dbg_stamp(epi, 8);
-  }
-  if (threadIdx.x == 0) dbg_stamp(epi, 11);
-}
-
 static int g_sm_limit = 0;    // tuning hook: cap on the persistent grid (0 = every SM). A long-running co-resident kernel (an NCCL
                               // all-reduce overlapped with the backward pass) pins some SMs for its whole duration; with the static
                               // round-robin tile schedule the CTAs that cannot be placed run as a second wave. Capping the grid at
@@ -875,7 +761,6 @@ static int sm_count() {
 static int plan_sm_count() { return g_det.load(std::memory_order_relaxed) ? sm_count_device() : sm_count(); }
 
 static long long* g_gemm_timeline = nullptr;
-static int g_force_kch = 0;   // tuning hook: chunks per stage (0 = automatic)
 static int g_mn3d = 1;        // 1 (default) = MN-major operands through one 3-D TMA box per k-chunk (GemmEpi::mn3d); cb_debug_gemm_mn3d
 
 
@@ -909,7 +794,6 @@ static SmemPlan plan_ring(int bn, bool staging, int kiters, int force_kch, int i
   const int min_stages = kiters > chunks_fit ? 3 : 2;
   p.kch = 1;
   if (force_kch > 0) p.kch = force_kch;
-  else if (g_force_kch > 0) p.kch = g_force_kch;
   else if (kiters >= 4 && chunks_fit >= 4 * min_stages) p.kch = 4;
   else if (kiters >= 2 && chunks_fit >= 2 * min_stages) p.kch = 2;
   if (p.kch > kiters) p.kch = kiters;
@@ -979,18 +863,13 @@ static int launch_split_reduce(const SplitReduce& r, cudaStream_t stream, const 
   return check_launch(what);
 }
 
-// MODE 0 / 2 (TN / NN): gemm_pingpong_kernel, BN = 64 / 128. MODE 1 (WGRAD): gemm_kernel. One CTA per SM.
-template <int BN, int MODE, bool DET = false>
-static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_t stream, float* ws = nullptr) {
-  static_assert(MODE == 1 || BN <= 128, "TN / NN: 128 x 64 or 128 x 128 tiles");
-  static_assert(MODE == 1 || !DET, "only the weight gradients have a deterministic instantiation");
+// MODE 0 / 2 (TN / NN): gemm_pingpong_kernel, BN = 64 / 128. One CTA per SM.
+template <int BN, int MODE>
+static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_t stream) {
   GemmEpi epi = epi_in;
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
-  auto kern = [] {
-    if constexpr (MODE == 1) return gemm_kernel<BN, DET>;
-    else return gemm_pingpong_kernel<BN, MODE>;
-  }();
+  auto kern = gemm_pingpong_kernel<BN, MODE>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
@@ -1002,42 +881,29 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
   // Tensor maps are copied out of the cache into this frame (and from here into the kernel's parameter space)
   alignas(64) CUtensorMap ta, tb, tr, tx;
   bool mn3d = false;
-  int iters_per_split = 0;
   const int tiles_m = ceil_div(d.m, BM), tiles_n = ceil_div(d.n, BN);
-  int total = tiles_m * tiles_n;
-  int kiters;
-  bool ok;
+  const int total = tiles_m * tiles_n;
+  const int kiters = ceil_div(d.k, BK) * d.ntaps;
+  bool ok = get_tmap_2d(&ta, d.a, d.k, d.a_rows, d.a_ld, BK, BM);
   if (MODE == 0) {
-    ok = get_tmap_2d(&ta, d.a, d.k, d.a_rows, d.a_ld, BK, BM) &&
-         get_tmap_2d(&tb, d.b, static_cast<uint64_t>(d.k) * d.ntaps, d.b_rows, d.b_ld, BK, BN);
-    kiters = ceil_div(d.k, BK) * d.ntaps;
-  } else if (MODE == 2) {
-    ok = get_tmap_2d(&ta, d.a, d.k, d.a_rows, d.a_ld, BK, BM);
+    ok = ok && get_tmap_2d(&tb, d.b, static_cast<uint64_t>(d.k) * d.ntaps, d.b_rows, d.b_ld, BK, BN);
+  } else {
     mn3d = g_mn3d && d.n % 64 == 0 &&
            get_tmap_3d_mn(&tb, d.b, static_cast<uint64_t>(d.n) * d.ntaps, d.b_rows, d.b_ld, BK, BN / 64);
     // not asked for, or the driver refused the 3-D view: the 2-D boxes always work
     if (!mn3d) ok = ok && get_tmap_2d(&tb, d.b, static_cast<uint64_t>(d.n) * d.ntaps, d.b_rows, d.b_ld, 64, BK);
-    kiters = ceil_div(d.k, BK) * d.ntaps;
-  } else {
-    mn3d = g_mn3d && d.m % 64 == 0 && d.n % 64 == 0 && get_tmap_3d_mn(&ta, d.a, d.m, d.a_rows, d.a_ld, BK, BM / 64) &&
-           get_tmap_3d_mn(&tb, d.b, d.n, d.b_rows, d.b_ld, BK, BN / 64);
-    ok = mn3d || (get_tmap_2d(&ta, d.a, d.m, d.a_rows, d.a_ld, 64, BK) && get_tmap_2d(&tb, d.b, d.n, d.b_rows, d.b_ld, 64, BK));
-    const int kc = ceil_div(d.k, BK);
-    iters_per_split = ceil_div(kc, real_splits(kc, d.split_k));
-    total *= real_splits(kc, d.split_k) * d.ntaps;
-    kiters = iters_per_split;
   }
-  // epilogue inputs (TN / NN): residual / aux [M, N] at the tile's A rows, 128 x 64 boxes; unused map slots carry a copy of ta
+  // epilogue inputs: residual / aux [M, N] at the tile's A rows, 128 x 64 boxes; unused map slots carry a copy of ta
   tr = ta;
   tx = ta;
-  if (MODE != 1 && d.residual) ok = ok && get_tmap_2d(&tr, d.residual, d.n, d.m, d.res_ld, 64, BM);
-  if (MODE != 1 && d.aux) ok = ok && get_tmap_2d(&tx, d.aux, d.n, d.m, d.aux_ld, 64, BM);
+  if (d.residual) ok = ok && get_tmap_2d(&tr, d.residual, d.n, d.m, d.res_ld, 64, BM);
+  if (d.aux) ok = ok && get_tmap_2d(&tx, d.aux, d.n, d.m, d.aux_ld, 64, BM);
   if (!ok) return CB_ERR_CUDA;
   epi.mn3d = mn3d ? 1 : 0;
   const int units = sm_count();
   const int grid = total < units ? total : units;
   const int in_bytes = epi_in_bytes(d, BN);
-  const SmemPlan sp = plan_smem(BN, MODE != 1, kiters, (d.reserved >> 8) & 15, in_bytes);
+  const SmemPlan sp = plan_smem(BN, true, kiters, (d.reserved >> 8) & 15, in_bytes);
   const int kch = sp.kch, stages = sp.stages;
   if (stages < 2) {
     set_error("cb_gemm: not enough shared memory for a 2-stage pipeline (BN=%d, epilogue %d B + inputs %d B)", BN, sp.epi_bytes,
@@ -1045,12 +911,8 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
     return CB_ERR_INVALID;
   }
   const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + sp.n_in * in_bytes + sp.epi_bytes + Cfg::BAR_BYTES + 1024;
-  if constexpr (MODE == 1)
-    launch_gemm_k(kern, grid, GEMM_THREADS, smem_bytes, stream, ta, tb, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, iters_per_split,
-                  tiles_m, tiles_n, total, stages, kch, epi, ws);
-  else
-    launch_gemm_k(kern, grid, PP_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, tiles_m,
-                  tiles_n, total, stages, kch, sp.n_in, epi);
+  launch_gemm_k(kern, grid, PP_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, tiles_m,
+                tiles_n, total, stages, kch, sp.n_in, epi);
   return check_launch("cb_gemm");
 }
 
@@ -1112,13 +974,13 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, int units) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Grouped weight gradients: ONE persistent launch walks the tiles of several independent dW = dY^T X problems (the four
-// Linear layers of a BertLayer, the three / four convs of a bottleneck block). The problems of a group share the reduction
-// length (tokens / pixels), so their tiles cost the same and the static round-robin schedule stays balanced; what the group buys
-// is one prologue + one tail instead of four, tiles of all problems filling the SMs together, and - because four problems
-// together have enough tiles - no K-split, i.e. half the fp32 red.global traffic of the single launches. Same warp roles, ring
-// and red.add epilogue as gemm_kernel<BN, 1>; the problem descriptors (tensor maps included) travel in the kernel's
-// parameter space.
+// Weight gradients: ONE persistent launch walks the tiles of a group of independent dW = dY^T X problems. cb_gemm launches a
+// single weight gradient as a group of one; cb_gemm_wgrad_group groups several (the four Linear layers of a BertLayer, the
+// three / four convs of a bottleneck block). The problems of a group share the reduction length (tokens / pixels), so their
+// tiles cost the same and the static round-robin schedule stays balanced; what the group buys is one prologue + one tail
+// instead of four, tiles of all problems filling the SMs together, and - because four problems together have enough tiles -
+// no K-split, i.e. half the fp32 red.global traffic of the single launches. The problem descriptors (tensor maps included)
+// travel in the kernel's parameter space.
 // ------------------------------------------------------------------------------------------------
 constexpr int WG_MAX_PROBLEMS = 8;
 struct WgradProblem {
@@ -1165,16 +1027,20 @@ __device__ __forceinline__ WgTile wg_decode(const WgradGroup& g, int tile) {
   return t;
 }
 
+// DET: a problem with split planes in ws writes every tile's scaled partial into plane `split` with plain stores; the planes are
+// added into out afterwards in split order (deterministic mode with a K-split).
 template <int BN, bool DET = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     wgrad_group_kernel(const __grid_constant__ WgradGroup g, int STAGES, int KCH, const __grid_constant__ WgradWorkspace ws) {
   using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  const int stage_bytes = KCH * Cfg::STAGE_BYTES;
+  const int stage_bytes = KCH * Cfg::STAGE_BYTES;           // a stage holds KCH consecutive 64-deep k-chunks (one barrier round trip)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // warp-uniform: see gemm_kernel
+  // warp-uniform for the compiler: with a plain threadIdx.x >> 5 ptxas takes the consumer path for divergent and serialises
+  // every wgmma behind the warpgroup arrive it inserts (advisory C7520), which leaves one m64nBNk16 in flight per warpgroup
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const int unit = blockIdx.x, n_units = gridDim.x;
   pdl_trigger();
@@ -1249,8 +1115,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   }
 }
 
-template <int BN, bool DET = false>
-static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cudaStream_t stream, float* ws = nullptr) {
+// The n problems of descs (n = 1 for cb_gemm) with `splits` K-splits each in one launch. The ring stage depth follows
+// descs[0].reserved bits 8-11 when set. ws (DET): the split planes of every problem with more than one split, one problem's after
+// the previous ones'; a second launch adds them into out in split order.
+template <int BN, bool DET>
+static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, float* ws, cudaStream_t stream, const char* what) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   auto kern = wgrad_group_kernel<BN, DET>;
@@ -1285,7 +1154,7 @@ static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cuda
     const int sp = real_splits(kc, splits);
     P.iters_per_split = ceil_div(kc, sp);
     wsp.p[i] = nullptr;
-    if (DET && sp > 1) {     // this problem's planes follow the previous problems' in the workspace
+    if (DET && sp > 1) {
       wsp.p[i] = ws;
       red.j[red.njobs++] = {static_cast<float*>(d.out), ws, d.out_ld, d.m, d.ntaps * d.n, sp};
       ws += static_cast<int64_t>(sp) * d.m * d.ntaps * d.n;
@@ -1297,17 +1166,17 @@ static int launch_wgrad_group(const cb_gemm_desc* descs, int n, int splits, cuda
     if (P.iters_per_split > max_iters) max_iters = P.iters_per_split;
   }
   g.total_tiles = total;
-  const SmemPlan sp = plan_smem(BN, false, max_iters);
+  const SmemPlan sp = plan_smem(BN, false, max_iters, (descs[0].reserved >> 8) & 15);
   if (sp.stages < 2) {
-    set_error("cb_gemm_wgrad_group: not enough shared memory for a 2-stage pipeline (BN=%d)", BN);
+    set_error("%s: not enough shared memory for a 2-stage pipeline (BN=%d)", what, BN);
     return CB_ERR_INVALID;
   }
   const int smem_bytes = sp.stages * sp.kch * Cfg::STAGE_BYTES + Cfg::BAR_BYTES + 1024;
   const int units = sm_count();
   launch_gemm_k(kern, total < units ? total : units, GEMM_THREADS, smem_bytes, stream, g, sp.stages, sp.kch, wsp);
-  const int rc = check_launch("cb_gemm_wgrad_group");
+  const int rc = check_launch(what);
   if (rc != CB_OK || red.njobs == 0) return rc;
-  return launch_split_reduce(red, stream, "cb_gemm_wgrad_group(split reduce)");
+  return launch_split_reduce(red, stream, what);
 }
 
 // Tile width and K-split of a grouped launch (groupable = false: the problems run as separate cb_gemm launches).
@@ -1361,11 +1230,43 @@ static int64_t group_ws_bytes(const cb_gemm_desc* descs, int n) {
   return bytes;
 }
 
+// What every weight-gradient descriptor must satisfy, for cb_gemm and for each problem of cb_gemm_wgrad_group.
+static int check_wgrad_desc(const cb_gemm_desc& d, const char* who) {
+  CB_REQUIRE(d.mode == CB_GEMM_WGRAD && d.out_fp32 == 1, "%s: not an fp32 WGRAD descriptor", who);
+  CB_REQUIRE(d.a && d.b && d.out && d.m > 0 && d.n > 0 && d.k > 0, "%s: null operand / empty shape", who);
+  CB_REQUIRE(d.m % 8 == 0 && d.n % 8 == 0, "%s: m, n must be multiples of 8 (got %d, %d)", who, d.m, d.n);
+  CB_REQUIRE(d.out_ld % 4 == 0, "%s: out_ld must be a multiple of 4", who);
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "%s: out must be 16-byte aligned", who);
+  CB_REQUIRE(d.ntaps == 1 || d.ntaps == 9, "%s: ntaps must be 1 or 9 (got %d)", who, d.ntaps);
+  return CB_OK;
+}
+
+// Every weight-gradient launch, of one problem (what = "cb_gemm") or a group (what = "cb_gemm_wgrad_group"): tile width bn,
+// `splits` K-splits per problem. In deterministic mode the split planes need descs[0].workspace (see launch_wgrad_group).
+static int launch_wgrad(const cb_gemm_desc* descs, int n, int bn, int splits, cudaStream_t stream, const char* what) {
+  int64_t need = 0;
+  if (g_det.load(std::memory_order_relaxed))
+    for (int i = 0; i < n; ++i) need += wgrad_ws_bytes(descs[i], real_splits(ceil_div(descs[i].k, BK), splits));
+  const cb_gemm_desc& d0 = descs[0];
+  CB_REQUIRE(need == 0 || (d0.workspace != nullptr && d0.workspace_bytes >= need && (reinterpret_cast<uintptr_t>(d0.workspace) & 15) == 0),
+             "%s: deterministic mode needs a 16-byte aligned workspace of %lld bytes in descs[0] (%s_workspace_bytes), got %lld", what,
+             static_cast<long long>(need), what, static_cast<long long>(d0.workspace ? d0.workspace_bytes : 0));
+  float* ws = static_cast<float*>(d0.workspace);
+  switch (bn) {
+    case 64: return need ? launch_wgrad_group<64, true>(descs, n, splits, ws, stream, what)
+                         : launch_wgrad_group<64, false>(descs, n, splits, ws, stream, what);
+    case 128: return need ? launch_wgrad_group<128, true>(descs, n, splits, ws, stream, what)
+                          : launch_wgrad_group<128, false>(descs, n, splits, ws, stream, what);
+    case 256: return need ? launch_wgrad_group<256, true>(descs, n, splits, ws, stream, what)
+                          : launch_wgrad_group<256, false>(descs, n, splits, ws, stream, what);
+    default: set_error("%s: block_n must be 0, 64, 128 or 256 (got %d)", what, bn); return CB_ERR_INVALID;
+  }
+}
+
 }  // namespace cb
 
 /* bring-up / tuning hook (not part of the public header): device buffer of >= 32 x grid int64 receiving clock64() stamps of every CTA */
 extern "C" void cb_debug_gemm_timeline(void* device_buf) { cb::g_gemm_timeline = static_cast<long long*>(device_buf); }
-extern "C" void cb_debug_gemm_kch(int kch) { cb::g_force_kch = kch; }
 extern "C" void cb_debug_gemm_mn3d(int on) { cb::g_mn3d = on ? 1 : 0; }
 // Weight gradients used to have a two-CTAs-per-SM instantiation (128 x 64 tiles) selected through this hook. With the wgmma of a
 // stage pipelined, it was slower than one CTA per SM on every weight-gradient shape of the step, and it is gone; the hook stays so
@@ -1433,38 +1334,10 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
       default: CB_REQUIRE(false, "cb_gemm: no tile width for block_n %d", d.block_n);
     }
   } else {
-    CB_REQUIRE(d.out_fp32 == 1, "cb_gemm(WGRAD): output must be fp32");
-    CB_REQUIRE(d.m % 8 == 0 && d.n % 8 == 0, "cb_gemm(WGRAD): m, n must be multiples of 8 (got %d, %d)", d.m, d.n);
-    CB_REQUIRE(d.out_ld % 4 == 0, "cb_gemm(WGRAD): out_ld must be a multiple of 4");
-    CB_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "cb_gemm(WGRAD): out must be 16-byte aligned");
+    const int rc = check_wgrad_desc(d, "cb_gemm(WGRAD)");
+    if (rc != CB_OK) return rc;
     const LaunchCfg lc = choose_config(d, plan_sm_count());
-    cb_gemm_desc d2 = d;
-    d2.split_k = lc.splits;
-    if (g_det.load(std::memory_order_relaxed) && lc.splits > 1) {
-      const int64_t need = wgrad_ws_bytes(d, lc.splits);
-      CB_REQUIRE(d.workspace != nullptr && d.workspace_bytes >= need && (reinterpret_cast<uintptr_t>(d.workspace) & 15) == 0,
-                 "cb_gemm(WGRAD): deterministic mode needs a 16-byte aligned workspace of %lld bytes (cb_gemm_workspace_bytes), got %lld",
-                 static_cast<long long>(need), static_cast<long long>(d.workspace ? d.workspace_bytes : 0));
-      float* ws = static_cast<float*>(d.workspace);
-      int rc = CB_ERR_INVALID;
-      switch (lc.bn) {
-        case 64: rc = launch_gemm<64, 1, true>(d2, epi, stream, ws); break;
-        case 128: rc = launch_gemm<128, 1, true>(d2, epi, stream, ws); break;
-        case 256: rc = launch_gemm<256, 1, true>(d2, epi, stream, ws); break;
-        default: CB_REQUIRE(false, "cb_gemm(WGRAD): block_n must be 0, 64, 128 or 256 (got %d)", lc.bn);
-      }
-      if (rc != CB_OK) return rc;
-      SplitReduce red;
-      red.njobs = 1;
-      red.j[0] = {static_cast<float*>(d.out), ws, d.out_ld, d.m, d.ntaps * d.n, lc.splits};
-      return launch_split_reduce(red, stream, "cb_gemm(split reduce)");
-    }
-    switch (lc.bn) {
-      case 64: return launch_gemm<64, 1>(d2, epi, stream);
-      case 128: return launch_gemm<128, 1>(d2, epi, stream);
-      case 256: return launch_gemm<256, 1>(d2, epi, stream);
-      default: CB_REQUIRE(false, "cb_gemm(WGRAD): block_n must be 0, 64, 128 or 256 (got %d)", lc.bn);
-    }
+    return launch_wgrad(&d, 1, lc.bn, lc.splits, stream, "cb_gemm");
   }
   return CB_ERR_INVALID;
 }
@@ -1473,24 +1346,11 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
 extern "C" int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* stream_v) {
   using namespace cb;
   CB_REQUIRE(descs != nullptr && n >= 1, "cb_gemm_wgrad_group: no problems");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   for (int i = 0; i < n; ++i) {
-    const cb_gemm_desc& d = descs[i];
-    CB_REQUIRE(d.mode == CB_GEMM_WGRAD && d.out_fp32 == 1, "cb_gemm_wgrad_group: problem %d is not an fp32 WGRAD descriptor", i);
-    CB_REQUIRE(d.a && d.b && d.out && d.m > 0 && d.n > 0 && d.k > 0, "cb_gemm_wgrad_group: problem %d: null operand / empty shape", i);
-    CB_REQUIRE(d.m % 8 == 0 && d.n % 8 == 0 && d.out_ld % 4 == 0 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0,
-               "cb_gemm_wgrad_group: problem %d: m, n multiples of 8, out 16-byte aligned, out_ld a multiple of 4", i);
-    CB_REQUIRE(d.ntaps == 1 || d.ntaps == 9, "cb_gemm_wgrad_group: problem %d: ntaps must be 1 or 9", i);
-  }
-  const bool det = g_det.load(std::memory_order_relaxed);
-  int64_t need = 0;
-  if (det) {
-    need = group_ws_bytes(descs, n);
-    CB_REQUIRE(need == 0 || (descs[0].workspace != nullptr && descs[0].workspace_bytes >= need &&
-                             (reinterpret_cast<uintptr_t>(descs[0].workspace) & 15) == 0),
-               "cb_gemm_wgrad_group: deterministic mode needs a 16-byte aligned workspace of %lld bytes in descs[0] "
-               "(cb_gemm_wgrad_group_workspace_bytes), got %lld",
-               static_cast<long long>(need), static_cast<long long>(descs[0].workspace ? descs[0].workspace_bytes : 0));
+    char who[48];
+    snprintf(who, sizeof(who), "cb_gemm_wgrad_group: problem %d", i);
+    const int rc = check_wgrad_desc(descs[i], who);
+    if (rc != CB_OK) return rc;
   }
   const GroupPlan gp = group_plan(descs, n, plan_sm_count());
   if (!gp.groupable) {      // a single problem, too many, or very different reduction lengths: the ordinary launches
@@ -1503,16 +1363,7 @@ extern "C" int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* strea
     }
     return CB_OK;
   }
-  CB_REQUIRE(gp.bn == 64 || gp.bn == 128 || gp.bn == 256, "cb_gemm_wgrad_group: block_n must be 0, 64, 128 or 256 (got %d)", gp.bn);
-  if (det && need > 0) {
-    float* ws = static_cast<float*>(descs[0].workspace);
-    if (gp.bn == 256) return launch_wgrad_group<256, true>(descs, n, gp.split, stream, ws);
-    if (gp.bn == 128) return launch_wgrad_group<128, true>(descs, n, gp.split, stream, ws);
-    return launch_wgrad_group<64, true>(descs, n, gp.split, stream, ws);
-  }
-  if (gp.bn == 256) return launch_wgrad_group<256>(descs, n, gp.split, stream);
-  if (gp.bn == 128) return launch_wgrad_group<128>(descs, n, gp.split, stream);
-  return launch_wgrad_group<64>(descs, n, gp.split, stream);
+  return launch_wgrad(descs, n, gp.bn, gp.split, static_cast<cudaStream_t>(stream_v), "cb_gemm_wgrad_group");
 }
 
 extern "C" int64_t cb_gemm_workspace_bytes(const cb_gemm_desc* d) {

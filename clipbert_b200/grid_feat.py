@@ -467,8 +467,7 @@ class GridFeatBackbone(nn.Module):
     def _wgrad_kw(self, m, dy, x, p, ntaps=1, tap_w=0):
         """dW[cout, t*cin + c] += scale[cout] * sum_p dy[p, cout] * x[p + shift_t, c]."""
         return dict(mode=ops.CB_GEMM_WGRAD, m=m.cout, n=m.cin, k=p, a=dy, a_rows=p, a_ld=m.cout, b=x, b_rows=p, b_ld=m.cin,
-                    ntaps=ntaps, tap_w=tap_w, tap_sign=1, split_k=ops.wgrad_split(m.cout, m.cin, p, ntaps), scale=m._scale,
-                    out=m._gw, out_ld=ntaps * m.cin, out_fp32=1)
+                    ntaps=ntaps, tap_w=tap_w, tap_sign=1, scale=m._scale, out=m._gw, out_ld=ntaps * m.cin, out_fp32=1)
 
     def _wgrad(self, m, dy, x, p, ntaps=1, tap_w=0):
         ops.gemm(**self._wgrad_kw(m, dy, x, p, ntaps, tap_w))

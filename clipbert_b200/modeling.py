@@ -593,7 +593,7 @@ class _ClipBertHeadModel(nn.Module):
     # ---- backward ---------------------------------------------------------------------------------
     def _wgrad_kw(self, li, dy, x, rows, x_ld=None):
         return dict(mode=ops.CB_GEMM_WGRAD, m=li.n, n=li.k, k=rows, a=dy, a_rows=rows, a_ld=li.n, b=x, b_rows=rows,
-                    b_ld=li.k if x_ld is None else x_ld, split_k=ops.wgrad_split(li.n, li.k, rows), out=li.gw, out_ld=li.k, out_fp32=1)
+                    b_ld=li.k if x_ld is None else x_ld, out=li.gw, out_ld=li.k, out_fp32=1)
 
     def _wgrad(self, li, dy, x, rows, x_ld=None):
         ops.gemm(**self._wgrad_kw(li, dy, x, rows, x_ld))
@@ -1064,7 +1064,7 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
             e = self._spec["emb.word"]
             gword = self._flat.grad[e["offset"]: e["offset"] + vp * H].view(vp, H)
             eb = self._spec["mlm_bias"]
-            ops.gemm(mode=ops.CB_GEMM_WGRAD, m=vp, n=H, k=R, a=ds, a_rows=R, a_ld=vp, b=st["mlm_t2"], b_rows=R, b_ld=H, split_k=0, out=gword,
+            ops.gemm(mode=ops.CB_GEMM_WGRAD, m=vp, n=H, k=R, a=ds, a_rows=R, a_ld=vp, b=st["mlm_t2"], b_rows=R, b_ld=H, out=gword,
                      out_ld=H, out_fp32=1)
             ops.colsum(ds, self._flat.grad[eb["offset"]: eb["offset"] + vp], R, vp)
             dt2 = torch.empty(R, H, dtype=bf16, device=dev)

@@ -391,11 +391,6 @@ def gemm_wgrad_group(kws):
     _launch_gemm("cb_gemm_wgrad_group", kws)
 
 
-def wgrad_split(m, n, k, ntaps=1, block_n=128):
-    """0 = the library's launch-configuration model picks tile width, CTA pairing and the K-split."""
-    return 0
-
-
 # ------------------------------------------------------------------------------------------------
 # BERT-side memory-bound ops
 # ------------------------------------------------------------------------------------------------

@@ -107,7 +107,8 @@ int cb_dropout_offset_advance(uint64_t* counter, uint64_t* snapshot, void* strea
  *     the dgrad of Linear / conv straight from the forward weight layout (no transposed copy).
  * mode CB_GEMM_WGRAD : out[m, t*N + n] += rowscale[m] * sum_p A[p, m] * B[p + shift_t, n]
  *     A: bf16 [P, M] (dY), B: bf16 [P, N] (X); both operands are read "MN-major" straight from
- *     the activation layout; fp32 red.global.add accumulation (split over P across grid.z).
+ *     the activation layout; fp32 red.global.add accumulation. Persistent CTAs walk the 128 x block_n tiles of out (per
+ *     tap), each tile over the whole of P or, with a K-split, over one of split_k consecutive ranges of P.
  *
  * Epilogue (TN), applied in this order on the fp32 accumulator v of element (m, n):
  *     v = v * scale[n] + shift[n]        (FrozenBN affine / bias; either may be NULL)
@@ -168,7 +169,8 @@ typedef struct cb_gemm_desc {
   int32_t block_n;  /* 0 = let the library choose (64 / 128; 256 for CB_GEMM_WGRAD). TN / NN run 128 x 64 or 128 x 128 tiles:
                        a 128 x 256 tile would need 256 fp32 accumulators per thread of the warpgroup that owns it, more
                        than its 232 registers, so an explicit 256 for TN / NN runs on 128-wide tiles */
-  int32_t reserved; /* tuning / test knobs: bits 8-11 k-chunks per pipeline stage (0 = automatic); other bits ignored */
+  int32_t reserved; /* tuning / test knobs: bits 8-11 k-chunks per pipeline stage (0 = automatic; for cb_gemm_wgrad_group,
+                       descs[0]'s apply to the whole group); other bits ignored */
   void* workspace;  /* deterministic mode, CB_GEMM_WGRAD: fp32 split planes, 16-byte aligned (NULL / ignored otherwise) */
   int64_t workspace_bytes;
 } cb_gemm_desc;

@@ -26,7 +26,7 @@ def test_library_builds_and_exports_every_declared_symbol():
         assert hasattr(lib, n), "header declares %s but the library does not export it" % n
     exported = subprocess.run(["nm", "-D", "--defined-only", path], capture_output=True, text=True).stdout
     extra = set(re.findall(r" T (cb_[a-z0-9_]+)", exported)) - set(names)
-    assert not (extra - {"cb_debug_gemm_timeline", "cb_debug_gemm_kch", "cb_debug_gemm_sm_limit", "cb_debug_gemm_occ2", "cb_debug_gemm_mn3d", "cb_debug_attention_general", "cb_debug_attention_flash", "cb_debug_attention_rows48", "cb_debug_attention_flash_pipe"}), "exported but undeclared: %s" % sorted(extra)
+    assert not (extra - {"cb_debug_gemm_timeline", "cb_debug_gemm_sm_limit", "cb_debug_gemm_occ2", "cb_debug_gemm_mn3d", "cb_debug_attention_general", "cb_debug_attention_flash", "cb_debug_attention_rows48", "cb_debug_attention_flash_pipe"}), "exported but undeclared: %s" % sorted(extra)
 
 
 def test_header_compiles_as_plain_c(tmp_path):

@@ -1,6 +1,7 @@
 """Weight-gradient main loop with one wgmma group in flight: every tile width, K-splits with a ragged last split and a ragged
 last k-chunk, and many tiles per persistent CTA, so that the operand ring wraps across tiles while a stage's products are still
-being waited for. Grouped launches at every tile width and with a forced K-split."""
+being waited for. Grouped launches at every tile width and with a forced K-split, and in deterministic mode the bits of a single
+launch against the same problem inside a group."""
 import pytest
 import torch
 
@@ -69,3 +70,32 @@ def test_grouped_wgrad_tile_widths_and_splits(cuda, bn, split):
     ops.gemm_wgrad_group(kws)
     for kw, dW, ref in probs:
         assert relerr(dW, ref) < TOL_FP32_OP, (bn, split, kw["m"], kw["n"])
+
+
+@pytest.mark.parametrize("split", [1, 3])
+@pytest.mark.parametrize("bn", [64, 128, 256])
+def test_single_wgrad_gives_the_bits_of_its_group(cuda, bn, split):
+    """Deterministic mode: a weight gradient launched alone and the same problem inside a group of three, at the same tile width
+    and K-split, run the same tiles in the same k order and add their split planes in the same order."""
+    from clipbert_b200 import ops
+    g = torch.Generator().manual_seed(43)
+    probs = []
+    for mo, no, p in ((1024, 768, 2373), (768, 1024, 2373), (512, 256, 2400)):
+        dy, x = _rnd(g, p, mo), _rnd(g, p, no)
+        out0 = torch.randn(mo, no, generator=g).to(cuda)          # += semantics: the planes are added onto non-zero outputs
+        probs.append((dict(mode=ops.CB_GEMM_WGRAD, m=mo, n=no, k=p, a=dy, a_rows=p, a_ld=mo, b=x, b_rows=p, b_ld=no, out_ld=no,
+                           out_fp32=1), out0))
+    prev = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(True)
+    try:
+        kw, out0 = probs[1]
+        alone = out0.clone()
+        ops.gemm(**kw, out=alone, block_n=bn, split_k=split, reserved=SINGLE)
+        grouped = [o.clone() for _, o in probs]
+        kws = [dict(k, out=o) for (k, _), o in zip(probs, grouped)]
+        kws[0] = dict(kws[0], block_n=bn, split_k=split)
+        ops.gemm_wgrad_group(kws)
+    finally:
+        torch.use_deterministic_algorithms(prev)
+    assert not torch.equal(alone, out0)
+    assert torch.equal(alone, grouped[1])
