@@ -437,8 +437,13 @@ void cb_debug_attention_flash_pipe(int on) { cb::attention_tc_set_flash_pipe(on)
 int cb_attention_fwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, void* ctx, int64_t ld_ctx, float* lse,
                      int nseq, int l, int lt, int heads, int head_dim, float dropout_p, uint64_t seed, void* stream) {
   CB_REQUIRE(head_dim == HD, "cb_attention_fwd: head_dim %d unsupported (built for 64)", head_dim);
-  CB_REQUIRE(qkv && text_mask && ctx && nseq > 0 && l > 0 && lt >= 0 && lt <= l && heads > 0, "cb_attention_fwd: bad arguments");
+  CB_REQUIRE(qkv && text_mask && ctx && nseq > 0 && l > 0 && lt >= 0 && lt <= l && heads > 0 && nseq <= 65535 && heads <= 65535,
+             "cb_attention_fwd: bad arguments");
   CB_REQUIRE(ld_qkv % 8 == 0 && ld_ctx % 8 == 0, "cb_attention_fwd: row pitches must be multiples of 8");
+  CB_REQUIRE(ld_qkv >= 3 * static_cast<int64_t>(heads) * HD && ld_ctx >= static_cast<int64_t>(heads) * HD,
+             "cb_attention_fwd: row pitches must hold Q | K | V and the merged heads");
+  CB_REQUIRE(reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(ctx) % 16 == 0,
+             "cb_attention_fwd: qkv and ctx must be 16-byte aligned");
   if (l <= 64 && !g_attention_force_general)
     return attention_tc_fwd(qkv, ld_qkv, text_mask, ctx, ld_ctx, lse, nseq, l, lt, heads, dropout_p, seed, static_cast<cudaStream_t>(stream));
   if (l > 64 && g_attention_flash && !g_attention_force_general)
@@ -463,8 +468,16 @@ int cb_attention_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, 
                      int64_t ld_ctx, const float* lse, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads,
                      int head_dim, float dropout_p, uint64_t seed, void* stream) {
   CB_REQUIRE(head_dim == HD, "cb_attention_bwd: head_dim %d unsupported (built for 64)", head_dim);
-  CB_REQUIRE(qkv && text_mask && ctx && dctx && lse && dqkv && nseq > 0 && l > 0, "cb_attention_bwd: bad arguments");
+  CB_REQUIRE(qkv && text_mask && ctx && dctx && lse && dqkv && nseq > 0 && l > 0 && lt >= 0 && lt <= l && heads > 0 && nseq <= 65535 &&
+                 heads <= 65535,
+             "cb_attention_bwd: bad arguments");
   CB_REQUIRE(ld_qkv % 8 == 0 && ld_ctx % 8 == 0 && ld_dqkv % 8 == 0, "cb_attention_bwd: row pitches must be multiples of 8");
+  CB_REQUIRE(ld_qkv >= 3 * static_cast<int64_t>(heads) * HD && ld_dqkv >= 3 * static_cast<int64_t>(heads) * HD &&
+                 ld_ctx >= static_cast<int64_t>(heads) * HD,
+             "cb_attention_bwd: row pitches must hold Q | K | V and the merged heads");
+  CB_REQUIRE(reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(ctx) % 16 == 0 &&
+                 reinterpret_cast<uintptr_t>(dctx) % 16 == 0 && reinterpret_cast<uintptr_t>(dqkv) % 16 == 0,
+             "cb_attention_bwd: qkv, ctx, dctx and dqkv must be 16-byte aligned");
   if (l <= 64 && !g_attention_force_general)
     return attention_tc_bwd(qkv, ld_qkv, text_mask, ctx, dctx, ld_ctx, lse, dqkv, ld_dqkv, nseq, l, lt, heads, dropout_p, seed,
                             static_cast<cudaStream_t>(stream));

@@ -257,11 +257,21 @@ int cb_embed_visual_bwd_det(const void* dh, const void* grid, const int32_t* seq
 
 /* ------------------------------------------------------------------------------------------
  * Fused self-attention, BertSelfAttention.forward (transformers.py:230-286):
- *   S = Q K^T / 8 + (1 - mask) * -10000 ; P = softmax(S) (fp32) ; dropout(P) ; ctx = P V ; heads merged.
+ *   S = Q K^T / 8 + (1 - mask) * -10000 ; P = softmax(S) ; dropout(P) ; ctx = P V ; heads merged.
  * qkv: bf16 [nseq*l, 3*heads*64] (Q | K | V as produced by the fused N=2304 projection);
  * text_mask: int64 [nseq, lt] (visual tokens are always attendable, modeling.py:217-220);
- * ctx: bf16 [nseq*l, heads*64]; lse: fp32 [nseq, heads, l] log-sum-exp saved for the backward.
- * The backward recomputes P tile by tile from Q, K, lse and regenerates the dropout mask. Every length runs on tensor
+ * ctx: bf16 [nseq*l, heads*64]; lse: fp32 [nseq, heads, l] log-sum-exp saved for the backward (fwd: may be NULL).
+ * Arguments (checked on the host, nothing is launched otherwise): 0 <= lt <= l, 0 < nseq, heads <= 65535 (grid limits);
+ * row pitches multiples of 8 with ld_qkv, ld_dqkv >= 3*heads*64 and ld_ctx >= heads*64 (ld_ctx is also dctx's pitch);
+ * qkv, ctx, dctx and dqkv 16-byte aligned (read and written as 16-byte vectors).
+ * The backward recomputes P tile by tile from Q, K and the SAVED lse, takes D_i = dO_i . ctx_i from the SAVED ctx, and
+ * regenerates the dropout mask: dS = P (r dO V^T - D), dV = (P r)^T dO, dQ = dS K / 8, dK = dS^T Q / 8 (r: multipliers).
+ * Rounding (fp32 arithmetic and accumulation everywhere else):
+ *   tensor-core forward: x_ij = exp(S_ij - m_i) r_ij is rounded to bf16 before the P V product, m_i the running row maximum
+ *     (the whole row when l <= 64, 64-key tiles 0..t on the longer path); the products are rescaled as m_i grows and divided
+ *     by the unrounded (undropped) row sum;
+ *   tensor-core backward: P r and dS are rounded to bf16 before the dV / dK / dQ products;
+ *   CUDA-core kernels (cb_debug_attention_general): P and dS stay fp32. Every length runs on tensor
  * cores (mma.sync): l <= 64 in one CTA per (sequence, head); longer sequences in two kernels, one per 64-key tile
  * (dK, dV) and one per 64-query tile (dQ). Each output row is written by one CTA: no atomics, no workspace, results
  * bit-identical from run to run. cb_debug_attention_general(1) selects the CUDA-core kernels instead, for every length.

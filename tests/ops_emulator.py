@@ -235,31 +235,41 @@ def embed_visual_bwd(dh, grid, seq2vid, vid_start, n_ex, rowemb, colemb, typ, ga
         dgrid.view(nvid, t, lv, h).copy_(per_vid[:, None].expand(nvid, t, lv, h))
 
 
-def _attention(qkv, text_mask, nseq, l, lt, heads, p, seed):
-    hd = qkv.shape[1] // (3 * heads)
-    q, k, v = (x.reshape(nseq, l, heads, hd).permute(0, 2, 1, 3) for x in qkv.view(nseq, l, 3, heads * hd).unbind(2))
-    mask = torch.cat([text_mask.to(qkv.dtype), torch.ones(nseq, l - lt, dtype=qkv.dtype)], dim=1)
-    s = q @ k.transpose(-1, -2) / math.sqrt(hd) + ((1.0 - mask) * -10000.0)[:, None, None, :]
-    pr = torch.softmax(s, dim=-1)
-    mult = _drop_mult(p, seed, D.attention_index(nseq, heads, l))
-    if mult is not None:                                # the log-sum-exp is of the undropped scores
-        pr = pr * mult.to(pr.dtype)
-    return (pr @ v).permute(0, 2, 1, 3).reshape(nseq * l, heads * hd), torch.logsumexp(s, dim=-1)
+def _heads(x, nseq, l, heads):
+    """[nseq * l, heads * 64] -> [nseq, heads, l, 64] float64."""
+    return x.double().reshape(nseq, l, heads, -1).permute(0, 2, 1, 3)
+
+
+def _attention_scores(qkv, text_mask, nseq, l, lt, heads):
+    """S = Q K^T / 8 + madd (float64) and V, from the bf16 qkv; text_mask [nseq, >= lt] (only its first lt columns are keys)."""
+    q, k, v = (_heads(x, nseq, l, heads) for x in qkv.view(nseq, l, 3, -1).unbind(2))
+    mask = torch.cat([text_mask[:, :lt].double(), torch.ones(nseq, l - lt, dtype=torch.float64)], dim=1)
+    return q, k, v, q @ k.transpose(-1, -2) / math.sqrt(q.shape[-1]) + ((1.0 - mask) * -10000.0)[:, None, None, :]
 
 
 def attention_fwd(qkv, text_mask, ctx, lse, nseq, l, lt, heads, p, seed):
-    o, ls = _attention(qkv.double(), text_mask, nseq, l, lt, heads, p, seed)
-    ctx.copy_(o)
+    _, _, v, s = _attention_scores(qkv, text_mask, nseq, l, lt, heads)
+    pr = torch.softmax(s, dim=-1)
+    mult = _drop_mult(p, seed, D.attention_index(nseq, heads, l))
+    if mult is not None:                                # the log-sum-exp is of the undropped scores
+        pr = pr * mult.double()
+    ctx.copy_((pr @ v).permute(0, 2, 1, 3).reshape(nseq * l, -1))
     if lse is not None:
-        lse.copy_(ls)
+        lse.copy_(torch.logsumexp(s, dim=-1))
 
 
 def attention_bwd(qkv, text_mask, ctx, dctx, lse, dqkv, nseq, l, lt, heads, p, seed):
-    x = qkv.to(F32).clone().requires_grad_(True)
-    with torch.enable_grad():
-        o, _ = _attention(x, text_mask, nseq, l, lt, heads, p, seed)
-        o.backward(dctx.to(F32))
-    dqkv.copy_(x.grad)
+    """The header's backward: P = exp(S - lse) from the SAVED lse, D_i = dO_i . ctx_i from the SAVED ctx, dS = P (r dO V^T - D),
+    dV = (P r)^T dO, dQ = dS K / 8, dK = dS^T Q / 8 (r: dropout multipliers) - the forward is not re-run."""
+    q, k, v, s = _attention_scores(qkv, text_mask, nseq, l, lt, heads)
+    do, o = _heads(dctx, nseq, l, heads), _heads(ctx, nseq, l, heads)
+    pr = torch.exp(s - lse.double()[..., None])
+    mult = _drop_mult(p, seed, D.attention_index(nseq, heads, l))
+    r = torch.ones_like(pr) if mult is None else mult.double()
+    ds = pr * (r * (do @ v.transpose(-1, -2)) - (do * o).sum(-1, keepdim=True))
+    scale = 1.0 / math.sqrt(q.shape[-1])
+    grads = [ds @ k * scale, ds.transpose(-1, -2) @ q * scale, (pr * r).transpose(-1, -2) @ do]
+    dqkv.view(nseq, l, 3, -1).copy_(torch.stack([g.permute(0, 2, 1, 3).reshape(nseq, l, -1) for g in grads], 2))
 
 
 def colsum(x, out, m, n, ld=None):

@@ -90,6 +90,43 @@ def test_attention_probs_rejects_bad_arguments(cuda):
         ops._call("cb_attention_probs", ops._p(qkv), qkv.shape[1], ops._p(mask), ops._p(lse), ops._p(buf), 2, 41, 42, HEADS, 64, 0.0, 1, ops._s())
 
 
+def test_attention_fwd_bwd_reject_bad_arguments(cuda):
+    """cb_attention_fwd / _bwd check what cb_attention_probs checks, on the host, before any launch: 0 <= lt <= l, heads > 0,
+    nseq and heads within the grid (65535), row pitches that hold Q | K | V and the merged heads, 16-byte aligned vectors."""
+    from clipbert_b200 import ops
+    n, L = 2, 41
+    hid = HEADS * 64
+    qkv, mask, lt = _qkv_case(L, False, 3, n, cuda)
+    flat = torch.zeros(n * L * 3 * hid + 8, dtype=torch.bfloat16, device=cuda)
+    ctx, dctx = (torch.zeros(n * L * hid + 8, dtype=torch.bfloat16, device=cuda) for _ in range(2))
+    lse = torch.zeros(n, HEADS, L, device=cuda)
+    P = ops._p
+
+    def fwd(q=qkv, ld_q=3 * hid, c=ctx, ld_c=hid, nseq=n, lt_=lt, heads=HEADS):
+        ops._call("cb_attention_fwd", P(q), ld_q, P(mask), P(c), ld_c, P(lse), nseq, L, lt_, heads, 64, 0.0, 1, ops._s())
+
+    def bwd(q=qkv, ld_q=3 * hid, c=ctx, d=dctx, ld_c=hid, dq=flat, ld_dq=3 * hid, nseq=n, lt_=lt, heads=HEADS):
+        ops._call("cb_attention_bwd", P(q), ld_q, P(mask), P(c), P(d), ld_c, P(lse), P(dq), ld_dq, nseq, L, lt_, heads, 64, 0.0, 1,
+                  ops._s())
+
+    for f in (fwd, bwd):
+        for kw in (dict(lt_=L + 1), dict(lt_=-1), dict(heads=0), dict(nseq=65536), dict(heads=65536)):
+            with pytest.raises(RuntimeError, match="bad arguments"):
+                f(**kw)
+        for kw in (dict(ld_q=3 * hid - 8), dict(ld_c=hid - 8)):
+            with pytest.raises(RuntimeError, match="row pitches must hold"):
+                f(**kw)
+        for kw in (dict(q=flat[1:]), dict(c=ctx[1:])):
+            with pytest.raises(RuntimeError, match="16-byte aligned"):
+                f(**kw)
+    with pytest.raises(RuntimeError, match="row pitches must hold"):
+        bwd(ld_dq=3 * hid - 8)
+    for kw in (dict(d=dctx[1:]), dict(dq=flat[1:])):
+        with pytest.raises(RuntimeError, match="16-byte aligned"):
+            bwd(**kw)
+    torch.cuda.synchronize()
+
+
 # ------------------------------------------------------------------------------------------------ module
 def _base(sd, cuda, hidden=True, attn=True, **cfg_extra):
     import clipbert_b200 as cb
