@@ -111,6 +111,17 @@ struct GemmCfg {
 // under predicates for every element whatever the launch asked for (~2.4 k cycles per 16 columns for a bare multiply).
 enum { EK_GENERIC = 0, EK_SHIFT_ACT = 1, EK_RELU_MASK = 2, EK_DROP_RES = 3, EK_GELU_STASH = 4, EK_AUX_MUL = 5 };
 
+// ReLU of the epilogue: NaN propagates (as ATen's relu; fmaxf would return 0) and a -0 pre-activation gives +0. One FSETP.GTU +
+// FSEL per element.
+__device__ __forceinline__ float relu_nan(float v) { return !(v <= 0.0f) ? v : 0.0f; }
+// ReLU' of a bf16 activation, tested on its bits (lo: the low half of x): > 0 for a positive normal number or +inf. A NaN,
+// a zero of either sign and a subnormal give 0 - the same answer as the flush-to-zero float compare (act > 0) of the library's
+// other ReLU backwards, whatever the packing.
+__device__ __forceinline__ bool bf16_relu_pos(uint32_t x, bool lo) {
+  const uint32_t b = lo ? (x & 0xffffu) : (x >> 16);
+  return b - 0x0080u <= 0x7f80u - 0x0080u;
+}
+
 template <int NC>
 __device__ __forceinline__ void add_shift(float (&f)[NC], const float (&shv)[NC]) {
 #pragma unroll
@@ -133,18 +144,17 @@ __device__ __forceinline__ void epilogue_shift_act(float (&f)[NC], const float (
   if (has_res) add_residual<NC>(f, res16);
   if (relu) {
 #pragma unroll
-    for (int j = 0; j < NC; ++j) f[j] = fmaxf(f[j], 0.0f);
+    for (int j = 0; j < NC; ++j) f[j] = relu_nan(f[j]);
   }
 }
-//   EK_RELU_MASK : v = (v (+ residual)) * (aux > 0)                dgrad through a ReLU (CB_AUX_RELU_MASK)
+//   EK_RELU_MASK : v = (aux > 0) ? v (+ residual) : 0              dgrad through a ReLU (CB_AUX_RELU_MASK), a select
 template <int NC>
 __device__ __forceinline__ void epilogue_relu_mask(float (&f)[NC], const uint32_t (&res16)[NC / 2], bool has_res, const uint32_t (&aux16)[NC / 2]) {
   if (has_res) add_residual<NC>(f, res16);
 #pragma unroll
-  for (int j = 0; j < NC / 2; ++j) {     // bf16 > 0  <=>  sign bit clear and magnitude non-zero, tested on the packed halves
-    const uint32_t a = aux16[j];
-    f[2 * j] = ((a & 0x8000u) == 0u && (a & 0x7fffu) != 0u) ? f[2 * j] : 0.0f;
-    f[2 * j + 1] = ((a & 0x80000000u) == 0u && (a & 0x7fff0000u) != 0u) ? f[2 * j + 1] : 0.0f;
+  for (int j = 0; j < NC / 2; ++j) {     // tested on the packed halves
+    f[2 * j] = bf16_relu_pos(aux16[j], true) ? f[2 * j] : 0.0f;
+    f[2 * j + 1] = bf16_relu_pos(aux16[j], false) ? f[2 * j + 1] : 0.0f;
   }
 }
 //   EK_DROP_RES  : v = dropout(v + shift) + residual               BertSelfOutput / BertOutput dense (transformers.py:297-301,377-381)
@@ -230,7 +240,7 @@ __device__ __forceinline__ void epilogue_math(float (&f)[NC], const GemmEpi& epi
   switch (epi.act) {
     case CB_ACT_RELU:
 #pragma unroll
-      for (int j = 0; j < NC; ++j) f[j] = fmaxf(f[j], 0.0f);
+      for (int j = 0; j < NC; ++j) f[j] = relu_nan(f[j]);
       break;
     case CB_ACT_GELU:
 #pragma unroll
@@ -246,10 +256,9 @@ __device__ __forceinline__ void epilogue_math(float (&f)[NC], const GemmEpi& epi
     switch (epi.aux_mode) {
       case CB_AUX_RELU_MASK:
 #pragma unroll
-        for (int j = 0; j < NC / 2; ++j) {
-          const float2 a2 = unpack_bf16x2(aux16[j]);
-          f[2 * j] = a2.x > 0.0f ? f[2 * j] : 0.0f;
-          f[2 * j + 1] = a2.y > 0.0f ? f[2 * j + 1] : 0.0f;
+        for (int j = 0; j < NC / 2; ++j) {        // as EK_RELU_MASK
+          f[2 * j] = bf16_relu_pos(aux16[j], true) ? f[2 * j] : 0.0f;
+          f[2 * j + 1] = bf16_relu_pos(aux16[j], false) ? f[2 * j + 1] : 0.0f;
         }
         break;
       case CB_AUX_GELU_GRAD:
@@ -1237,6 +1246,8 @@ static int check_wgrad_desc(const cb_gemm_desc& d, const char* who) {
   CB_REQUIRE(d.m % 8 == 0 && d.n % 8 == 0, "%s: m, n must be multiples of 8 (got %d, %d)", who, d.m, d.n);
   CB_REQUIRE(d.out_ld % 4 == 0, "%s: out_ld must be a multiple of 4", who);
   CB_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "%s: out must be 16-byte aligned", who);
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(d.a) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.b) & 15) == 0,
+             "%s: a and b must be 16-byte aligned (TMA)", who);
   CB_REQUIRE(d.ntaps == 1 || d.ntaps == 9, "%s: ntaps must be 1 or 9 (got %d)", who, d.ntaps);
   return CB_OK;
 }
@@ -1321,6 +1332,11 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
     CB_REQUIRE(!d.aux || d.aux_ld % 8 == 0, "cb_gemm(TN): aux_ld must be a multiple of 8");
     CB_REQUIRE((reinterpret_cast<uintptr_t>(d.residual) & 15) == 0, "cb_gemm(TN): residual must be 16-byte aligned");
     CB_REQUIRE((reinterpret_cast<uintptr_t>(d.aux) & 15) == 0, "cb_gemm(TN): aux must be 16-byte aligned");
+    // TMA reads A and B from 16-byte aligned bases; the epilogue writes out and out2 as 16-byte vectors
+    CB_REQUIRE((reinterpret_cast<uintptr_t>(d.a) & 15) == 0, "cb_gemm(TN): a must be 16-byte aligned");
+    CB_REQUIRE((reinterpret_cast<uintptr_t>(d.b) & 15) == 0, "cb_gemm(TN): b must be 16-byte aligned");
+    CB_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "cb_gemm(TN): out must be 16-byte aligned");
+    CB_REQUIRE((reinterpret_cast<uintptr_t>(d.out2) & 15) == 0, "cb_gemm(TN): out2 must be 16-byte aligned");
     CB_REQUIRE(!d.out2 || d.out2_ld % 8 == 0, "cb_gemm(TN): out2_ld must be a multiple of 8");
     CB_REQUIRE(!(d.out2 && d.out_fp32), "cb_gemm(TN): out2 requires a bf16 primary output");
     CB_REQUIRE(d.rowmap == CB_ROWMAP_NONE || (d.map_h > 0 && d.map_w > 0), "cb_gemm: rowmap needs map_h/map_w");

@@ -119,6 +119,20 @@ int cb_dropout_offset_advance(uint64_t* counter, uint64_t* snapshot, void* strea
  *     v *= auxfn(aux[m, n])              (backward masks: relu' , gelu', tanh' ; optional)
  *     out[row(m), n] = v                 (bf16 or fp32)
  * row(m) re-maps between compact NHWC pixel rows and zero-bordered rows (cb_rowmap).
+ * Rounding: the products of bf16 A and B are accumulated in fp32 on the tensor cores; every epilogue step above is one fp32
+ * operation (gelu / gelu' use fast_erf, |error| <= 1.5e-7; tanh is tanh.approx.f32, relative error 2^-10.987); the result is
+ * rounded once to bf16 (nearest even) unless out_fp32, and out2 once from its fp32 value. fp32 results below 2^-126 flush to
+ * zero.
+ * NaN / inf: a NaN or inf reaches out like any other value (a NaN in row m of A makes row m NaN; an overflowing accumulator
+ * is +-inf). relu passes NaN and +inf and writes +0 for -inf and for a pre-activation of -0 or +0, so a NaN from an
+ * overflowing bf16 conv reaches the loss. CB_AUX_RELU_MASK is a select, v = (aux > 0) ? v : 0, with aux > 0 meaning a
+ * positive normal bf16 or +inf: a NaN, zero or subnormal aux gives 0 even for a NaN / inf v (the (act > 0) rule of every ReLU
+ * backward below). Nothing is promised about gelu / gelu' of +-inf.
+ * Alignment (checked, CB_ERR_INVALID and nothing launched otherwise): a, b, out, out2, residual, aux 16-byte aligned (TMA
+ * reads the operands and epilogue inputs; out / out2 take 16-byte stores); n, k, out_ld, out2_ld, res_ld, aux_ld multiples
+ * of 8. WGRAD: a, b, out 16-byte aligned, m, n multiples of 8, out_ld a multiple of 4.
+ * ntaps = 9 with k % 64 != 0 is supported: the last 64-deep chunk of a tap reads the next tap's first columns of B, and they
+ * meet the zero fill of A past column k, so the result is exact for finite B (an inf / NaN there would turn 0 * inf into NaN).
  * ------------------------------------------------------------------------------------------ */
 enum { CB_GEMM_TN = 0, CB_GEMM_WGRAD = 1, CB_GEMM_NN = 2 };
 enum {
@@ -129,7 +143,7 @@ enum {
 };
 enum {
   CB_AUX_NONE = 0,
-  CB_AUX_RELU_MASK = 1, /* v *= (aux > 0)              aux = forward output of the ReLU       */
+  CB_AUX_RELU_MASK = 1, /* v = (aux > 0) ? v : 0       aux = forward output of the ReLU       */
   CB_AUX_GELU_GRAD = 2, /* v *= gelu'(aux)             aux = forward pre-activation            */
   CB_AUX_TANH_GRAD = 3, /* v *= 1 - aux^2              aux = forward tanh output               */
   CB_AUX_MUL = 4        /* v *= aux                    aux = stashed derivative (CB_ACT_GELU_STASH_GRAD) */

@@ -114,17 +114,19 @@ def gemm(**kw):
     act = kw.get("act", 0)
     if kw.get("out2") is not None:
         _mat(kw["out2"], n_dst, n, kw["out2_ld"])[dst[keep]] = (_gelu_grad(v) if act == 4 else v)[keep].to(kw["out2"].dtype)
-    if act == 1:
-        v = torch.relu(v)
+    if act == 1:                                        # NaN passes, -0 gives +0 (include/clipbert_b200.h)
+        v = torch.where(v <= 0, torch.zeros_like(v), v)
     elif act in (2, 4):
         v = _gelu(v)
     elif act == 3:
         v = torch.tanh(v)
     if kw.get("aux") is not None:
-        x = _mat(kw["aux"], m, n, kw["aux_ld"]).to(F32)
+        xb = _mat(kw["aux"], m, n, kw["aux_ld"])
+        x = xb.to(F32)
         am = kw.get("aux_mode", 0)
-        if am == 1:
-            v = v * (x > 0).to(F32)
+        if am == 1:                                     # a select on aux > 0: a positive normal bf16 or +inf
+            bits = xb.contiguous().view(torch.int16).to(torch.int64) & 0xFFFF
+            v = torch.where((bits >= 0x0080) & (bits <= 0x7F80), v, torch.zeros_like(v))
         elif am == 2:
             v = v * _gelu_grad(x)
         elif am == 3:

@@ -55,3 +55,24 @@ def test_wgmma_kernels_are_not_serialised():
         assert k in names, "no wgmma kernel %s in the library" % k
     bad = {f: c for f, c in kernels.items() if c[1] > MAX_DEPBAR}
     assert not bad, "wgmma serialised (HGMMA, WARPGROUP.DEPBAR): %s" % bad
+
+
+def test_gemm_kernels_do_not_spill():
+    """No GEMM kernel (TN / NN ping-pong, weight gradients, split reduce) uses local memory or a stack: a spill in the
+    consumer warpgroups' fused epilogue, beside 2 x BN / 2 fp32 accumulators, would put local-memory traffic on every tile."""
+    tool = _cuobjdump()
+    if tool is None or not os.path.exists(LIB):
+        pytest.skip("needs the built library and cuobjdump")
+    out = subprocess.run([tool, "-res-usage", LIB], capture_output=True, text=True, check=True).stdout
+    usage, fn = {}, None
+    for line in out.splitlines():
+        m = re.search(r"Function (\S+):", line)
+        if m:
+            fn = m.group(1)
+            continue
+        m = re.search(r"STACK:(\d+).*LOCAL:(\d+)", line)
+        if m and fn and ("gemm" in fn or "wgrad" in fn):
+            usage[fn] = (int(m.group(1)), int(m.group(2)))
+    assert any("gemm_pingpong_kernel" in f for f in usage) and any("wgrad_group_kernel" in f for f in usage), sorted(usage)
+    bad = {f: u for f, u in usage.items() if u != (0, 0)}
+    assert not bad, "GEMM kernels with stack / local memory (spills): %s" % bad

@@ -1,7 +1,7 @@
 """GEMM epilogue inputs (residual / aux, loaded by TMA into shared memory ahead of the epilogue) on the shapes of the HBM-bound
 1x1 convolutions: a one-chunk K loop and many tiles per persistent CTA, so that the input buffers and the operand ring wrap their
-barrier phases many times; strided residual / aux views; ragged M and N % 16 == 8; the PAD row map; both CTA-per-SM
-instantiations; long K loops, whose inputs share the operand ring; bit-identical repeats; and the alignment check on the
+barrier phases many times; strided residual / aux views; ragged M and N % 16 == 8; the PAD row map; the full grid and a
+grid of three CTAs; long K loops, whose inputs share the operand ring; bit-identical repeats; and the alignment check on the
 residual / aux bases."""
 import pytest
 import torch
@@ -28,12 +28,14 @@ def _strided(g, M, N, pad):
     return _rnd(g, M, ld)[:, 8:8 + N], ld
 
 
-@pytest.fixture(params=["one_cta_per_sm", "two_ctas_per_sm"])
-def occ(request):
+@pytest.fixture(params=["all_sms", "three_ctas"])
+def grid(request):
+    """The persistent grid on every SM, and capped at three CTAs (ops.set_sm_limit): hundreds of tiles per CTA, so that the
+    input buffers and the operand ring wrap their phases many more times."""
     ops = _ops()
-    ops.set_occ2(2 if request.param == "two_ctas_per_sm" else 0)
+    ops.set_sm_limit(3 if request.param == "three_ctas" else 0)
     yield request.param
-    ops.set_occ2(1)
+    ops.set_sm_limit(0)
 
 
 # (M, N, K): 1x1-conv shapes with one or two k-chunks and ~7-30 tiles per CTA; M % 128 != 0 with N % 16 == 8; a short launch
@@ -42,7 +44,7 @@ SHAPES = [(60000, 256, 64), (60000, 512, 128), (30001, 392, 64), (777, 136, 256)
 
 @pytest.mark.parametrize("block_n", [0, 64, 128])
 @pytest.mark.parametrize("shape", SHAPES)
-def test_tn_shift_residual_relu(cuda, occ, shape, block_n):
+def test_tn_shift_residual_relu(cuda, grid, shape, block_n):
     """conv + FrozenBN shift + shortcut + ReLU (a bottleneck's conv3), twice: same bits."""
     ops = _ops()
     M, N, K = shape
@@ -63,7 +65,7 @@ def test_tn_shift_residual_relu(cuda, occ, shape, block_n):
 @pytest.mark.parametrize("strided", [False, True])
 @pytest.mark.parametrize("block_n", [0, 64])
 @pytest.mark.parametrize("shape", SHAPES)
-def test_nn_residual_relu_mask(cuda, occ, shape, block_n, strided):
+def test_nn_residual_relu_mask(cuda, grid, shape, block_n, strided):
     """dgrad of conv1 + shortcut gradient, through the block input's ReLU (residual and aux), and aux alone; residual / aux as
     strided views (res_ld, aux_ld > N) when asked; twice: same bits."""
     ops = _ops()
@@ -91,7 +93,7 @@ def test_nn_residual_relu_mask(cuda, occ, shape, block_n, strided):
 
 @pytest.mark.parametrize("block_n", [0, 64])
 @pytest.mark.parametrize("dims", [(40, 28, 28, 64, 256), (3, 5, 6, 128, 392)])
-def test_rowmap_pad_residual_aux(cuda, occ, dims, block_n):
+def test_rowmap_pad_residual_aux(cuda, grid, dims, block_n):
     """PAD row map (compact rows in, zero-bordered rows out): residual and aux are read at the compact row; the border stays zero."""
     ops = _ops()
     NB, H, W, K, N = dims
@@ -114,9 +116,9 @@ def test_rowmap_pad_residual_aux(cuda, occ, dims, block_n):
 
 @pytest.mark.parametrize("block_n", [0, 64, 128])
 @pytest.mark.parametrize("shape", [(20000, 256, 1024), (3001, 392, 576), (2624, 768, 3072)])
-def test_long_k_inputs(cuda, occ, shape, block_n):
+def test_long_k_inputs(cuda, grid, shape, block_n):
     """K loops longer than four chunks (BERT dense layers, 3x3 dgrad): the inputs of a tile land in the ring stage after its
-    operands where one stage holds them, in a dedicated buffer otherwise (residual + aux on the two-CTAs-per-SM tiles); several
+    operands where one stage holds them, in a dedicated buffer otherwise; several
     tiles per CTA on the first shape; twice: same bits."""
     ops = _ops()
     M, N, K = shape
