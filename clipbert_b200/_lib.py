@@ -63,6 +63,8 @@ def lib():
     L.cb_gemm.restype = ctypes.c_int
     L.cb_gemm_wgrad_group.argtypes = [ctypes.POINTER(GemmDesc), ctypes.c_int, ctypes.c_void_p]
     L.cb_gemm_wgrad_group.restype = ctypes.c_int
+    L.cb_gemm_tile_width.argtypes = [ctypes.POINTER(GemmDesc)]
+    L.cb_gemm_tile_width.restype = ctypes.c_int
     L.cb_gemm_workspace_bytes.argtypes = [ctypes.POINTER(GemmDesc)]
     L.cb_gemm_workspace_bytes.restype = ctypes.c_int64
     L.cb_gemm_wgrad_group_workspace_bytes.argtypes = [ctypes.POINTER(GemmDesc), ctypes.c_int]

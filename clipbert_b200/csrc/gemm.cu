@@ -32,6 +32,9 @@
 //                 tile's operands (plan_smem). Reading them with per-lane global loads inside the epilogue left four dependent
 //                 HBM round trips per tile and warp exposed on the one-chunk main loops of the HBM-bound 1x1 convs.
 //
+// TN / NN 128 x 256: gemm_coop_kernel, the same three warpgroups, both consumers on rows 0-63 / 64-127 of ONE tile (see there);
+//   choose_config picks it for long tensor-bound K loops where it about halves the wave count.
+//
 // WGRAD: wgrad_group_kernel, 288 threads, one CTA per SM. It walks the tiles of a group of problems; a single weight gradient
 //   (cb_gemm) is a group of one. Warp 8 is the TMA producer, warps 0..7 two consumer warpgroups that multiply rows
 //   64g .. 64g+63 of one 128 x BN tile (BN up to 256) with wgmma m64nBNk16, hand every ring stage back as soon as the products
@@ -432,6 +435,157 @@ __device__ __forceinline__ void wgrad_epilogue(const float (&acc)[BN / 2], float
 // same logical chunk fall into 8 different bank groups.
 __device__ __forceinline__ uint32_t swz128(uint32_t box, int r, int q) { return box + r * 128 + ((q ^ (r & 7)) << 4); }
 
+// ---- TN / NN producer: one ring stage of a tile ----------------------------------------------------------------------------------
+// k-chunks i .. i + nch - 1 of the tile at (m0, n0) into `stage`: the A rows shifted by the chunk's tap (9 taps of a 3x3 conv over a
+// zero-bordered activation, or row taps), B K-major (TN) or MN-major (NN: one 3-D box or BN / 64 2-D boxes per chunk).
+template <int BN, int MODE>
+__device__ __forceinline__ void load_operand_stage(uint8_t* stage, const CUtensorMap* tmA, const CUtensorMap* tmB, uint64_t* bar, TileInfo t, int i,
+                                                   int nch, int kc_per_tap, int K, int N, int ntaps, int tap_w, int tap_sign, int mn3d) {
+  using Cfg = GemmCfg<BN>;
+  constexpr int B_BOXES = (MODE == 0) ? 1 : BN / 64;
+  // the producer thread is issue-bound: per-chunk index math is done once, box loops are fully unrolled
+  int tp = 0, kc = i;
+  if (ntaps > 1) { tp = i / kc_per_tap; kc = i - tp * kc_per_tap; }
+  for (int ch = 0; ch < nch; ++ch) {
+    uint8_t* sa = stage + ch * Cfg::STAGE_BYTES;
+    uint8_t* sb = sa + Cfg::A_BYTES;
+    int shift = 0;
+    if (ntaps == 9) shift = tap_sign * ((tp / 3 - 1) * tap_w + (tp % 3 - 1));
+    else if (ntaps > 1) shift = tap_sign * tp * tap_w;        // row taps (space-to-depth stem): tap t reads row m + t * tap_w
+    tma_load_2d(sa, tmA, bar, kc * BK, t.m0 + shift);
+    if (MODE == 0) {
+      tma_load_2d(sb, tmB, bar, tp * K + kc * BK, t.n0);
+    } else if (mn3d) {
+      tma_load_3d(sb, tmB, bar, 0, kc * BK, (tp * N + t.n0) >> 6);
+    } else {
+#pragma unroll
+      for (int j = 0; j < B_BOXES; ++j) tma_load_2d(sb + j * (BK * 128), tmB, bar, tp * N + t.n0 + j * 64, kc * BK);
+    }
+    if (++kc == kc_per_tap) { kc = 0; ++tp; }
+  }
+}
+
+// ---- TN / NN epilogue -------------------------------------------------------------------------------------------------------------
+// Output row of A-row m: re-mapped between zero-bordered and compact pixel rows where asked; -1 = not written (m >= M, or a border
+// row under UNPAD). Output rows are int: cb_gemm's row counts are.
+__device__ __forceinline__ int output_row(const GemmEpi& epi, int m, int M) {
+  bool row_ok = m < M;
+  int64_t orow = m;
+  if (epi.rowmap == CB_ROWMAP_PAD) {
+    const int hw = epi.H * epi.W;
+    const int img = m / hw;
+    const int r = m - img * hw;
+    const int y = r / epi.W, x = r - y * epi.W;
+    orow = (static_cast<int64_t>(img) * (epi.H + 2) + y + 1) * (epi.W + 2) + x + 1;
+  } else if (epi.rowmap == CB_ROWMAP_UNPAD) {
+    const int wp = epi.W + 2, hp = epi.H + 2;
+    const int img = m / (hp * wp);
+    const int r = m - img * (hp * wp);
+    const int y = r / wp, x = r - y * wp;
+    row_ok = row_ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
+    orow = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
+  }
+  return row_ok ? static_cast<int>(orow) : -1;
+}
+
+// The launch's epilogue kind (see the EK_* functions) and switches, fixed per launch.
+struct EpiKind {
+  int kind;
+  bool relu, guard, has_res, has_aux, has_shift, has_out2;
+};
+__device__ __forceinline__ EpiKind epilogue_kind(const GemmEpi& epi, int N) {
+  EpiKind k;
+  k.has_res = epi.residual != nullptr;
+  k.has_aux = epi.aux != nullptr;
+  k.has_shift = epi.shift != nullptr;
+  k.has_out2 = epi.out2 != nullptr;
+  const bool full = (N & 15) == 0 && epi.scale == nullptr;
+  const bool drop = epi.drop_thresh != 0;
+  k.kind = EK_GENERIC;
+  if (full) {
+    if (!drop && !k.has_out2 && !k.has_aux && (epi.act == CB_ACT_NONE || epi.act == CB_ACT_RELU)) k.kind = EK_SHIFT_ACT;
+    else if (!drop && !k.has_out2 && !k.has_shift && k.has_aux && epi.aux_mode == CB_AUX_RELU_MASK && epi.act == CB_ACT_NONE) k.kind = EK_RELU_MASK;
+    else if (drop && !k.has_out2 && !k.has_aux && epi.act == CB_ACT_NONE) k.kind = EK_DROP_RES;
+    else if (!drop && k.has_out2 && !k.has_aux && !k.has_res && epi.act == CB_ACT_GELU_STASH_GRAD) k.kind = EK_GELU_STASH;
+    else if (!drop && !k.has_out2 && !k.has_shift && k.has_aux && epi.aux_mode == CB_AUX_MUL && epi.act == CB_ACT_NONE) k.kind = EK_AUX_MUL;
+  }
+  k.relu = epi.act == CB_ACT_RELU;
+  k.guard = (N & 15) != 0;                 // ragged last 16 columns: per-vector column checks in the generic epilogue
+  return k;
+}
+
+// One lane's 16 columns [nb, nb + 16) of output row orow (nb < N): the fp32 values from its staging row at srow, the residual /
+// aux 16-byte chunks q, q + 1 of row brow of their 128B-swizzled [128 x 64] boxes (zeros beyond N), the fused epilogue, 16-byte
+// stores.
+__device__ __forceinline__ void epilogue_store16(const GemmEpi& epi, const EpiKind& ek, uint64_t dseed, uint32_t srow, int64_t orow, int nb, int N,
+                                                 uint32_t res_box, uint32_t aux_box, int brow, int q) {
+  constexpr int NC = 16;
+  float f[NC];
+#pragma unroll
+  for (int j = 0; j < NC / 4; ++j) {
+    const uint4 u = lds128(srow + j * 16);
+    f[4 * j] = __uint_as_float(u.x); f[4 * j + 1] = __uint_as_float(u.y);
+    f[4 * j + 2] = __uint_as_float(u.z); f[4 * j + 3] = __uint_as_float(u.w);
+  }
+  uint32_t res16[NC / 2], aux16[NC / 2];
+  if (ek.has_res) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint4 u = lds128(swz128(res_box, brow, q + j));
+      res16[4 * j] = u.x; res16[4 * j + 1] = u.y; res16[4 * j + 2] = u.z; res16[4 * j + 3] = u.w;
+    }
+  }
+  if (ek.has_aux) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint4 u = lds128(swz128(aux_box, brow, q + j));
+      aux16[4 * j] = u.x; aux16[4 * j + 1] = u.y; aux16[4 * j + 2] = u.z; aux16[4 * j + 3] = u.w;
+    }
+  }
+  float shv[NC];                                  // shift (bias / FrozenBN shift) of these columns
+  if (ek.has_shift) {
+#pragma unroll
+    for (int j = 0; j < NC; j += 4) {
+      float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (nb + j + 4 <= N) s4 = __ldg(reinterpret_cast<const float4*>(epi.shift + nb + j));
+      shv[j] = s4.x; shv[j + 1] = s4.y; shv[j + 2] = s4.z; shv[j + 3] = s4.w;
+    }
+  }
+  uint32_t o2_16[NC / 2];
+  switch (ek.kind) {
+    case EK_SHIFT_ACT: epilogue_shift_act<NC>(f, shv, ek.has_shift, res16, ek.has_res, ek.relu); break;
+    case EK_RELU_MASK: epilogue_relu_mask<NC>(f, res16, ek.has_res, aux16); break;
+    case EK_DROP_RES:
+      epilogue_drop_res<NC>(f, shv, ek.has_shift, res16, ek.has_res, dseed, static_cast<uint64_t>(orow) * static_cast<uint64_t>(N) + nb,
+                            epi.drop_thresh, epi.drop_inv_keep);
+      break;
+    case EK_GELU_STASH: epilogue_gelu_stash<NC>(f, shv, ek.has_shift, o2_16); break;
+    case EK_AUX_MUL: epilogue_aux_mul<NC>(f, res16, ek.has_res, aux16); break;
+    default:
+      if (ek.guard) epilogue_math<NC, true>(f, epi, shv, ek.has_shift, dseed, nb, N, orow, res16, ek.has_res, aux16, ek.has_aux, o2_16, ek.has_out2);
+      else epilogue_math<NC, false>(f, epi, shv, ek.has_shift, dseed, nb, N, orow, res16, ek.has_res, aux16, ek.has_aux, o2_16, ek.has_out2);
+  }
+  if (epi.out_fp32) {
+    float* o = reinterpret_cast<float*>(epi.out) + orow * epi.out_ld + nb;
+#pragma unroll
+    for (int j = 0; j < NC; j += 4)
+      if (nb + j + 4 <= N) *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+  } else {
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(epi.out) + orow * epi.out_ld + nb;
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+      if (nb + 8 * j + 8 <= N)
+        *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
+                                                          pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
+  }
+  if (ek.has_out2) {
+    __nv_bfloat16* o = epi.out2 + orow * epi.out2_ld + nb;
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+      if (nb + 8 * j + 8 <= N) *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(o2_16[4 * j], o2_16[4 * j + 1], o2_16[4 * j + 2], o2_16[4 * j + 3]);
+  }
+}
+
 // ===================================== TN / NN: ping-pong consumers =====================================
 template <int BN, int MODE>
 __global__ void __launch_bounds__(PP_THREADS, 1)
@@ -491,7 +645,6 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
     // ===================== TMA producer warpgroup =====================
     setmaxnreg_dec<PP_PRODUCER_REGS>();
     if (warp == 0 && lane == 0) {
-      constexpr int B_BOXES = (MODE == 0) ? 1 : BN / 64;
       int s = 0;        // smem ring position / phase, carried across tiles
       uint32_t ph = 0;
       // residual / aux boxes of a tile into its input buffer, or into the next ring stage (N_IN = 0); rows and columns outside
@@ -537,26 +690,8 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
           const int nch = min(KCH, n_iters - i);
           mbar_wait(&empty_bar[s], ph ^ 1);
           mbar_expect_tx(&full_bar[s], nch * Cfg::STAGE_BYTES);
-          // the producer thread is issue-bound: per-chunk index math is done once, box loops are fully unrolled
-          int tp = 0, kc = i;
-          if (ntaps > 1) { tp = i / kc_per_tap; kc = i - tp * kc_per_tap; }
-          for (int ch = 0; ch < nch; ++ch) {
-            uint8_t* sa = smem + s * stage_bytes + ch * Cfg::STAGE_BYTES;
-            uint8_t* sb = sa + Cfg::A_BYTES;
-            int shift = 0;
-            if (ntaps == 9) shift = tap_sign * ((tp / 3 - 1) * tap_w + (tp % 3 - 1));
-            else if (ntaps > 1) shift = tap_sign * tp * tap_w;        // row taps (space-to-depth stem): tap t reads row m + t * tap_w
-            tma_load_2d(sa, &tmA, &full_bar[s], kc * BK, t.m0 + shift);
-            if (MODE == 0) {
-              tma_load_2d(sb, &tmB, &full_bar[s], tp * K + kc * BK, t.n0);
-            } else if (epi.mn3d) {
-              tma_load_3d(sb, &tmB, &full_bar[s], 0, kc * BK, (tp * N + t.n0) >> 6);
-            } else {
-#pragma unroll
-              for (int j = 0; j < B_BOXES; ++j) tma_load_2d(sb + j * (BK * 128), &tmB, &full_bar[s], tp * N + t.n0 + j * 64, kc * BK);
-            }
-            if (++kc == kc_per_tap) { kc = 0; ++tp; }
-          }
+          load_operand_stage<BN, MODE>(smem + s * stage_bytes, &tmA, &tmB, &full_bar[s], t, i, nch, kc_per_tap, K, N, ntaps, tap_w, tap_sign,
+                                       epi.mn3d);
           if (++s == STAGES) { s = 0; ph ^= 1; }
           if (i == 0 && tile == unit) dbg_stamp(epi, 2);
         }
@@ -591,21 +726,7 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
   // epilogue: lane (er, eh) handles row er of the warp's 16, columns eh * 16 .. eh * 16 + 15 of each 32-column slice
   const int er = lane & 15, eh = lane >> 4;
   float* stg = reinterpret_cast<float*>(stg_base) + (warp - 4) * STG_WARP_FLOATS;
-  const bool has_out2 = epi.out2 != nullptr;
-  const bool has_shift = epi.shift != nullptr;
-  // epilogue kind, fixed for the launch (see the EK_* functions)
-  const bool full = (N & 15) == 0 && epi.scale == nullptr;
-  const bool drop = epi.drop_thresh != 0;
-  int kind = EK_GENERIC;
-  if (full) {
-    if (!drop && !has_out2 && !has_aux && (epi.act == CB_ACT_NONE || epi.act == CB_ACT_RELU)) kind = EK_SHIFT_ACT;
-    else if (!drop && !has_out2 && !has_shift && has_aux && epi.aux_mode == CB_AUX_RELU_MASK && epi.act == CB_ACT_NONE) kind = EK_RELU_MASK;
-    else if (drop && !has_out2 && !has_aux && epi.act == CB_ACT_NONE) kind = EK_DROP_RES;
-    else if (!drop && has_out2 && !has_aux && !has_res && epi.act == CB_ACT_GELU_STASH_GRAD) kind = EK_GELU_STASH;
-    else if (!drop && !has_out2 && !has_shift && has_aux && epi.aux_mode == CB_AUX_MUL && epi.act == CB_ACT_NONE) kind = EK_AUX_MUL;
-  }
-  const bool kind_relu = epi.act == CB_ACT_RELU;
-  const bool guard = (N & 15) != 0;                 // ragged last 16 columns: per-vector column checks in the generic epilogue
+  const EpiKind ek = epilogue_kind(epi, N);
 
   for (int local = wg, tile = unit + wg * n_units; tile < total_tiles; local += 2, tile += 2 * n_units) {
     const TileInfo t = decode_tile<BN>(tile, tiles_m, tiles_n);
@@ -623,26 +744,7 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
     // this lane's row in each 64-row half: A-row space m (residual / aux) -> output row (re-mapped; -1 = not written)
     int orow_half[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = t.m0 + h * 64 + wq * 16 + er;
-      bool row_ok = m < M;
-      int64_t orow = m;
-      if (epi.rowmap == CB_ROWMAP_PAD) {
-        const int hw = epi.H * epi.W;
-        const int img = m / hw;
-        const int r = m - img * hw;
-        const int y = r / epi.W, x = r - y * epi.W;
-        orow = (static_cast<int64_t>(img) * (epi.H + 2) + y + 1) * (epi.W + 2) + x + 1;
-      } else if (epi.rowmap == CB_ROWMAP_UNPAD) {
-        const int wp = epi.W + 2, hp = epi.H + 2;
-        const int img = m / (hp * wp);
-        const int r = m - img * (hp * wp);
-        const int y = r / wp, x = r - y * wp;
-        row_ok = row_ok && y >= 1 && y <= epi.H && x >= 1 && x <= epi.W;
-        orow = (static_cast<int64_t>(img) * epi.H + (y - 1)) * epi.W + (x - 1);
-      }
-      orow_half[h] = row_ok ? static_cast<int>(orow) : -1;     // (output rows are int: cb_gemm's row counts are)
-    }
+    for (int h = 0; h < 2; ++h) orow_half[h] = output_row(epi, t.m0 + h * 64 + wq * 16 + er, M);
     // per 32-column slice, the staging pass of each half: rows wrow .. wrow + 15 of the tile from accumulator half h
 #pragma unroll
     for (int sc = 0; sc < BN / 32; ++sc) {
@@ -666,75 +768,11 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
         const int nb = t.n0 + sc * 32 + eh * 16;        // global column of f[0]
         const int64_t orow = h ? orow_half[1] : orow_half[0];
         if (orow < 0 || nb >= N) continue;
-        constexpr int NC = 16;
-        float f[NC];
-        const uint32_t srow = smem_u32(stg + er * STG_PITCH + eh * 16);
-#pragma unroll
-        for (int j = 0; j < NC / 4; ++j) {
-          const uint4 u = lds128(srow + j * 16);
-          f[4 * j] = __uint_as_float(u.x); f[4 * j + 1] = __uint_as_float(u.y);
-          f[4 * j + 2] = __uint_as_float(u.z); f[4 * j + 3] = __uint_as_float(u.w);
-        }
-        // residual / aux of these 16 columns: box (column / 64), 16-byte chunks q, q + 1 of row wrow + er (zeros beyond N)
-        uint32_t res16[NC / 2], aux16[NC / 2];
+        // residual / aux of these 16 columns: box (tile column / 64)
         const int tc = sc * 32 + eh * 16;               // tile column of f[0]
-        const int q = (tc & 63) >> 3;
-        if (has_res) {
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint4 u = lds128(swz128(in_buf + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
-            res16[4 * j] = u.x; res16[4 * j + 1] = u.y; res16[4 * j + 2] = u.z; res16[4 * j + 3] = u.w;
-          }
-        }
-        if (has_aux) {
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint4 u = lds128(swz128(in_buf + (has_res ? IN_TILE_BYTES : 0) + (tc >> 6) * IN_BOX_BYTES, wrow + er, q + j));
-            aux16[4 * j] = u.x; aux16[4 * j + 1] = u.y; aux16[4 * j + 2] = u.z; aux16[4 * j + 3] = u.w;
-          }
-        }
-        float shv[NC];                                  // shift (bias / FrozenBN shift) of these columns
-        if (has_shift) {
-#pragma unroll
-          for (int j = 0; j < NC; j += 4) {
-            float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (nb + j + 4 <= N) s4 = __ldg(reinterpret_cast<const float4*>(epi.shift + nb + j));
-            shv[j] = s4.x; shv[j + 1] = s4.y; shv[j + 2] = s4.z; shv[j + 3] = s4.w;
-          }
-        }
-        uint32_t o2_16[NC / 2];
-        switch (kind) {
-          case EK_SHIFT_ACT: epilogue_shift_act<NC>(f, shv, has_shift, res16, has_res, kind_relu); break;
-          case EK_RELU_MASK: epilogue_relu_mask<NC>(f, res16, has_res, aux16); break;
-          case EK_DROP_RES:
-            epilogue_drop_res<NC>(f, shv, has_shift, res16, has_res, dseed, static_cast<uint64_t>(orow) * static_cast<uint64_t>(N) + nb,
-                                  epi.drop_thresh, epi.drop_inv_keep);
-            break;
-          case EK_GELU_STASH: epilogue_gelu_stash<NC>(f, shv, has_shift, o2_16); break;
-          case EK_AUX_MUL: epilogue_aux_mul<NC>(f, res16, has_res, aux16); break;
-          default:
-            if (guard) epilogue_math<NC, true>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
-            else epilogue_math<NC, false>(f, epi, shv, has_shift, dseed, nb, N, orow, res16, has_res, aux16, has_aux, o2_16, has_out2);
-        }
-        if (epi.out_fp32) {
-          float* o = reinterpret_cast<float*>(epi.out) + orow * epi.out_ld + nb;
-#pragma unroll
-          for (int j = 0; j < NC; j += 4)
-            if (nb + j + 4 <= N) *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-        } else {
-          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(epi.out) + orow * epi.out_ld + nb;
-#pragma unroll
-          for (int j = 0; j < 2; ++j)
-            if (nb + 8 * j + 8 <= N)
-              *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                                                                pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
-        }
-        if (has_out2) {
-          __nv_bfloat16* o = epi.out2 + orow * epi.out2_ld + nb;
-#pragma unroll
-          for (int j = 0; j < 2; ++j)
-            if (nb + 8 * j + 8 <= N) *reinterpret_cast<uint4*>(o + 8 * j) = make_uint4(o2_16[4 * j], o2_16[4 * j + 1], o2_16[4 * j + 2], o2_16[4 * j + 3]);
-        }
+        const uint32_t res_box = in_buf + (tc >> 6) * IN_BOX_BYTES;
+        epilogue_store16(epi, ek, dseed, smem_u32(stg + er * STG_PITCH + eh * 16), orow, nb, N, res_box,
+                         res_box + (has_res ? IN_TILE_BYTES : 0), wrow + er, (tc & 63) >> 3);
       }
     }
     if (in_bytes) {                                 // this warp is done with the tile's inputs: hand the buffer / stage back
@@ -747,7 +785,135 @@ __global__ void __launch_bounds__(PP_THREADS, 1)
   if (threadIdx.x == 4 * 32) dbg_stamp(epi, 11);
 }
 
-static int g_sm_limit = 0;    // tuning hook: cap on the persistent grid (0 = every SM). A long-running co-resident kernel (an NCCL
+// ===================================== TN / NN: one 128 x 256 tile on both consumers =====================================
+// Warpgroup 0 is the TMA producer as in gemm_pingpong_kernel; consumer warpgroup g multiplies rows 64g .. 64g + 63 of the CTA's
+// current tile with one wgmma m64n256k16 per k16 step (mma_tile, 128 accumulators per thread) and runs their epilogue, one tile at
+// a time: only the producer's run-ahead into the next tile overlaps an epilogue. A stage is read by both consumers, so its empty
+// barrier counts all eight consumer warps. The epilogue inputs (residual / aux, four [128 x 64] boxes each, 64 KB per input) fit
+// neither one ring stage nor a buffer beside a ring of four 48 KB stages, and three stages leave the main loop short of operands
+// (H100: 0.9 against 0.6 us per k-chunk). So they travel through the ring itself: after a tile's last operand stage the producer
+// fills one ring stage per 64 output columns with that column block's residual box and aux box, and the consumer warps hand the
+// stage back once both 32-column slices of the block are written. Those stages load under the end of the tile's main loop, and
+// the next tile's operands follow as the epilogue frees them.
+template <int MODE>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+    gemm_coop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmR,
+                     const __grid_constant__ CUtensorMap tmX, int M, int N, int K, int ntaps, int tap_w, int tap_sign, int tiles_m, int tiles_n,
+                     int total_tiles, int STAGES, int KCH, GemmEpi epi) {
+  static_assert(MODE != 1, "TN / NN only");
+  constexpr int BN = 256;
+  using Cfg = GemmCfg<BN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  const int stage_bytes = KCH * Cfg::STAGE_BYTES;
+  const bool has_res = epi.residual != nullptr, has_aux = epi.aux != nullptr;
+  const int n_in = has_res + has_aux;                       // input boxes per 64 columns (one ring stage)
+  uint8_t* stg_base = smem + STAGES * stage_bytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + EPI_BYTES);
+  uint64_t* empty_bar = full_bar + MAX_STAGES;
+
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
+  const int lane = threadIdx.x & 31;
+  const int unit = blockIdx.x, n_units = gridDim.x;
+  pdl_trigger();
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    if (has_res) tma_prefetch_desc(&tmR);
+    if (has_aux) tma_prefetch_desc(&tmX);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], CONSUMER_WARPS);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  const int kc_per_tap = (K + BK - 1) / BK;
+  const int n_iters = ntaps * kc_per_tap;
+  pdl_wait();
+
+  if (warp < 4) {
+    // ===================== TMA producer warpgroup =====================
+    setmaxnreg_dec<PP_PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
+      int s = 0;
+      uint32_t ph = 0;
+      for (int tile = unit; tile < total_tiles; tile += n_units) {
+        const TileInfo t = decode_tile<BN>(tile, tiles_m, tiles_n);
+        for (int i = 0; i < n_iters; i += KCH) {
+          const int nch = min(KCH, n_iters - i);
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          mbar_expect_tx(&full_bar[s], nch * Cfg::STAGE_BYTES);
+          load_operand_stage<BN, MODE>(smem + s * stage_bytes, &tmA, &tmB, &full_bar[s], t, i, nch, kc_per_tap, K, N, ntaps, tap_w, tap_sign,
+                                       epi.mn3d);
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+        // epilogue inputs, one ring stage per 64 columns: residual box, then aux box (rows and columns outside [M, N] arrive as zeros)
+        for (int j = 0; n_in && j < BN / 64; ++j) {
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          mbar_expect_tx(&full_bar[s], n_in * IN_BOX_BYTES);
+          uint8_t* dst = smem + s * stage_bytes;
+          if (has_res) tma_load_2d(dst, &tmR, &full_bar[s], t.n0 + j * 64, t.m0);
+          if (has_aux) tma_load_2d(dst + (has_res ? IN_BOX_BYTES : 0), &tmX, &full_bar[s], t.n0 + j * 64, t.m0);
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumer warpgroups: rows 64 wg .. 64 wg + 63 of every tile =====================
+  setmaxnreg_inc<PP_CONSUMER_REGS>();
+  const int wg = (warp >> 2) - 1;
+  const int wq = warp & 3;                  // rows 16 wq .. 16 wq + 15 of the warpgroup's 64
+  const uint32_t smem0 = smem_u32(smem);
+  const uint64_t dseed = epi.drop_thresh ? drop_seed(epi.seed, epi.seed_off) : 0ull;   // after pdl_wait: the word is device data
+  const EpiKind ek = epilogue_kind(epi, N);
+  // epilogue: lane (er, eh) handles row er of the warp's 16, columns eh * 16 .. eh * 16 + 15 of each 32-column slice
+  const int er = lane & 15, eh = lane >> 4;
+  const int brow = wg * 64 + wq * 16 + er;  // this lane's tile row
+  float* stg = reinterpret_cast<float*>(stg_base) + (warp - 4) * STG_WARP_FLOATS;
+  float acc[BN / 2];
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = unit; tile < total_tiles; tile += n_units) {
+    const TileInfo t = decode_tile<BN>(tile, tiles_m, tiles_n);
+    mma_tile<BN, 0, MODE != 0>(acc, smem0, stage_bytes, KCH, STAGES, n_iters, wg, lane, s, ph, full_bar, empty_bar);
+    const int orow = output_row(epi, t.m0 + brow, M);
+#pragma unroll
+    for (int j = 0; j < BN / 64; ++j) {
+      // the residual and aux boxes of columns 64 j .. 64 j + 63, in ring stage s
+      if (n_in) mbar_wait_unguarded(&full_bar[s], ph);
+      const uint32_t res_box = smem0 + s * stage_bytes;
+      const uint32_t aux_box = res_box + (has_res ? IN_BOX_BYTES : 0);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int sc = 2 * j + h;
+        // fragment -> staging: this warp's 16 rows x 32 columns, then one row segment per lane
+        __syncwarp();
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int f = sc * 4 + jj;
+          float* p = stg + (lane >> 2) * STG_PITCH + jj * 8 + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(p) = make_float2(acc[4 * f], acc[4 * f + 1]);
+          *reinterpret_cast<float2*>(p + 8 * STG_PITCH) = make_float2(acc[4 * f + 2], acc[4 * f + 3]);
+        }
+        __syncwarp();
+        const int tc = sc * 32 + eh * 16;               // tile column of this lane's 16
+        const int nb = t.n0 + tc;
+        if (orow >= 0 && nb < N)
+          epilogue_store16(epi, ek, dseed, smem_u32(stg + er * STG_PITCH + eh * 16), orow, nb, N, res_box, aux_box, brow, (tc & 63) >> 3);
+      }
+      if (n_in) {                               // this warp is done with the boxes: hand the stage back
+        __syncwarp();
+        mbar_arrive_if(&empty_bar[s], lane == 0);
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+    }
+  }
+}
+
+static int g_sm_limit = 0;   // tuning hook: cap on the persistent grid (0 = every SM). A long-running co-resident kernel (an NCCL
                               // all-reduce overlapped with the backward pass) pins some SMs for its whole duration; with the static
                               // round-robin tile schedule the CTAs that cannot be placed run as a second wave. Capping the grid at
                               // the SM count minus the co-resident kernel's CTAs avoids the second wave.
@@ -814,7 +980,9 @@ static SmemPlan plan_ring(int bn, bool staging, int kiters, int force_kch, int i
   if (p.stages > cap) p.stages = cap;
   return p;
 }
+// TN / NN 128 x 256 (gemm_coop_kernel): the ring alone, four one-chunk stages of 48 KB; epilogue inputs pass through it.
 static SmemPlan plan_smem(int bn, bool staging, int kiters, int force_kch = 0, int in_bytes = 0) {
+  if (staging && bn == 256) return plan_ring(bn, staging, kiters, force_kch, 0, 0);
   const SmemPlan none = plan_ring(bn, staging, kiters, force_kch, 0, 0);
   if (in_bytes == 0) return none;
   const SmemPlan two = plan_ring(bn, staging, kiters, force_kch, in_bytes, 2);
@@ -872,13 +1040,14 @@ static int launch_split_reduce(const SplitReduce& r, cudaStream_t stream, const 
   return check_launch(what);
 }
 
-// MODE 0 / 2 (TN / NN): gemm_pingpong_kernel, BN = 64 / 128. One CTA per SM.
+// MODE 0 / 2 (TN / NN): gemm_pingpong_kernel for BN = 64 / 128, gemm_coop_kernel for BN = 256. One CTA per SM.
 template <int BN, int MODE>
 static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_t stream) {
   GemmEpi epi = epi_in;
   using Cfg = GemmCfg<BN>;
+  constexpr bool wide = BN == 256;
   static bool attr_set = false;
-  auto kern = gemm_pingpong_kernel<BN, MODE>;
+  const void* kern = wide ? reinterpret_cast<const void*>(gemm_coop_kernel<MODE>) : reinterpret_cast<const void*>(gemm_pingpong_kernel<wide ? 128 : BN, MODE>);
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
@@ -920,8 +1089,12 @@ static int launch_gemm(const cb_gemm_desc& d, const GemmEpi& epi_in, cudaStream_
     return CB_ERR_INVALID;
   }
   const int smem_bytes = stages * kch * Cfg::STAGE_BYTES + sp.n_in * in_bytes + sp.epi_bytes + Cfg::BAR_BYTES + 1024;
-  launch_gemm_k(kern, grid, PP_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign, tiles_m,
-                tiles_n, total, stages, kch, sp.n_in, epi);
+  if constexpr (wide)
+    launch_gemm_k(gemm_coop_kernel<MODE>, grid, PP_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w, d.tap_sign,
+                  tiles_m, tiles_n, total, stages, kch, epi);
+  else
+    launch_gemm_k(gemm_pingpong_kernel<BN, MODE>, grid, PP_THREADS, smem_bytes, stream, ta, tb, tr, tx, d.m, d.n, d.k, d.ntaps, d.tap_w,
+                  d.tap_sign, tiles_m, tiles_n, total, stages, kch, sp.n_in, epi);
   return check_launch("cb_gemm");
 }
 
@@ -939,16 +1112,19 @@ struct LaunchCfg {
 static LaunchCfg choose_config(const cb_gemm_desc& d, int units) {
   const int kc = ceil_div(d.k, BK);
   const bool wgrad = d.mode == CB_GEMM_WGRAD;
-  // TN / NN: 128 x 256 would need 256 fp32 accumulators per consumer thread, more than its 232 registers; an explicit
-  // block_n = 256 runs on 128-wide tiles
+  if (!wgrad && (d.reserved & CB_GEMM_FORCE_WIDE)) return {256, 1};
+  // TN / NN: a ping-pong consumer owning a 128 x 256 tile would need 256 fp32 accumulators per thread, more than its 232
+  // registers, so an explicit block_n = 256 runs on 128-wide tiles; the 128 x 256 tile of gemm_coop_kernel is only ever the
+  // model's pick (block_n = 0) or forced through reserved
   const int block_n = (!wgrad && d.block_n == 256) ? 128 : d.block_n;
+  const bool wide_ok = !wgrad && d.block_n == 0 && !(d.reserved & CB_GEMM_NO_WIDE);
   static const int cand[3] = {64, 128, 256};
   LaunchCfg best = {64, 1};
   double best_cost = 1e30;
   for (int c = 0; c < 3; ++c) {
     const int bn = cand[c];
     if (block_n && bn != block_n) continue;
-    if (!wgrad && bn == 256) continue;
+    if (!wgrad && bn == 256 && !wide_ok) continue;
     if (bn > 64 && d.n <= bn / 2) continue;               // mostly padding
     const int64_t base = static_cast<int64_t>(ceil_div(d.m, BM)) * ceil_div(d.n, bn) * (wgrad ? d.ntaps : 1);
     const int max_split = wgrad ? (d.split_k > 0 ? d.split_k : (kc < 32 ? kc : 32)) : 1;
@@ -968,13 +1144,20 @@ static LaunchCfg choose_config(const cb_gemm_desc& d, int units) {
       double cost;
       if (wgrad) {
         cost = rounds * (main_loop + bn * 24.0) + 2500.0;
+      } else if (bn == 256) {
+        // one tile at a time: its epilogue, on all eight consumer warps, is not overlapped by another tile's main loop; a second
+        // output (the gelu' stash) about doubles it. Fitted on an H100 to the TN / NN launches of the training step, each timed
+        // on 128 x 256 tiles and on the model's pick of 128 x 64 / 128 x 128 (tools/profile_gemm_launches.py --ab): no pick
+        // slower than the other tile
+        cost = rounds * (main_loop + bn * 20.0 * (d.out2 ? 2.0 : 1.0)) + 2500.0;
       } else {
         const double epi = bn * 30.0;
         const double per_tile = main_loop > 0.5 * (main_loop + epi) ? main_loop : 0.5 * (main_loop + epi);
         cost = rounds * per_tile + 0.5 * epi + 2500.0;
       }
-      if (cost < best_cost) {
-        best_cost = cost;
+      // the 128 x 256 tile must beat the best ping-pong width by 5 %: within that the model cannot tell them apart
+      if ((bn == 256 && !wgrad ? cost / 0.95 : cost) < best_cost) {
+        best_cost = bn == 256 && !wgrad ? cost / 0.95 : cost;
         best = {bn, real_sp};
       }
     }
@@ -1347,6 +1530,7 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream_v) {
     switch (lc.bn) {
       case 64: return nn ? launch_gemm<64, 2>(d, epi, stream) : launch_gemm<64, 0>(d, epi, stream);
       case 128: return nn ? launch_gemm<128, 2>(d, epi, stream) : launch_gemm<128, 0>(d, epi, stream);
+      case 256: return nn ? launch_gemm<256, 2>(d, epi, stream) : launch_gemm<256, 0>(d, epi, stream);
       default: CB_REQUIRE(false, "cb_gemm: no tile width for block_n %d", d.block_n);
     }
   } else {
@@ -1380,6 +1564,13 @@ extern "C" int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* strea
     return CB_OK;
   }
   return launch_wgrad(descs, n, gp.bn, gp.split, static_cast<cudaStream_t>(stream_v), "cb_gemm_wgrad_group");
+}
+
+extern "C" int cb_gemm_tile_width(const cb_gemm_desc* d) {
+  using namespace cb;
+  if (d == nullptr || d->m <= 0 || d->n <= 0 || d->k <= 0) return 0;
+  if (d->mode != CB_GEMM_WGRAD) return choose_config(*d, sm_count()).bn;
+  return choose_config(*d, plan_sm_count()).bn;
 }
 
 extern "C" int64_t cb_gemm_workspace_bytes(const cb_gemm_desc* d) {

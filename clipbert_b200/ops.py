@@ -12,6 +12,8 @@ from ._lib import (ACT_GELU, ACT_GELU_STASH_GRAD, ACT_NONE, ACT_RELU, ACT_TANH, 
                    AUX_RELU_MASK, AUX_TANH_GRAD, CB_GEMM_TN, CB_GEMM_WGRAD, ROWMAP_NONE, ROWMAP_PAD, ROWMAP_UNPAD)
 
 CB_GEMM_NN = 2
+GEMM_FORCE_WIDE = 1 << 12   # cb_gemm_desc.reserved: TN / NN on 128 x 256 tiles (CB_GEMM_FORCE_WIDE)
+GEMM_NO_WIDE = 1 << 13      # ... never on 128 x 256 tiles (CB_GEMM_NO_WIDE)
 _c = ctypes
 _vp, _i, _i64, _f, _u64 = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_float, _c.c_uint64
 
@@ -298,6 +300,22 @@ def _load_tuning():
             _tuning = {}
 
 
+def _tuned(kw):
+    """kw with the tuning table's launch configuration, when it has one for the shape and kw sets none. A TN / NN entry with
+    block_n 256 is the 128 x 256 tile (an explicit block_n = 256 means 128 x 128 there)."""
+    if _tuning is None:
+        _load_tuning()
+    if not _tuning or "block_n" in kw or "reserved" in kw:
+        return kw
+    t = _tuning.get(gemm_key(kw))
+    if t is None:
+        return kw
+    bn, reserved = t[0], (t[2] << 8) | (32 if (len(t) > 3 and t[3]) else 0)
+    if bn == 256 and kw.get("mode", CB_GEMM_TN) != CB_GEMM_WGRAD:
+        bn, reserved = 0, reserved | GEMM_FORCE_WIDE
+    return dict(kw, block_n=bn, split_k=t[1], reserved=reserved)
+
+
 def _gemm_descs(kws):
     arr = (L.GemmDesc * len(kws))()
     for d, kw in zip(arr, kws):
@@ -309,6 +327,12 @@ def _gemm_descs(kws):
                 v = _p(v) if isinstance(v, torch.Tensor) else v
             setattr(d, k, v)
     return arr
+
+
+def gemm_tile_width(kw):
+    """cb_gemm_tile_width: the tile width cb_gemm runs the descriptor with (TN / NN 256: the 128 x 256 tile), after the tuning
+    table as gemm() applies it."""
+    return int(L.lib().cb_gemm_tile_width(_gemm_descs([_tuned(kw)])))
 
 
 def gemm_workspace_bytes(kw):
@@ -360,10 +384,7 @@ def gemm(**kw):
         _load_tuning()
     if _gemm_record is not None:
         _gemm_record.append(dict(kw))
-    if _tuning and "block_n" not in kw and "reserved" not in kw:
-        t = _tuning.get(gemm_key(kw))
-        if t is not None:
-            kw = dict(kw, block_n=t[0], split_k=t[1], reserved=(t[2] << 8) | (32 if (len(t) > 3 and t[3]) else 0))
+    kw = _tuned(kw)
     if kw.get("mode", CB_GEMM_TN) == CB_GEMM_WGRAD and deterministic():
         kw = _with_workspace(kw, gemm_workspace_bytes(kw))
     _launch_gemm("cb_gemm", [kw])

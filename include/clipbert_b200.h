@@ -180,16 +180,26 @@ typedef struct cb_gemm_desc {
   int32_t rowmap, map_h, map_w; /* spatial size (unpadded) for cb_rowmap */
   float dropout_p;
   uint64_t dropout_seed;
-  int32_t block_n;  /* 0 = let the library choose (64 / 128; 256 for CB_GEMM_WGRAD). TN / NN run 128 x 64 or 128 x 128 tiles:
-                       a 128 x 256 tile would need 256 fp32 accumulators per thread of the warpgroup that owns it, more
-                       than its 232 registers, so an explicit 256 for TN / NN runs on 128-wide tiles */
+  int32_t block_n;  /* 0 = let the library choose (64 / 128 / 256). An explicit block_n for TN / NN picks the ping-pong kernel's
+                       128 x 64 or 128 x 128 tiles: there a 128 x 256 tile would need 256 fp32 accumulators per thread of
+                       the warpgroup that owns it, more than its 232 registers, so an explicit 256 runs on 128-wide tiles.
+                       TN / NN 128 x 256 tiles (both consumer warpgroups on one tile) are chosen by the library only, or
+                       forced through reserved */
   int32_t reserved; /* tuning / test knobs: bits 8-11 k-chunks per pipeline stage (0 = automatic; for cb_gemm_wgrad_group,
-                       descs[0]'s apply to the whole group); other bits ignored */
+                       descs[0]'s apply to the whole group); CB_GEMM_FORCE_WIDE / CB_GEMM_NO_WIDE (TN / NN, for tests and A/B
+                       runs); other bits ignored */
   void* workspace;  /* deterministic mode, CB_GEMM_WGRAD: fp32 split planes, 16-byte aligned (NULL / ignored otherwise) */
   int64_t workspace_bytes;
 } cb_gemm_desc;
 
+/* cb_gemm_desc.reserved bits, TN / NN: run on 128 x 256 tiles whatever block_n says / never on 128 x 256 tiles */
+#define CB_GEMM_FORCE_WIDE (1 << 12)
+#define CB_GEMM_NO_WIDE (1 << 13)
+
 int cb_gemm(const cb_gemm_desc* desc, void* stream);
+/* tile width cb_gemm runs desc with (64, 128 or 256; for TN / NN 256 is the 128 x 256 tile of both consumer warpgroups), or 0
+ * for an empty shape; launches nothing */
+int cb_gemm_tile_width(const cb_gemm_desc* desc);
 /* bytes of workspace a CB_GEMM_WGRAD descriptor needs in deterministic mode (0: one K-split, or not a weight gradient) */
 int64_t cb_gemm_workspace_bytes(const cb_gemm_desc* desc);
 /* n independent CB_GEMM_WGRAD problems in ONE persistent launch: the weight gradients of the four Linear layers of a BertLayer

@@ -176,7 +176,10 @@ def main():
         cands = [c + (0,) for c in cands] + [c + (1,) for c in cands if c[0] == 64 and c[2] in (0, 1)]
         best, best_t = None, base if base is not None else 1e9
         for (bn, sp, kch, occ2) in cands:
-            t = time_cfg(ops, dict(call, block_n=bn, split_k=sp, reserved=(kch << 8) | (32 if occ2 else 64)))
+            reserved = (kch << 8) | (32 if occ2 else 64)
+            if bn == 256 and mode != 1:      # TN / NN 128 x 256 tiles are forced through reserved (block_n = 256 means 128 there)
+                reserved |= ops.GEMM_FORCE_WIDE
+            t = time_cfg(ops, dict(call, block_n=0 if reserved & ops.GEMM_FORCE_WIDE else bn, split_k=sp, reserved=reserved))
             if t is not None and t < best_t * 0.97:
                 best, best_t = (bn, sp, kch, occ2), t
         if best is not None:
@@ -192,7 +195,8 @@ def main():
         except Exception:
             old = {}
     old.update(table)
-    json.dump(dict(device=torch.cuda.get_device_name(0), note="(block_n, split_k, kch, two CTAs per SM) per GEMM shape; see tools/autotune_gemm.py",
+    json.dump(dict(device=torch.cuda.get_device_name(0), note="(block_n, split_k, kch, two CTAs per SM) per GEMM shape (TN / NN block_n 256: "
+                   "the 128 x 256 tile); see tools/autotune_gemm.py",
                    configs=old), open(args.out, "w"), indent=0, sort_keys=True)
     print("tuned %d / %d shapes; predicted saving %.2f ms per step; wrote %s (%.1f s)" % (len(table), len(uniq), saved / 1e3, args.out, time.time() - t0))
     os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)

@@ -1,7 +1,9 @@
 """Device time of every GEMM shape of one training step, each timed on its own: the cb_gemm descriptors of one eager step are
 recorded (as bench.py's roofline pass does), then every distinct descriptor is replayed --reps times back to back on one stream
-between CUDA events. Unlike tools/profile_step.py, no host gap and no side-stream kernel lands inside a launch's window.
-Writes tool_out/gemm_launches.txt (or --out). Usage: python tools/profile_gemm_launches.py [--reps 20]"""
+between CUDA events. Unlike tools/profile_step.py, no host gap and no side-stream kernel lands inside a launch's window. The tile
+column is the tile the launch ran with (128 x 256 on TN / NN: both consumer warpgroups on one tile). --ab also times every TN / NN
+shape forced onto 128 x 256 tiles and kept off them (cb_gemm_desc.reserved CB_GEMM_FORCE_WIDE / CB_GEMM_NO_WIDE).
+Writes tool_out/gemm_launches.txt (or --out). Usage: python tools/profile_gemm_launches.py [--reps 20] [--ab]"""
 import argparse
 import os
 import sys
@@ -24,6 +26,7 @@ def main():
     ap.add_argument("--txt_len", type=int, default=32)
     ap.add_argument("--n_ex", type=int, default=1)
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--ab", action="store_true")
     ap.add_argument("--out", default="tool_out/gemm_launches.txt")
     args = ap.parse_args()
     import clipbert_b200 as cb
@@ -63,7 +66,8 @@ def main():
     peaks = bench.load_peaks()
     rows = []
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for key, (kw, cnt) in shapes.items():
+
+    def time_us(kw):
         for _ in range(3):
             ops.gemm(**kw)
         e0.record()
@@ -71,16 +75,25 @@ def main():
             ops.gemm(**kw)
         e1.record()
         torch.cuda.synchronize()
-        us = e0.elapsed_time(e1) * 1e3 / args.reps
+        return e0.elapsed_time(e1) * 1e3 / args.reps
+
+    for key, (kw, cnt) in shapes.items():
+        us = time_us(kw)
+        tile = "128x%d" % ops.gemm_tile_width(kw)
+        ab = ""
+        if args.ab and kw.get("mode", 0) != ops.CB_GEMM_WGRAD:
+            ab = " %9.1f %9.1f" % (time_us(dict(kw, reserved=ops.GEMM_NO_WIDE)), time_us(dict(kw, reserved=ops.GEMM_FORCE_WIDE)))
         fl = 2.0 * kw["m"] * kw["n"] * kw["k"] * kw.get("ntaps", 1)
         by = bench.gemm_algorithmic_bytes(kw)
         ideal = max(fl / (peaks["tflops"] * 1e12), by / (peaks["hbm"] * 1e9)) * 1e6
-        rows.append((us * cnt / 1e3, key, cnt, us, ideal, "hbm" if by / (peaks["hbm"] * 1e9) > fl / (peaks["tflops"] * 1e12) else "tensor"))
+        rows.append((us * cnt / 1e3, key, cnt, us, ideal, "hbm" if by / (peaks["hbm"] * 1e9) > fl / (peaks["tflops"] * 1e12) else "tensor",
+                     tile, ab))
     lines = ["GEMM launches of one step (grouped wgrad launches excluded), each shape replayed %d x back to back; ideal = max(flop / %.0f"
              " TF/s, algorithmic bytes / %.0f GB/s)" % (args.reps, peaks["tflops"], peaks["hbm"]),
-             "%-62s %4s %9s %9s %9s %6s %6s" % ("shape", "n", "us", "ms/step", "ideal us", "frac", "bound")]
-    for ms, key, cnt, us, ideal, bound in sorted(rows, key=lambda r: -r[0]):
-        lines.append("%-62s %4d %9.1f %9.3f %9.1f %6.2f %6s" % (key, cnt, us, ms, ideal, ideal / us, bound))
+             "%-62s %4s %9s %9s %9s %6s %6s %8s" % ("shape", "n", "us", "ms/step", "ideal us", "frac", "bound", "tile")
+             + (" %9s %9s" % ("us <=128", "us 256") if args.ab else "")]
+    for ms, key, cnt, us, ideal, bound, tile, ab in sorted(rows, key=lambda r: -r[0]):
+        lines.append("%-62s %4d %9.1f %9.3f %9.1f %6.2f %6s %8s" % (key, cnt, us, ms, ideal, ideal / us, bound, tile) + ab)
     lines.append("total %.3f ms/step over %d launches" % (sum(r[0] for r in rows), sum(r[2] for r in rows)))
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     open(args.out, "w").write("\n".join(lines) + "\n")
