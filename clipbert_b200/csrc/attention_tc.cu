@@ -837,6 +837,208 @@ __global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_kernel(const __nv_bf
   }
 }
 
+// ------------------------------------------------------------------------------------------------ backward through the probabilities
+// The gradient of a loss on the returned probabilities A = P r (output_attentions; G = dloss / dA, fp32 [nseq, heads, l, l]):
+//   g = r G ;  D_i = sum_j P_ij g_ij ;  dS = P (g - D) ;  dQ += dS K / 8 ;  dK += dS^T Q / 8
+// added to the dQ / dK cb_attention_bwd wrote. Two kernels on the grid (ceil(l / 64), heads, nseq), the split of the long
+// backward: attn_tc_probs_bwd_q_kernel owns a 64-query tile (pass 1 over the key tiles: D, written to drow; pass 2: dS in
+// registers, dQ += dS K), attn_tc_probs_bwd_k_kernel owns a 64-key tile and loops over the query tiles with D from drow
+// (dS through shared memory, dK += dS^T Q). P is rebuilt from Q, K and the saved lse as attn_tc_probs_kernel forms it, never
+// read from the returned tensor. Every output element has one writer and a fixed order: no atomics, bit-identical runs.
+// G is read in the accumulator layout straight from global memory: a quad reads 8 consecutive floats of a row, and a row
+// starts at any 4-byte alignment (l is odd at 224 px), so the reads are scalar; elements at or beyond l are never read.
+
+// one 64-key tile of a warp's 16 query rows, from the S accumulator: ROWSUM: t0 / t1 += sum_j P r G over this thread's
+// elements of rows rq / rq + 8 (s is left as is); else s[j] becomes dS = P (r G - D). e0 = element index of (row rq, key k0)
+// in G viewed as [nseq*heads*l, l] (also the dropout index); rows with !ok and keys >= l give P = G = 0.
+template <bool ROWSUM>
+__device__ __forceinline__ void tc_probs_ds(float (&s)[8][4], const float* madd, float l0, float l1, float D0, float D1, bool ok0, bool ok1,
+                                            const float* __restrict__ dprobs, uint64_t e0, int L, int k0, int cq, float scale, const TcDrop& dc,
+                                            float& t0, float& t1) {
+  const uint64_t e1 = e0 + static_cast<uint64_t>(8) * L;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = k0 + j * 8 + cq;
+    const float m0 = madd[j * 8 + cq], m1 = madd[j * 8 + cq + 1];
+    const float p0 = ok0 ? __expf(s[j][0] * scale + m0 - l0) : 0.f, p1 = ok0 ? __expf(s[j][1] * scale + m1 - l0) : 0.f;
+    const float p2 = ok1 ? __expf(s[j][2] * scale + m0 - l1) : 0.f, p3 = ok1 ? __expf(s[j][3] * scale + m1 - l1) : 0.f;
+    float g0 = 0.f, g1 = 0.f, g2 = 0.f, g3 = 0.f;
+    if (ok0 && c < L) g0 = __ldg(dprobs + e0 + j * 8 + cq);
+    if (ok0 && c + 1 < L) g1 = __ldg(dprobs + e0 + j * 8 + cq + 1);
+    if (ok1 && c < L) g2 = __ldg(dprobs + e1 + j * 8 + cq);
+    if (ok1 && c + 1 < L) g3 = __ldg(dprobs + e1 + j * 8 + cq + 1);
+    if (dc.thresh) {
+      float r_0, r_1, r_2, r_3;
+      dropout_mult2(dc.seed, e0 + j * 8 + cq, dc.thresh, dc.inv_keep, r_0, r_1);
+      dropout_mult2(dc.seed, e1 + j * 8 + cq, dc.thresh, dc.inv_keep, r_2, r_3);
+      g0 *= r_0; g1 *= r_1; g2 *= r_2; g3 *= r_3;
+    }
+    if (ROWSUM) {
+      t0 += p0 * g0 + p1 * g1;
+      t1 += p2 * g2 + p3 * g3;
+    } else {
+      s[j][0] = p0 * (g0 - D0); s[j][1] = p1 * (g1 - D0);
+      s[j][2] = p2 * (g2 - D1); s[j][3] = p3 * (g3 - D1);
+    }
+  }
+}
+
+// dst (bf16, 16 rows r0 + lane / 4, + 8 of a 64-column block, row pitch ld) += acc * mul, in fp32, rounded once; rows >= nrows
+// are not touched
+__device__ __forceinline__ void tc_acc_add_global(const float (&acc)[8][4], __nv_bfloat16* dst, int64_t ld, int r0, int lane, int nrows,
+                                                  float mul) {
+  const int r = r0 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    if (r + 8 * half < nrows) {
+      uint32_t* row = reinterpret_cast<uint32_t*>(dst + static_cast<int64_t>(r + 8 * half) * ld + c);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 o = unpack_bf16x2(row[j * 4]);
+        row[j * 4] = pack_bf16x2(o.x + acc[j][2 * half] * mul, o.y + acc[j][2 * half + 1] * mul);
+      }
+    }
+  }
+}
+
+// dQ of one 64-query tile; writes D of its rows to drow [nseq, heads, l]
+__global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_bwd_q_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                                         int64_t ld_qkv, const int64_t* __restrict__ text_mask,
+                                                                         const float* __restrict__ lse, const float* __restrict__ dprobs,
+                                                                         float* __restrict__ drow, __nv_bfloat16* __restrict__ dq, int64_t ld_dqkv,
+                                                                         int L, int Lt, int H, float scale, TcDrop dc_in) {
+  pdl_wait();
+  const TcDrop dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
+  pdl_trigger();
+  extern __shared__ __align__(16) uint8_t tc_smem[];
+  __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(tc_smem);
+  __nv_bfloat16* Ks = Qs + TC_TILE;
+  float* madd = reinterpret_cast<float*>(Ks + TC_TILE);
+  float* lses = madd + 64;
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = qb * 64;
+  const int nq = min(64, L - q0);
+  const int64_t row0 = static_cast<int64_t>(b) * L;
+  const uint64_t prow0 = (static_cast<uint64_t>(b) * H + h) * L + q0;   // row of query q0 in G viewed as [nseq*H*L, L]
+  const bool live = warp < tc_live_slabs(nq);                          // this warp holds at least one query row < L
+  tc_load_tile(Qs, q + (row0 + q0) * ld_qkv + h * 64, ld_qkv, nq);
+  if (threadIdx.x < 64) lses[threadIdx.x] = threadIdx.x < nq ? lse[prow0 + threadIdx.x] : 0.f;
+  const int r0 = warp * 16;
+  const int rq = r0 + (lane >> 2), cq = 2 * (lane & 3);
+  const bool ok0 = rq < nq, ok1 = rq + 8 < nq;
+  const int nkb = (L + 63) / 64;
+  float D0 = 0.f, D1 = 0.f;
+  float acc[8][4];
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
+  // pass 0: D_i = sum_j P_ij r_ij G_ij; pass 1: dQ += dS K
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int kb = 0; kb < nkb; ++kb) {
+      const int k0 = kb * 64, nks = tc_live_slabs(L - k0);
+      __syncthreads();                   // every warp is done with the previous key tile
+      tc_load_tile(Ks, k + (row0 + k0) * ld_qkv + h * 64, ld_qkv, L - k0);
+      tc_key_mask(madd, text_mask, b, k0, L, Lt);
+      __syncthreads();
+      if (live) {
+        float s[8][4];
+        tc_mm_abt_live(s, Qs, Ks, r0, lane, nks);
+        const uint64_t e0 = (prow0 + rq) * L + k0;
+        if (pass == 0) {
+          tc_probs_ds<true>(s, madd, lses[rq], lses[rq + 8], 0.f, 0.f, ok0, ok1, dprobs, e0, L, k0, cq, scale, dc, D0, D1);
+        } else {
+          float u0, u1;
+          tc_probs_ds<false>(s, madd, lses[rq], lses[rq + 8], D0, D1, ok0, ok1, dprobs, e0, L, k0, cq, scale, dc, u0, u1);
+          uint32_t dsf[4][4];              // dS in the accumulator layout = the A fragments of dS K
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            dsf[j >> 1][(j & 1) * 2] = pack_bf16x2(s[j][0], s[j][1]);
+            dsf[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(s[j][2], s[j][3]);
+          }
+          tc_mm_ab_reg_live(acc, dsf, Ks, lane, nks);
+        }
+      }
+    }
+    if (pass == 0) {
+      D0 = quad_sum(D0);
+      D1 = quad_sum(D1);
+      if ((lane & 3) == 0) {
+        if (ok0) drow[prow0 + rq] = D0;
+        if (ok1) drow[prow0 + rq + 8] = D1;
+      }
+    }
+  }
+  if (live) tc_acc_add_global(acc, dq + (row0 + q0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nq, scale);
+}
+
+// dK of one 64-key tile, with D from drow
+__global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_bwd_k_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                                         int64_t ld_qkv, const int64_t* __restrict__ text_mask,
+                                                                         const float* __restrict__ lse, const float* __restrict__ dprobs,
+                                                                         const float* __restrict__ drow, __nv_bfloat16* __restrict__ dk,
+                                                                         int64_t ld_dqkv, int L, int Lt, int H, float scale, TcDrop dc_in) {
+  pdl_wait();      // drow is written by attn_tc_probs_bwd_q_kernel, the launch before this one
+  const TcDrop dc = drop_resolve(dc_in);
+  pdl_trigger();
+  extern __shared__ __align__(16) uint8_t tc_smem[];
+  __nv_bfloat16* Ks = reinterpret_cast<__nv_bfloat16*>(tc_smem);
+  __nv_bfloat16* Qs = Ks + TC_TILE;
+  __nv_bfloat16* dSs = Qs + TC_TILE;     // dS [query][key]
+  float* madd = reinterpret_cast<float*>(dSs + TC_TILE);
+  float* lses = madd + 64;
+  float* Ds = lses + 64;
+  const int kb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int k0 = kb * 64;
+  const int nk = min(64, L - k0), nks = tc_live_slabs(nk);
+  const int64_t row0 = static_cast<int64_t>(b) * L;
+  const uint64_t bh0 = (static_cast<uint64_t>(b) * H + h) * L;         // row of query 0 in G viewed as [nseq*H*L, L]
+  tc_load_tile(Ks, k + (row0 + k0) * ld_qkv + h * 64, ld_qkv, nk);
+  tc_key_mask(madd, text_mask, b, k0, L, Lt);
+  const int r0 = warp * 16;
+  const int rq = r0 + (lane >> 2), cq = 2 * (lane & 3);
+  float dkacc[8][4];
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) dkacc[j][e] = 0.f;
+  const int nqb = (L + 63) / 64;
+  for (int qb = 0; qb < nqb; ++qb) {
+    const int q0 = qb * 64, nq = min(64, L - q0);
+    const int nqs = tc_live_slabs(nq);
+    __syncthreads();                     // the previous query tile's dK products are done with Qs and dSs
+    tc_load_tile(Qs, q + (row0 + q0) * ld_qkv + h * 64, ld_qkv, nq);
+    if (threadIdx.x < 64) {
+      const bool ok = static_cast<int>(threadIdx.x) < nq;
+      lses[threadIdx.x] = ok ? lse[bh0 + q0 + threadIdx.x] : 0.f;
+      Ds[threadIdx.x] = ok ? drow[bh0 + q0 + threadIdx.x] : 0.f;
+    }
+    __syncthreads();
+    if (warp < nqs) {
+      float s[8][4], u0, u1;
+      tc_mm_abt_live(s, Qs, Ks, r0, lane, nks);
+      tc_probs_ds<false>(s, madd, lses[rq], lses[rq + 8], Ds[rq], Ds[rq + 8], rq < nq, rq + 8 < nq, dprobs, (bh0 + q0 + rq) * L + k0, L,
+                         k0, cq, scale, dc, u0, u1);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        *reinterpret_cast<uint32_t*>(dSs + rq * TC_LD + j * 8 + cq) = pack_bf16x2(s[j][0], s[j][1]);
+        *reinterpret_cast<uint32_t*>(dSs + (rq + 8) * TC_LD + j * 8 + cq) = pack_bf16x2(s[j][2], s[j][3]);
+      }
+    } else {                             // all 16 query rows beyond L: dS = 0
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        *reinterpret_cast<uint32_t*>(dSs + rq * TC_LD + j * 8 + cq) = 0u;
+        *reinterpret_cast<uint32_t*>(dSs + (rq + 8) * TC_LD + j * 8 + cq) = 0u;
+      }
+    }
+    __syncthreads();
+    if (warp < nks) tc_mm_atb_live(dkacc, dSs, Qs, r0, lane, nqs);   // this warp's 16 key rows: dK += dS^T Q
+  }
+  if (warp < nks) tc_acc_add_global(dkacc, dk + (row0 + k0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nk, scale);
+}
+
 static TcDrop make_tc_drop(float p, uint64_t seed) { return make_drop(p, seed); }
 
 // called from cb_attention_fwd / cb_attention_bwd (attention.cu) when l <= 64
@@ -971,4 +1173,36 @@ extern "C" int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t
   launch_k(attn_tc_probs_kernel, dim3(ceil_div(l, 64), heads, nseq), TC_THREADS, smem, static_cast<cudaStream_t>(stream), base, base + hid,
            ld_qkv, text_mask, lse, probs, l, lt, heads, 0.125f, make_tc_drop(dropout_p, seed));
   return check_launch("cb_attention_probs");
+}
+
+extern "C" int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const float* dprobs,
+                                      float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
+                                      float dropout_p, uint64_t seed, void* stream) {
+  using namespace cb;
+  CB_REQUIRE(head_dim == 64, "cb_attention_probs_bwd: head_dim %d unsupported (built for 64)", head_dim);
+  CB_REQUIRE(qkv && text_mask && lse && dprobs && drow && dqkv && nseq > 0 && l > 0 && lt >= 0 && lt <= l && heads > 0 && nseq <= 65535 &&
+                 heads <= 65535,
+             "cb_attention_probs_bwd: bad arguments");
+  CB_REQUIRE(ld_qkv % 8 == 0 && ld_dqkv % 8 == 0 && ld_qkv >= 3 * static_cast<int64_t>(heads) * 64 &&
+                 ld_dqkv >= 3 * static_cast<int64_t>(heads) * 64,
+             "cb_attention_probs_bwd: row pitches must be multiples of 8 and hold Q | K | V");
+  CB_REQUIRE(reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(dqkv) % 16 == 0 &&
+                 reinterpret_cast<uintptr_t>(dprobs) % 16 == 0,
+             "cb_attention_probs_bwd: qkv, dqkv and dprobs must be 16-byte aligned");
+  // q kernel: Q, K tiles + key mask, lse = 18.5 KB; k kernel: K, Q, dS tiles + key mask, lse, D = 27.8 KB
+  const int smem_q = 2 * TC_TILE * 2 + 2 * 64 * 4;
+  const int smem_k = 3 * TC_TILE * 2 + 3 * 64 * 4;
+  const __nv_bfloat16* base = static_cast<const __nv_bfloat16*>(qkv);
+  __nv_bfloat16* dbase = static_cast<__nv_bfloat16*>(dqkv);
+  const int hid = heads * 64;
+  const TcDrop dc = make_tc_drop(dropout_p, seed);
+  const dim3 grid(ceil_div(l, 64), heads, nseq);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  launch_k(attn_tc_probs_bwd_q_kernel, grid, TC_THREADS, smem_q, st, base, base + hid, ld_qkv, text_mask, lse, dprobs, drow, dbase, ld_dqkv,
+           l, lt, heads, 0.125f, dc);
+  int rc = check_launch("cb_attention_probs_bwd(q)");
+  if (rc) return rc;
+  launch_k(attn_tc_probs_bwd_k_kernel, grid, TC_THREADS, smem_k, st, base, base + hid, ld_qkv, text_mask, lse, dprobs,
+           static_cast<const float*>(drow), dbase + hid, ld_dqkv, l, lt, heads, 0.125f, dc);
+  return check_launch("cb_attention_probs_bwd(k)");
 }

@@ -130,9 +130,19 @@ class ClipBertBaseModel(nn.Module):
     Dtypes: sequence_output, pooled_output and the 13 hidden states are bf16 - the engine's own activation buffers, no copy
     (the reference's amp-O2 runs hand out fp16 here). The attentions are fp32 (B', heads, L, L), one per layer, the
     post-dropout probabilities. Autograd flows from sequence_output, pooled_output and every hidden state into every
-    parameter and into ``visual_inputs``; the attention probabilities are returned non-differentiable, the one departure
-    from the reference (whose attentions are ordinary autograd tensors).
+    parameter and into ``visual_inputs``.
+
+    ``model.differentiable_attentions = True`` (default False; also on ``head.bert``) makes the attentions of a pass that
+    records autograd differentiable too, as the reference's are: a loss on ``attentions[layer]`` (attention supervision,
+    distillation of a teacher's maps, entropy penalties) then trains every parameter below that layer and ``visual_inputs``,
+    through cb_attention_probs_bwd (include/clipbert_b200.h). A pass whose loss does not use the attentions costs and
+    computes exactly what it does with the switch off. With the default the attentions are returned non-differentiable.
+    Unsupported either way: the gradient of a score WITH RESPECT TO the returned maps (``torch.autograd.grad(score, attn)``,
+    hooks on them), which in the reference also carries dO V^T from the context product; here the context is made from the
+    kernel's own probabilities, not from the returned tensor.
     """
+
+    differentiable_attentions = False
 
     def __init__(self, config, _engine=None):
         super().__init__()
@@ -150,7 +160,8 @@ class ClipBertBaseModel(nn.Module):
         self.__dict__["_engine"] = _engine
 
     def forward(self, text_input_ids, visual_inputs, attention_mask):
-        return self._engine._run_base(text_input_ids, visual_inputs, attention_mask, self.output_hidden_states, self.output_attentions)
+        return self._engine._run_base(text_input_ids, visual_inputs, attention_mask, self.output_hidden_states, self.output_attentions,
+                                      self.differentiable_attentions)
 
 
 def _require_cuda(t):
@@ -213,7 +224,8 @@ class _BaseModelFn(torch.autograd.Function):
         ctx.module, ctx.stash = module, stash
         ctx.grid_needs_grad = grid.requires_grad
         ctx.n_hidden = len(hidden)
-        ctx.mark_non_differentiable(*attn)
+        if not flags[2]:                        # ClipBertBaseModel.differentiable_attentions
+            ctx.mark_non_differentiable(*attn)
         ctx.set_materialize_grads(False)        # unused outputs arrive as None and cost nothing in the backward
         return (seq, pooled) + tuple(hidden) + tuple(attn)
 
@@ -221,7 +233,7 @@ class _BaseModelFn(torch.autograd.Function):
     def backward(ctx, dseq, dpooled, *rest):
         stash, ctx.stash = ctx.stash, None
         m = ctx.module
-        stash["base_grads"] = (dseq, dpooled, rest[:ctx.n_hidden])
+        stash["base_grads"] = (dseq, dpooled, rest[:ctx.n_hidden], rest[ctx.n_hidden:])
         dgrid = m._backward_impl(stash, None, ctx.grid_needs_grad)
         m._backward_done()
         return None, dgrid, None, None, None, None
@@ -415,7 +427,7 @@ class _ClipBertHeadModel(nn.Module):
             return _TransformerFn.apply(self, grid, anchor, ids, mask, repeat)
         return self._forward_impl(ids, grid, mask, repeat, need_backward=False)[0]
 
-    def _run_base(self, text_input_ids, visual_inputs, attention_mask, want_hidden, want_attn):
+    def _run_base(self, text_input_ids, visual_inputs, attention_mask, want_hidden, want_attn, diff_attn=False):
         """ClipBertBaseModel.forward on this engine (the head itself is not run). visual_inputs: (B', T, h, w, 768)."""
         _require_cuda(text_input_ids)
         self._ensure_ready(text_input_ids.device)
@@ -424,7 +436,7 @@ class _ClipBertHeadModel(nn.Module):
         grid = grid.contiguous()
         ids = text_input_ids.contiguous()
         mask = attention_mask.to(torch.int64).contiguous()
-        flags = (bool(want_hidden), bool(want_attn))
+        flags = (bool(want_hidden), bool(want_attn), bool(want_attn and diff_attn))
         if torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters())):
             outs = _BaseModelFn.apply(self, grid, self.bert.pooler.dense.weight, ids, mask, flags)
             n_hidden = len(self.bert.encoder.layer) + 1 if flags[0] else 0
@@ -464,7 +476,7 @@ class _ClipBertHeadModel(nn.Module):
         H = _cfg(cfg, "hidden_size")
         heads = _cfg(cfg, "num_attention_heads")
         eps = float(_cfg(cfg, "layer_norm_eps"))
-        want_hidden, want_attn = base if base is not None else (False, False)
+        want_hidden, want_attn = base[:2] if base is not None else (False, False)
         train = self.bert.training if base is not None else self.training
         p_h = float(_cfg(cfg, "hidden_dropout_prob")) if train else 0.0
         p_a = float(_cfg(cfg, "attention_probs_dropout_prob")) if train else 0.0
@@ -648,11 +660,11 @@ class _ClipBertHeadModel(nn.Module):
         ops.dropout_offset_bind(st.get("drop_word"))       # regenerate exactly this forward's masks
         sq = ops.SideQueue()                               # wgrad GEMMs / bias sums run beside the dgrad chain
         base = st.get("base_grads")                        # ClipBertBaseModel.forward: (d sequence, d pooled, d hidden states)
-        dhidden = None
+        dhidden = dattn = None
         if base is None:
             dpre = self._head_backward(st, dout, nseq, H)  # grad w.r.t. pooler pre-activation
         else:
-            dpre, dseq, dhidden = self._base_output_grads(st, base, M, H)
+            dpre, dseq, dhidden, dattn = self._base_output_grads(st, base, M, H)
         pl = self._lin["pooler"]
         x_last = st["x_last"]
         if dpre is not None:
@@ -707,6 +719,9 @@ class _ClipBertHeadModel(nn.Module):
             self._dgrad(ao_l, dd1, M, dctx)
             dqkv = new(M, 3 * H)
             ops.attention_bwd(ly["qkv"], st["mask"], ly["ctx"], dctx, ly["lse"], dqkv, nseq, L, lt, heads, p_a, ls + 1)
+            if dattn is not None and dattn[i] is not None:      # a loss on attentions[i]: its dQ / dK added into dqkv
+                drow = new(nseq, heads, L, dtype=f32)
+                ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn[i], drow, dqkv, nseq, L, lt, heads, p_a, ls + 1)
             wg.append(self._wgrad_kw(qkv_l, dqkv, ly["x"], M))
             if group:
                 sq.run(lambda: (ops.gemm_wgrad_group(wg), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dd, ly["gel"], du, ly["a"], dd1, ly["ctx"], dqkv, ly["x"])
@@ -753,9 +768,10 @@ class _ClipBertHeadModel(nn.Module):
 
     def _base_output_grads(self, st, grads, M, H):
         """Upstream gradients of ClipBertBaseModel.forward -> (d pooler pre-activation or None, dense d sequence_output or None,
-        [d hidden_states[k] or None] or None), all bf16. d pooled goes through tanh' = 1 - pooled^2 (BertPooler,
-        transformers.py:470-476) as the heads' dpre does, here as one product on the (B', 768) rows."""
-        dseq, dpooled, dh = grads
+        [d hidden_states[k] or None] or None, [d attentions[k] or None] or None), bf16 but the attention gradients (contiguous
+        fp32: an expanded gradient such as the one of attn.sum() is materialised). d pooled goes through tanh' = 1 - pooled^2
+        (BertPooler, transformers.py:470-476) as the heads' dpre does, here as one product on the (B', 768) rows."""
+        dseq, dpooled, dh, da = grads
         bf16 = torch.bfloat16
 
         def dense(g):
@@ -765,7 +781,10 @@ class _ClipBertHeadModel(nn.Module):
         if dpooled is not None:
             pooled = st["pooled"].float()
             dpre = (dpooled.float() * (1.0 - pooled * pooled)).to(bf16)
-        return dpre, dense(dseq), ([dense(g) for g in dh] if dh else None)
+        dattn = None
+        if any(g is not None for g in da):
+            dattn = [None if g is None else g.to(torch.float32).contiguous() for g in da]
+        return dpre, dense(dseq), ([dense(g) for g in dh] if dh else None), dattn
 
     # ---- misc -------------------------------------------------------------------------------------
     def zero_grad(self, set_to_none=False):

@@ -40,6 +40,7 @@ _SIGS = {
     "cb_attention_fwd": [_vp, _i64, _vp, _vp, _i64, _vp, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_attention_bwd": [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_attention_probs": [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _u64, _vp],
+    "cb_attention_probs_bwd": [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_stem_im2col": [_vp, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp],
     "cb_maxpool3x3s2": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool3x3s2_strided": [_vp, _vp, _i, _i, _i, _i, _i64, _i64, _vp],
@@ -600,6 +601,15 @@ def attention_probs(qkv, text_mask, lse, probs, nseq, l, lt, heads, p, seed):
     """probs: fp32 [nseq, heads, l, l] contiguous, from the lse cb_attention_fwd wrote for the same arguments."""
     assert probs.dtype == torch.float32 and probs.is_contiguous() and probs.numel() == nseq * heads * l * l
     _call("cb_attention_probs", _p(qkv), qkv.shape[1], _p(text_mask), _p(lse), _p(probs), nseq, l, lt, heads, 64, p, seed, _s())
+
+
+def attention_probs_bwd(qkv, text_mask, lse, dprobs, drow, dqkv, nseq, l, lt, heads, p, seed):
+    """Adds the gradient of a loss on the probabilities (dprobs: fp32 [nseq, heads, l, l] contiguous) into dqkv's Q and K
+    blocks; drow: fp32 scratch of nseq * heads * l floats."""
+    assert dprobs.dtype == torch.float32 and dprobs.is_contiguous() and dprobs.numel() == nseq * heads * l * l
+    assert drow.dtype == torch.float32 and drow.numel() >= nseq * heads * l
+    _call("cb_attention_probs_bwd", _p(qkv), qkv.shape[1], _p(text_mask), _p(lse), _p(dprobs), _p(drow), _p(dqkv), dqkv.shape[1],
+          nseq, l, lt, heads, 64, p, seed, _s())
 
 
 # ------------------------------------------------------------------------------------------------

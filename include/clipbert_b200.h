@@ -315,6 +315,21 @@ int cb_attention_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, 
  * tile, head, sequence); rows and columns beyond l are never written. */
 int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, float* probs, int nseq,
                        int l, int lt, int heads, int head_dim, float dropout_p, uint64_t seed, void* stream);
+/* Backward through the returned probabilities A = P r (r: the dropout multipliers, 0 or 1 / (1 - p)): with G = dloss / dA,
+ * dprobs fp32 [nseq, heads, l, l], contiguous, 16-byte aligned at its base (a row starts at any 4-byte alignment),
+ *   g_ij = r_ij G_ij ;  D_i = sum_j P_ij g_ij (= sum_j A_ij G_ij) ;  dS_ij = P_ij (g_ij - D_i)
+ *   dQ_i += sum_j dS_ij K_j / 8 ;  dK_j += sum_i dS_ij Q_i / 8          (dV unchanged)
+ * ADDED to the Q and K column blocks of dqkv (what cb_attention_bwd wrote: dS is linear in the upstream gradient, so the
+ * two contributions sum); the V block, the pitch padding and everything outside the window are not touched. P is rebuilt
+ * from qkv, the mask and lse as cb_attention_probs forms it (same seed, same bound device word); the returned tensor is never
+ * read. drow: caller-owned fp32 scratch of nseq * heads * l floats (D). Arguments and alignment (qkv, dqkv, dprobs) are
+ * checked as for cb_attention_bwd, nothing is launched otherwise.
+ * Rounding: P, g, D and dS in fp32, dS rounded to bf16 before the dQ / dK products (mma.sync, fp32 accumulation), and each
+ * dQ / dK element read, added to in fp32 and rounded to bf16 once. Two kernels, one per 64-query tile (D, then dQ) and one
+ * per 64-key tile (dK); every element has one writer: no atomics, bit-identical from run to run. */
+int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const float* dprobs,
+                           float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
+                           float dropout_p, uint64_t seed, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Small helpers on the transformer side.

@@ -1,9 +1,13 @@
-"""cb_attention_probs (the attention probabilities behind ClipBertBaseModel's output_attentions) timed with CUDA events, and an eval
-bert(...) forward at 448 px with output_hidden_states / output_attentions off and on.
+"""cb_attention_probs (the attention probabilities behind ClipBertBaseModel's output_attentions) and cb_attention_probs_bwd (the
+backward through them, ClipBertBaseModel.differentiable_attentions) timed with CUDA events, an eval bert(...) forward at 448 px with
+output_hidden_states / output_attentions off and on, and a train-mode bert(...) forward + backward at 448 px with a loss on the
+attentions of all 12 layers and with none.
 
-Per shape: median over `--rounds` rounds of `--reps` back-to-back calls, and the kernel's fraction of its lower bound =
-(bytes of P written + Q and K read once) / 3.35 TB/s (the H100 SXM data-sheet HBM3 bandwidth, for a card allowed 700 W) over
-the measured time. The card name, power limit and max SM clock are read in the same run.
+Per shape: median over `--rounds` rounds of `--reps` back-to-back calls, and the kernel's fraction of its lower bound = compulsory
+bytes / 3.35 TB/s (the H100 SXM data-sheet HBM3 bandwidth, for a card allowed 700 W) over the measured time. Compulsory bytes:
+cb_attention_probs: P written + Q and K read once; cb_attention_probs_bwd: G read three times (12 l^2 bytes per (sequence, head):
+the D pass, the dQ pass and the dK kernel) + the bf16 dQ and dK read and written. cb_attention_bwd at the same shape is timed
+beside it. The card name, power limit and max SM clock are read in the same run.
 Usage: python tools/profile_attention_probs.py [--reps 50 --rounds 7 --out tool_out/attention_probs.txt]"""
 import argparse
 import os
@@ -85,6 +89,44 @@ def main():
         lines.append(line)
         del qkv, ctx, lse, probs
         torch.cuda.empty_cache()
+    # ---- cb_attention_probs_bwd next to cb_attention_bwd ----
+    head = ["cb_attention_probs_bwd next to cb_attention_bwd, %d heads x 64, dropout 0.1; median of %d rounds of %d calls"
+            % (HEADS, args.rounds, args.reps),
+            "%-5s %-4s %-4s %10s %12s %12s %9s %12s  %s" % ("nseq", "L", "Lt", "G MB", "probs_bwd us", "bound us", "of bound",
+                                                            "attn_bwd us", "configuration")]
+    print("\n".join(head), flush=True)
+    lines += head
+    for nseq, L, lt, what in SHAPES:
+        g = torch.Generator().manual_seed(1)
+        qkv = torch.randn(nseq * L, 3 * 768, generator=g).to(dev, torch.bfloat16)
+        dctx = torch.randn(nseq * L, 768, generator=g).to(dev, torch.bfloat16)
+        mask = torch.ones(nseq, lt, dtype=torch.int64, device=dev)
+        mask[:, lt - lt // 4:] = 0
+        ctx = torch.empty(nseq * L, 768, device=dev, dtype=torch.bfloat16)
+        lse = torch.empty(nseq, HEADS, L, device=dev)
+        dprobs = torch.randn(nseq, HEADS, L, L, device=dev)
+        drow = torch.empty(nseq * HEADS * L, device=dev)
+        dqkv = torch.zeros(nseq * L, 3 * 768, device=dev, dtype=torch.bfloat16)
+        ops.attention_fwd(qkv, mask, ctx, lse, nseq, L, lt, HEADS, 0.1, 7)
+
+        def run_pb():
+            ops.attention_probs_bwd(qkv, mask, lse, dprobs, drow, dqkv, nseq, L, lt, HEADS, 0.1, 7)
+
+        def run_ab():
+            ops.attention_bwd(qkv, mask, ctx, dctx, lse, dqkv, nseq, L, lt, HEADS, 0.1, 7)
+        for _ in range(3):
+            run_pb()
+            run_ab()
+        torch.cuda.synchronize()
+        us_pb = timed(run_pb, args.reps, args.rounds)
+        us_ab = timed(run_ab, args.reps, args.rounds)
+        g_bytes = 4 * nseq * HEADS * L * L
+        bound = (3 * g_bytes + 2 * 2 * 2 * nseq * L * 768) / HBM_BYTES_PER_S * 1e6
+        line = "%-5d %-4d %-4d %10.1f %12.1f %12.1f %9.3f %12.1f  %s" % (nseq, L, lt, g_bytes / 1e6, us_pb, bound, bound / us_pb, us_ab, what)
+        print(line, flush=True)
+        lines.append(line)
+        del qkv, dctx, ctx, lse, dprobs, drow, dqkv
+        torch.cuda.empty_cache()
     # ---- eval bert(...) at 448 px (7 x 7 grid, 20-token captions: L = 69), flags off / on ----
     from oracle.clipbert_ref import BERT_CFG
     nseq, lt = 256, 20
@@ -110,6 +152,29 @@ def main():
         lines.append(line)
         del model
         torch.cuda.empty_cache()
+    # ---- train bert(...) forward + backward at 448 px, differentiable attentions, loss on all 12 layers' attentions or none ----
+    lines.append("train bert(...) forward + backward, %d sequences, L = %d (448 px), dropout 0.1, differentiable_attentions, "
+                 "median of %d rounds of %d steps:" % (nseq, lt + 49, args.rounds, 5))
+    torch.manual_seed(0)
+    cfg = types.SimpleNamespace(**dict(BERT_CFG, output_hidden_states=False, output_attentions=True))
+    model = cb.ClipBertBaseModel(cfg).to(dev).train()
+    model.differentiable_attentions = True
+    w_seq = torch.randn(nseq, lt + 49, 768, generator=g).to(dev)
+    w_attn = torch.randn(nseq, HEADS, lt + 49, lt + 49, generator=g).to(dev)
+    for attn_loss in (False, True):
+        def step():
+            seq, pooled, attn = model(ids, grid, mask)
+            loss = (seq.float() * w_seq).sum()
+            if attn_loss:
+                loss = loss + sum((a * w_attn).sum() for a in attn)
+            loss.backward()
+        for _ in range(3):
+            step()
+        torch.cuda.synchronize()
+        us = timed(step, 5, args.rounds)
+        line = "  loss on the attentions of %-9s %10.1f us" % ("12 layers" if attn_loss else "no layer", us)
+        print(line, flush=True)
+        lines.append(line)
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:
         f.write("\n".join(lines) + "\n")
