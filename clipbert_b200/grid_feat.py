@@ -144,7 +144,7 @@ class GridFeatBackbone(nn.Module):
         self._flat = None
         self._bn = None
         self._dirty = True
-        self._capture = None     # tests set this to a dict to receive per-stage activations
+        self._capture = None     # tests set this to a dict to receive per-stage / per-block activations (and, in backward, gradients)
         self._inject = None      # tests: {"res5.2": NHWC activation} makes that block start from the given tensor
         self._pending_backward = 0
         self._bucket_hook = None   # data-parallel: called as hook(flat_grad, first_finished_element, side_stream) mid-backward
@@ -313,14 +313,16 @@ class GridFeatBackbone(nn.Module):
 
     # ---- zero-bordered buffers --------------------------------------------------------------------
     # Only interior rows of a padded activation are ever written (CB_ROWMAP_PAD epilogues), so a buffer that was
-    # zeroed once keeps a valid zero border for its whole life: recycle instead of re-zeroing every step.
-    def _pad_get(self, rows, ch, device):
-        lst = self._pad_pool.setdefault((rows, ch), [])
-        return lst.pop() if lst else torch.zeros(rows, ch, dtype=torch.bfloat16, device=device)
+    # zeroed once keeps a valid zero border for its whole life: recycle instead of re-zeroing every step. Which rows
+    # are border depends on (n, h, w), not on the row count alone (1 x 6 x 6 and 4 x 2 x 2 both pad to 64 rows), so
+    # the pool is keyed by the full geometry.
+    def _pad_get(self, n, h, w, ch, device):
+        lst = self._pad_pool.setdefault((n, h, w, ch), [])
+        return lst.pop() if lst else torch.zeros(n * (h + 2) * (w + 2), ch, dtype=torch.bfloat16, device=device)
 
-    def _pad_put(self, t):
-        if t is not None:
-            self._pad_pool.setdefault((t.shape[0], t.shape[1]), []).append(t)
+    def _pad_put(self, t, n, h, w):
+        assert t.shape[0] == n * (h + 2) * (w + 2)
+        self._pad_pool.setdefault((n, h, w, t.shape[1]), []).append(t)
 
     # ---- forward ----------------------------------------------------------------------------------
     def forward(self, x):
@@ -400,6 +402,8 @@ class GridFeatBackbone(nn.Module):
                 ops.gemm(**dict(kw, a=s2d, a_ld=ld))
             del s2d
             ops.maxpool3x3s2(c1, cur, n, ho, wo, 64, row_pitch=ws, img_pitch=hs * ws)
+            if self._capture is not None:
+                self._capture["c1"] = c1.view(n, hs, ws, 64)[:, :ho, :wo]     # the pool's view of the s2d output grid
         else:
             # im2col gather (BGR flip + cast fused) -> GEMM over the [pixels, 152] patch matrix
             col = torch.empty(n * ho * wo, STEM_KP, dtype=bf16, device=dev)
@@ -409,6 +413,8 @@ class GridFeatBackbone(nn.Module):
                      b_rows=64, b_ld=STEM_KP, shift=stem._shift, act=ops.ACT_RELU, out=c1, out_ld=64)
             del col
             ops.maxpool3x3s2(c1, cur, n, ho, wo, 64)
+            if self._capture is not None:
+                self._capture["c1"] = c1.view(n, ho, wo, 64)
         del c1
         if self._capture is not None:
             self._capture["stem"] = cur.view(n, hh, ww, 64)
@@ -431,17 +437,20 @@ class GridFeatBackbone(nn.Module):
                     xs = x_in
                 rows = n * hh * ww
                 sc = self._conv1x1(blk.shortcut, xs, rows, ops.ACT_NONE) if blk.has_shortcut else xs
-                a_pad = self._pad_get(n * (hh + 2) * (ww + 2), blk.mid, dev)
+                a_pad = self._pad_get(n, hh, ww, blk.mid, dev)
                 self._conv1x1(blk.conv1, xs, rows, ops.ACT_RELU, rowmap=ops.ROWMAP_PAD, hw=(hh, ww), out=a_pad)
                 b = self._conv3x3(blk.conv2, a_pad, n, hh, ww, ops.ACT_RELU)
                 if last:
-                    y = self._pad_get(n * (hh + 2) * (ww + 2), blk.cout, dev)
+                    y = self._pad_get(n, hh, ww, blk.cout, dev)
                     self._conv1x1(blk.conv3, b, rows, ops.ACT_RELU, residual=sc, rowmap=ops.ROWMAP_PAD, hw=(hh, ww), out=y)
                 else:
                     y = self._conv1x1(blk.conv3, b, rows, ops.ACT_RELU, residual=sc)
+                if self._capture is not None:
+                    # clones of the pooled buffers: the pool hands them to a later call
+                    self._capture["%s.%d" % (name, bi)] = dict(xs=xs, sc=sc, a_pad=a_pad.clone(), b=b, y=y.clone() if last else y)
                 trainable = blk.conv1.weight.requires_grad
                 if not (need_backward and trainable):
-                    self._pad_put(a_pad)            # consumed by conv2 above; stream order makes the reuse safe
+                    self._pad_put(a_pad, n, hh, ww)     # consumed by conv2 above; stream order makes the reuse safe
                 if need_backward and trainable:
                     blocks.append(dict(name="%s.%d" % (name, bi), blk=blk, x_in=x_in, xs=xs, a_pad=a_pad, b=b, y=y, h=hh, w=ww, h_in=h_in, w_in=w_in,
                                        first_trainable=not blocks))
@@ -454,9 +463,11 @@ class GridFeatBackbone(nn.Module):
         gh, gw = hh // 2, ww // 2
         grid = torch.empty(bsz, n_frms, gh, gw, ge.cout, dtype=bf16, device=dev)
         ops.maxpool2x2_relu_fwd(gconv, grid, n, hh, ww, ge.cout)
+        if self._capture is not None:
+            self._capture["gconv"] = gconv
         stash = None
         if not need_backward:
-            self._pad_put(cur)                      # res5 output (padded), consumed by the grid_encoder conv
+            self._pad_put(cur, n, hh, ww)           # res5 output (padded), consumed by the grid_encoder conv
         if need_backward:
             stash = dict(n=n, h=hh, w=ww, res5_pad=cur, gconv=gconv, blocks=blocks)
             if self._capture is not None:
@@ -508,11 +519,14 @@ class GridFeatBackbone(nn.Module):
         # wgrad GEMMs run on the side queue beside the dgrad chain; zero-bordered buffers they read go back to the pool
         # only after the join at the end (a recycled buffer would be overwritten by a later main-stream launch)
         sq = ops.SideQueue()
-        recycle = []
+        recycle = []          # (zero-bordered buffer, n, h, w)
+        cap = None if self._capture is None else self._capture.setdefault("bwd", {})
         dg_pad = torch.empty(p, ge.cout, dtype=bf16, device=dev)
         ops.maxpool2x2_relu_bwd(dgrid, stash["gconv"], dg_pad, n, h, w, ge.cout)
         res5_pad = stash["res5_pad"]
-        recycle.append(res5_pad)
+        recycle.append((res5_pad, n, h, w))
+        if cap is not None:
+            cap["grid_encoder"] = dict(dg_pad=dg_pad)
         if ge.weight.requires_grad:
             sq.run(lambda: self._wgrad(ge, dg_pad, res5_pad, p, ntaps=9, tap_w=w + 2), dg_pad, res5_pad)
         blocks = stash["blocks"]
@@ -526,11 +540,13 @@ class GridFeatBackbone(nn.Module):
             pp = n * (hh + 2) * (ww + 2)
             # the block's three / four weight gradients as ONE grouped launch on the side queue, issued when its last dY (da) exists
             wg = [self._wgrad_kw(blk.conv3, g, st["b"], rows)]
-            db_pad = self._pad_get(pp, blk.mid, dev)
-            recycle += [db_pad, st["a_pad"]]
+            db_pad = self._pad_get(n, hh, ww, blk.mid, dev)
+            recycle += [(db_pad, n, hh, ww), (st["a_pad"], n, hh, ww)]
             self._dgrad1x1(blk.conv3, g, rows, aux=st["b"], rowmap=ops.ROWMAP_PAD, hw=(hh, ww), out=db_pad)
             wg.append(self._wgrad_kw(blk.conv2, db_pad, st["a_pad"], pp, ntaps=9, tap_w=ww + 2))
             da = self._dgrad3x3(blk.conv2, db_pad, n, hh, ww, st["a_pad"])
+            if cap is not None:
+                cap[st["name"]] = c = dict(g=g, db_pad=db_pad.clone(), da=da)
             wg.append(self._wgrad_kw(blk.conv1, da, st["xs"], rows))
             if blk.has_shortcut:
                 wg.append(self._wgrad_kw(blk.shortcut, g, st["xs"], rows))
@@ -545,19 +561,23 @@ class GridFeatBackbone(nn.Module):
                     self._bucket_hook(self._flat.grad, blk.shortcut._e["offset"], sq.side if sq.forked else None)
                 if st["first_trainable"]:
                     break                                     # d2 FREEZE_AT: no gradient below this block
-                dxs = self._dgrad1x1(blk.shortcut, g, rows)
-                dxs = self._dgrad1x1(blk.conv1, da, rows, residual=dxs)
+                dxs_sc = self._dgrad1x1(blk.shortcut, g, rows)
+                dxs = self._dgrad1x1(blk.conv1, da, rows, residual=dxs_sc)
                 g = torch.empty(n * st["h_in"] * st["w_in"], blk.cin, dtype=bf16, device=dev)
                 if blk.stride == 2:
                     ops.unsubsample2_mask(dxs, st["x_in"], g, n, st["h_in"], st["w_in"], blk.cin)
                 else:
                     ops.relu_mask(dxs, st["x_in"], g)
+                if cap is not None:
+                    c.update(dxs_sc=dxs_sc, dxs=dxs, gin=g)
             else:
                 if st["first_trainable"]:
                     break
                 g = self._dgrad1x1(blk.conv1, da, rows, residual=g, aux=st["x_in"])
+                if cap is not None:
+                    c.update(gin=g)
         sq.join()
-        for t in recycle:
-            self._pad_put(t)
+        for t, tn, th, tw in recycle:
+            self._pad_put(t, tn, th, tw)
         if not self._optimizer_emits_packed:
             self._dirty = True   # an optimizer step normally follows: repack bf16 operands on the next forward
