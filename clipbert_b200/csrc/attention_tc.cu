@@ -762,6 +762,36 @@ __global__ void __launch_bounds__(TC_THREADS) attn_tc_bwd_q_kernel(const __nv_bf
 // segment go out as scalar stores. Streaming stores (st.global.cs): P is written once and read by the host, not by a kernel.
 constexpr int PR_LD = 72;                 // fp32 elements per staged row: 64 keys + up to 3 of shift, 16-byte aligned rows
 
+// Writes the staged rows r < nq of one key tile (Ps row r: keys k0 .. k0 + nk - 1, shifted by the element index & 3 of its first
+// key) to out viewed as [rows, L], row prow0 + r. 16 threads per row, 8 rows per pass; rows >= nq and keys >= nk are never
+// written. ACC: each element becomes (its value in memory) + (the staged value), one fp32 add, the read through the same
+// aligned vectors.
+template <bool ACC>
+__device__ __forceinline__ void tc_store_staged_rows(const float* Ps, float* __restrict__ out, uint64_t prow0, int L, int k0, int nq, int nk) {
+  for (int r = threadIdx.x >> 4; r < nq; r += TC_THREADS / 16) {
+    const uint64_t e = (prow0 + r) * L + k0;
+    const int sh = static_cast<int>(e & 3), end = sh + nk;
+    float* dst = out + (e - sh);       // 16-byte aligned
+    const float* src = Ps + r * PR_LD;
+    for (int c = (threadIdx.x & 15) * 4; c < end; c += 64) {
+      const float4 v = *reinterpret_cast<const float4*>(src + c);
+      if (c >= sh && c + 4 <= end) {
+        if (ACC) {
+          const float4 o = __ldcs(reinterpret_cast<const float4*>(dst + c));
+          __stcs(reinterpret_cast<float4*>(dst + c), make_float4(o.x + v.x, o.y + v.y, o.z + v.z, o.w + v.w));
+        } else {
+          __stcs(reinterpret_cast<float4*>(dst + c), v);
+        }
+      } else {
+        const float w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (c + i >= sh && c + i < end) __stcs(dst + c + i, ACC ? __ldcs(dst + c + i) + w[i] : w[i]);
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                                                    int64_t ld_qkv, const int64_t* __restrict__ text_mask,
                                                                    const float* __restrict__ lse, float* __restrict__ probs, int L, int Lt,
@@ -816,24 +846,56 @@ __global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_kernel(const __nv_bf
       }
     }
     __syncthreads();
-    // 16 threads per row, 8 rows per pass; rows >= nq and keys >= nk are never written
-    for (int r = threadIdx.x >> 4; r < nq; r += TC_THREADS / 16) {
-      const uint64_t e = (prow0 + r) * L + k0;
-      const int sh = static_cast<int>(e & 3), end = sh + nk;
-      float* dst = probs + (e - sh);     // 16-byte aligned
-      const float* src = Ps + r * PR_LD;
-      for (int c = (threadIdx.x & 15) * 4; c < end; c += 64) {
-        const float4 v = *reinterpret_cast<const float4*>(src + c);
-        if (c >= sh && c + 4 <= end) {
-          __stcs(reinterpret_cast<float4*>(dst + c), v);
-        } else {
-          const float w[4] = {v.x, v.y, v.z, v.w};
+    tc_store_staged_rows<false>(Ps, probs, prow0, L, k0, nq, nk);
+  }
+}
+
+// The gradient the returned probabilities A receive from the context product ctx = A V (transformers.py:271-277):
+// dA[s, h, i, j] = sum_d dO[s l + i, h 64 + d] V[s l + j, h 64 + d], for every i, j < l (padded keys, padded query rows and
+// dropped positions included; A is post-dropout, so no dropout factor). One CTA = 64 query rows of one (sequence, head): the dO
+// tile stays in shared memory, each 64-key V tile is loaded in turn, dO V^T is the Q K^T product shape of attn_tc_probs_kernel
+// on mma.sync, and the tile leaves through the same staging and 16-byte streaming stores. ACC: added to the values in memory,
+// one fp32 add per element; every element has one writer and a fixed order, so runs are bit-identical.
+template <bool ACC>
+__global__ void __launch_bounds__(TC_THREADS) attn_tc_dprobs_kernel(const __nv_bfloat16* __restrict__ v, int64_t ld_qkv,
+                                                                    const __nv_bfloat16* __restrict__ dctx, int64_t ld_ctx,
+                                                                    float* __restrict__ dprobs, int L, int H) {
+  pdl_wait();
+  pdl_trigger();
+  extern __shared__ __align__(16) uint8_t tc_smem[];
+  __nv_bfloat16* dOs = reinterpret_cast<__nv_bfloat16*>(tc_smem);
+  __nv_bfloat16* Vs = dOs + TC_TILE;
+  float* Ps = reinterpret_cast<float*>(Vs + TC_TILE);       // [64][PR_LD] staged dA of one key tile
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = qb * 64;
+  const int nq = min(64, L - q0);
+  const int64_t row0 = static_cast<int64_t>(b) * L;
+  const uint64_t prow0 = (static_cast<uint64_t>(b) * H + h) * L + q0;   // row index of query q0 in dprobs viewed as [nseq*H*L, L]
+  const bool live = warp < tc_live_slabs(nq);
+  tc_load_tile(dOs, dctx + (row0 + q0) * ld_ctx + h * 64, ld_ctx, nq);
+  const int r0 = warp * 16;
+  const int rq = r0 + (lane >> 2), cq = 2 * (lane & 3);
+  const int nkb = (L + 63) / 64;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int k0 = kb * 64, nk = min(64, L - k0);
+    __syncthreads();                     // the previous tile has been written out: Vs and Ps are free
+    tc_load_tile(Vs, v + (row0 + k0) * ld_qkv + h * 64, ld_qkv, nk);
+    __syncthreads();
+    if (live) {
+      float s[8][4];
+      tc_mm_abt_live(s, dOs, Vs, r0, lane, tc_live_slabs(nk));
+      const uint64_t e0 = (prow0 + rq) * L + k0, e1 = e0 + static_cast<uint64_t>(8) * L;
+      float* d0 = Ps + rq * PR_LD + static_cast<int>(e0 & 3) + cq;
+      float* d1 = Ps + (rq + 8) * PR_LD + static_cast<int>(e1 & 3) + cq;
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
-            if (c + i >= sh && c + i < end) __stcs(dst + c + i, w[i]);
-        }
+      for (int j = 0; j < 8; ++j) {
+        d0[j * 8] = s[j][0]; d0[j * 8 + 1] = s[j][1];
+        d1[j * 8] = s[j][2]; d1[j * 8 + 1] = s[j][3];
       }
     }
+    __syncthreads();
+    tc_store_staged_rows<ACC>(Ps, dprobs, prow0, L, k0, nq, nk);
   }
 }
 
@@ -1205,4 +1267,29 @@ extern "C" int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int
   launch_k(attn_tc_probs_bwd_k_kernel, grid, TC_THREADS, smem_k, st, base, base + hid, ld_qkv, text_mask, lse, dprobs,
            static_cast<const float*>(drow), dbase + hid, ld_dqkv, l, lt, heads, 0.125f, dc);
   return check_launch("cb_attention_probs_bwd(k)");
+}
+
+extern "C" int cb_attention_dprobs(const void* qkv, int64_t ld_qkv, const void* dctx, int64_t ld_ctx, float* dprobs, int accumulate,
+                                   int nseq, int l, int heads, int head_dim, void* stream) {
+  using namespace cb;
+  CB_REQUIRE(head_dim == 64, "cb_attention_dprobs: head_dim %d unsupported (built for 64)", head_dim);
+  CB_REQUIRE(qkv && dctx && dprobs && (accumulate == 0 || accumulate == 1) && nseq > 0 && l > 0 && heads > 0 && nseq <= 65535 &&
+                 heads <= 65535,
+             "cb_attention_dprobs: bad arguments");
+  CB_REQUIRE(ld_qkv % 8 == 0 && ld_ctx % 8 == 0 && ld_qkv >= 3 * static_cast<int64_t>(heads) * 64 &&
+                 ld_ctx >= static_cast<int64_t>(heads) * 64,
+             "cb_attention_dprobs: row pitches must be multiples of 8 and hold Q | K | V and the merged heads");
+  CB_REQUIRE(reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(dctx) % 16 == 0 &&
+                 reinterpret_cast<uintptr_t>(dprobs) % 16 == 0,
+             "cb_attention_dprobs: qkv, dctx and dprobs must be 16-byte aligned");
+  const int smem = 2 * TC_TILE * 2 + 64 * PR_LD * 4;             // dO, V tiles (bf16) + staged dA (fp32): 36 KB
+  const __nv_bfloat16* v = static_cast<const __nv_bfloat16*>(qkv) + 2 * heads * 64;
+  const __nv_bfloat16* d = static_cast<const __nv_bfloat16*>(dctx);
+  const dim3 grid(ceil_div(l, 64), heads, nseq);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (accumulate)
+    launch_k(attn_tc_dprobs_kernel<true>, grid, TC_THREADS, smem, st, v, ld_qkv, d, ld_ctx, dprobs, l, heads);
+  else
+    launch_k(attn_tc_dprobs_kernel<false>, grid, TC_THREADS, smem, st, v, ld_qkv, d, ld_ctx, dprobs, l, heads);
+  return check_launch("cb_attention_dprobs");
 }

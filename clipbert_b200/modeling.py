@@ -18,6 +18,8 @@ is the hand-written sm_90a kernels behind libclipbert_sm90.so:
                  cb_gemm WGRAD accumulating fp32 into the flat gradient buffer, activation
                  derivatives and dropout masks fused into the dgrad / LayerNorm-backward epilogues.
 """
+import weakref
+
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -137,9 +139,17 @@ class ClipBertBaseModel(nn.Module):
     distillation of a teacher's maps, entropy penalties) then trains every parameter below that layer and ``visual_inputs``,
     through cb_attention_probs_bwd (include/clipbert_b200.h). A pass whose loss does not use the attentions costs and
     computes exactly what it does with the switch off. With the default the attentions are returned non-differentiable.
-    Unsupported either way: the gradient of a score WITH RESPECT TO the returned maps (``torch.autograd.grad(score, attn)``,
-    hooks on them), which in the reference also carries dO V^T from the context product; here the context is made from the
-    kernel's own probabilities, not from the returned tensor.
+
+    ``t.retain_grad()`` on a returned tensor gives, after ``backward()``, the ``.grad`` the reference's tensor holds (the HF
+    idiom of gradient-based attribution: attention x gradient relevance, Grad-SAM, gradient x input on the hidden states):
+    ``attentions[l].grad`` (switch on) is the loss's direct term plus dO V^T per head, the term from the context product
+    (cb_attention_dprobs: dO = d loss / d context of layer l, V its bf16 value block; at every position, dropped ones
+    included); ``hidden_states[k].grad`` is the full gradient at the input of layer k, and ``sequence_output.grad`` (the
+    same tensor as hidden_states[12] in the reference) the full top gradient, pooler path included; ``pooled_output.grad``
+    is its direct term, which is its full gradient. A pass with nothing retained issues the same launches as without.
+    Unsupported: ``torch.autograd.grad(score, attentions)`` (or hidden states), and tensor hooks on the maps or hidden
+    states. The whole pass is one autograd node, and a tensor's hooks fire before that node runs, so they see only the
+    loss's direct term; ``.grad`` of a retained tensor is completed inside the node.
     """
 
     differentiable_attentions = False
@@ -227,16 +237,39 @@ class _BaseModelFn(torch.autograd.Function):
         if not flags[2]:                        # ClipBertBaseModel.differentiable_attentions
             ctx.mark_non_differentiable(*attn)
         ctx.set_materialize_grads(False)        # unused outputs arrive as None and cost nothing in the backward
-        return (seq, pooled) + tuple(hidden) + tuple(attn)
+        outs = (seq, pooled) + tuple(hidden) + tuple(attn)
+        # weak: the node holding its own outputs would form a cycle (the outputs hold the node as grad_fn)
+        ctx.outputs = [weakref.ref(t) for t in outs]
+        return outs
 
     @staticmethod
     def backward(ctx, dseq, dpooled, *rest):
         stash, ctx.stash = ctx.stash, None
         m = ctx.module
         stash["base_grads"] = (dseq, dpooled, rest[:ctx.n_hidden], rest[ctx.n_hidden:])
+        stash["retained"] = _BaseModelFn._retained(ctx, len(stash["layers"]))
         dgrid = m._backward_impl(stash, None, ctx.grid_needs_grad)
         m._backward_done()
         return None, dgrid, None, None, None, None
+
+    @staticmethod
+    def _retained(ctx, n_layers):
+        """The outputs the caller called retain_grad() on, or None when there are none: ([tensors whose .grad is the gradient at
+        the input of layer k, k = 0 .. n_layers (n_layers: the top, where sequence_output is hidden_states[n_layers])],
+        [attentions[i] or None]). torch's retain hooks run before this node's backward, so each .grad holds the loss's direct
+        term on that output, if any, when the engine reads it."""
+        outs = [r() for r in ctx.outputs]
+        outs = [t if t is not None and t.retains_grad else None for t in outs]
+        if all(t is None for t in outs):
+            return None
+        hidden, attn = outs[2:2 + ctx.n_hidden], outs[2 + ctx.n_hidden:]
+        at_input = [[] for _ in range(n_layers + 1)]
+        for k, t in enumerate(hidden):
+            if t is not None:
+                at_input[k].append(t)
+        if outs[0] is not None:
+            at_input[n_layers].append(outs[0])
+        return at_input, (attn if any(t is not None for t in attn) else None)
 
 
 class _ClipBertHeadModel(nn.Module):
@@ -661,6 +694,7 @@ class _ClipBertHeadModel(nn.Module):
         sq = ops.SideQueue()                               # wgrad GEMMs / bias sums run beside the dgrad chain
         base = st.get("base_grads")                        # ClipBertBaseModel.forward: (d sequence, d pooled, d hidden states)
         dhidden = dattn = None
+        ret_hidden, ret_attn = st.get("retained") or (None, None)   # outputs of ClipBertBaseModel.forward with retain_grad()
         if base is None:
             dpre = self._head_backward(st, dout, nseq, H)  # grad w.r.t. pooler pre-activation
         else:
@@ -679,6 +713,8 @@ class _ClipBertHeadModel(nn.Module):
         for i in reversed(range(len(st["layers"]))):
             if dhidden is not None and dhidden[i + 1] is not None:     # output of layer i = hidden_states[i + 1]
                 dx += dhidden[i + 1]
+            if ret_hidden is not None:
+                _set_retained_hidden_grad(ret_hidden[i + 1], dx, nseq, L, H)
             ly = st["layers"][i]
             ls = ly["seed"]
             qkv_l, ao_l, in_l, out_l = (self._lin["l%d.%s" % (i, k)] for k in ("qkv", "ao", "inter", "out"))
@@ -722,6 +758,8 @@ class _ClipBertHeadModel(nn.Module):
             if dattn is not None and dattn[i] is not None:      # a loss on attentions[i]: its dQ / dK added into dqkv
                 drow = new(nseq, heads, L, dtype=f32)
                 ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn[i], drow, dqkv, nseq, L, lt, heads, p_a, ls + 1)
+            if ret_attn is not None and ret_attn[i] is not None:
+                _add_retained_attention_grad(ret_attn[i], ly["qkv"], dctx, nseq, L, heads)
             wg.append(self._wgrad_kw(qkv_l, dqkv, ly["x"], M))
             if group:
                 sq.run(lambda: (ops.gemm_wgrad_group(wg), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dd, ly["gel"], du, ly["a"], dd1, ly["ctx"], dqkv, ly["x"])
@@ -733,6 +771,8 @@ class _ClipBertHeadModel(nn.Module):
             st["layers"][i] = None     # free this layer's stash
         if dhidden is not None and dhidden[0] is not None:                 # hidden_states[0] = the embedding output
             dx += dhidden[0]
+        if ret_hidden is not None:
+            _set_retained_hidden_grad(ret_hidden[0], dx, nseq, L, H)
         # ---- embeddings ----
         g_t, _, dg_t, db_t = self._ln("emb.ln")
         g_v, _, dg_v, db_v = self._ln("vis.ln")
@@ -792,6 +832,28 @@ class _ClipBertHeadModel(nn.Module):
             self._flat.zero_grad()
         else:
             super().zero_grad(set_to_none=set_to_none)
+
+
+def _set_retained_hidden_grad(tensors, dx, nseq, L, H):
+    """.grad of a retained hidden state (or sequence_output) = dx, the full gradient at that layer boundary: it already holds
+    the direct term the retain hook put in .grad, and the backward writes dx no more after this point, so it is not copied."""
+    for t in tensors:
+        t.grad = dx.view(nseq, L, H)
+
+
+def _add_retained_attention_grad(t, qkv, dctx, nseq, L, heads):
+    """attentions[i].grad (+)= dO V^T, the term the returned map receives from the context product, by cb_attention_dprobs:
+    added in place to the direct term the retain hook left in .grad, or written into a fresh tensor when there is none (or
+    when .grad is not a contiguous, 16-byte aligned tensor, which is then copied first)."""
+    g = t.grad
+    if g is not None and g.is_contiguous() and g.data_ptr() % 16 == 0:
+        ops.attention_dprobs(qkv, dctx, g, True, nseq, L, heads)
+        return
+    out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
+    if g is not None:
+        out.copy_(g)
+    ops.attention_dprobs(qkv, dctx, out, g is not None, nseq, L, heads)
+    t.grad = out
 
 
 class _BaseModelEngine(_ClipBertHeadModel):

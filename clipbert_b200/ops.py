@@ -41,6 +41,7 @@ _SIGS = {
     "cb_attention_bwd": [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_attention_probs": [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_attention_probs_bwd": [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
+    "cb_attention_dprobs": [_vp, _i64, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp],
     "cb_stem_im2col": [_vp, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp],
     "cb_maxpool3x3s2": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool3x3s2_strided": [_vp, _vp, _i, _i, _i, _i, _i64, _i64, _vp],
@@ -610,6 +611,14 @@ def attention_probs_bwd(qkv, text_mask, lse, dprobs, drow, dqkv, nseq, l, lt, he
     assert drow.dtype == torch.float32 and drow.numel() >= nseq * heads * l
     _call("cb_attention_probs_bwd", _p(qkv), qkv.shape[1], _p(text_mask), _p(lse), _p(dprobs), _p(drow), _p(dqkv), dqkv.shape[1],
           nseq, l, lt, heads, 64, p, seed, _s())
+
+
+def attention_dprobs(qkv, dctx, dprobs, accumulate, nseq, l, heads):
+    """dprobs (fp32 [nseq, heads, l, l] contiguous) = (dprobs if accumulate else 0) + dO V^T per head: the gradient the returned
+    attention probabilities receive from the context product, with dctx = d loss / d context and V from qkv."""
+    assert dprobs.dtype == torch.float32 and dprobs.is_contiguous() and dprobs.numel() == nseq * heads * l * l
+    _call("cb_attention_dprobs", _p(qkv), qkv.shape[1], _p(dctx), dctx.shape[1], _p(dprobs), int(bool(accumulate)), nseq, l, heads,
+          64, _s())
 
 
 # ------------------------------------------------------------------------------------------------

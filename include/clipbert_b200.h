@@ -330,6 +330,19 @@ int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t* text_mask
 int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const float* dprobs,
                            float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
                            float dropout_p, uint64_t seed, void* stream);
+/* The gradient the returned probabilities A receive from the context product ctx = A V (transformers.py:271-277), for
+ * retain_grad() on the attentions: dctx [nseq * l, >= heads * 64] bf16 with row pitch ld_ctx (d loss / d context), V the third
+ * column block of qkv;
+ *   dprobs[s, h, i, j] = (accumulate ? dprobs[s, h, i, j] : 0) + sum_d dctx[s l + i, h 64 + d] V[s l + j, h 64 + d]
+ * for every i, j < l: padded text keys, padded query rows and dropped positions get their value too (A is post-dropout, so
+ * there is no dropout factor; no mask, lse or seed is read). dprobs fp32 [nseq, heads, l, l], contiguous, 16-byte aligned at
+ * its base (a row starts at any 4-byte alignment); rows and columns beyond l are never written. Tensor cores (mma.sync, bf16
+ * in, fp32 accumulation), one CTA per (64-query tile, head, sequence); accumulate = 1 reads each element and adds in fp32,
+ * once. Every element has one writer: no atomics, bit-identical from run to run. Arguments are checked as for
+ * cb_attention_probs (accumulate 0 or 1; pitches multiples of 8 holding Q | K | V and heads x 64; qkv, dctx, dprobs 16-byte
+ * aligned); nothing is launched otherwise. */
+int cb_attention_dprobs(const void* qkv, int64_t ld_qkv, const void* dctx, int64_t ld_ctx, float* dprobs, int accumulate,
+                        int nseq, int l, int heads, int head_dim, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Small helpers on the transformer side.

@@ -1,13 +1,14 @@
-"""cb_attention_probs (the attention probabilities behind ClipBertBaseModel's output_attentions) and cb_attention_probs_bwd (the
-backward through them, ClipBertBaseModel.differentiable_attentions) timed with CUDA events, an eval bert(...) forward at 448 px with
-output_hidden_states / output_attentions off and on, and a train-mode bert(...) forward + backward at 448 px with a loss on the
-attentions of all 12 layers and with none.
+"""cb_attention_probs (the attention probabilities behind ClipBertBaseModel's output_attentions), cb_attention_probs_bwd (the
+backward through them, ClipBertBaseModel.differentiable_attentions) and cb_attention_dprobs (the maps' own gradient dO V^T, for
+retain_grad() on them) timed with CUDA events, an eval bert(...) forward at 448 px with output_hidden_states / output_attentions off
+and on, a train-mode bert(...) forward + backward at 448 px with a loss on the attentions of all 12 layers and with none, and an
+eval bert(...) forward + backward at 448 px with all 12 maps and 13 hidden states retained and with none.
 
 Per shape: median over `--rounds` rounds of `--reps` back-to-back calls, and the kernel's fraction of its lower bound = compulsory
 bytes / 3.35 TB/s (the H100 SXM data-sheet HBM3 bandwidth, for a card allowed 700 W) over the measured time. Compulsory bytes:
 cb_attention_probs: P written + Q and K read once; cb_attention_probs_bwd: G read three times (12 l^2 bytes per (sequence, head):
-the D pass, the dQ pass and the dK kernel) + the bf16 dQ and dK read and written. cb_attention_bwd at the same shape is timed
-beside it. The card name, power limit and max SM clock are read in the same run.
+the D pass, the dQ pass and the dK kernel) + the bf16 dQ and dK read and written; cb_attention_dprobs: the map written (and read
+when accumulating) + dO and V read once. cb_attention_bwd at the same shape is timed beside cb_attention_probs_bwd. The card name, power limit and max SM clock are read in the same run.
 Usage: python tools/profile_attention_probs.py [--reps 50 --rounds 7 --out tool_out/attention_probs.txt]"""
 import argparse
 import os
@@ -127,6 +128,31 @@ def main():
         lines.append(line)
         del qkv, dctx, ctx, lse, dprobs, drow, dqkv
         torch.cuda.empty_cache()
+    # ---- cb_attention_dprobs, fresh and accumulating ----
+    head = ["cb_attention_dprobs, %d heads x 64; median of %d rounds of %d calls" % (HEADS, args.rounds, args.reps),
+            "%-5s %-4s %-10s %10s %10s %12s %9s  %s" % ("nseq", "L", "accumulate", "map MB", "time us", "bound us", "of bound",
+                                                        "configuration")]
+    print("\n".join(head), flush=True)
+    lines += head
+    for nseq, L, lt, what in SHAPES:
+        g = torch.Generator().manual_seed(1)
+        qkv = torch.randn(nseq * L, 3 * 768, generator=g).to(dev, torch.bfloat16)
+        dctx = torch.randn(nseq * L, 768, generator=g).to(dev, torch.bfloat16)
+        dprobs = torch.randn(nseq, HEADS, L, L, device=dev)
+        for acc in (0, 1):
+            def run():
+                ops.attention_dprobs(qkv, dctx, dprobs, acc, nseq, L, HEADS)
+            for _ in range(3):
+                run()
+            torch.cuda.synchronize()
+            us = timed(run, args.reps, args.rounds)
+            p_bytes = 4 * nseq * HEADS * L * L
+            bound = ((1 + acc) * p_bytes + 2 * 2 * nseq * L * 768) / HBM_BYTES_PER_S * 1e6
+            line = "%-5d %-4d %-10d %10.1f %10.1f %12.1f %9.3f  %s" % (nseq, L, acc, p_bytes / 1e6, us, bound, bound / us, what)
+            print(line, flush=True)
+            lines.append(line)
+        del qkv, dctx, dprobs
+        torch.cuda.empty_cache()
     # ---- eval bert(...) at 448 px (7 x 7 grid, 20-token captions: L = 69), flags off / on ----
     from oracle.clipbert_ref import BERT_CFG
     nseq, lt = 256, 20
@@ -173,6 +199,30 @@ def main():
         torch.cuda.synchronize()
         us = timed(step, 5, args.rounds)
         line = "  loss on the attentions of %-9s %10.1f us" % ("12 layers" if attn_loss else "no layer", us)
+        print(line, flush=True)
+        lines.append(line)
+    del model
+    torch.cuda.empty_cache()
+    # ---- eval bert(...) forward + backward at 448 px, score on pooled, every map and hidden state retained or none ----
+    lines.append("eval bert(...) forward + backward, %d sequences, L = %d (448 px), both flags and differentiable_attentions on, "
+                 "score on pooled_output, median of %d rounds of %d steps:" % (nseq, lt + 49, args.rounds, 5))
+    torch.manual_seed(0)
+    cfg = types.SimpleNamespace(**dict(BERT_CFG, output_hidden_states=True, output_attentions=True))
+    model = cb.ClipBertBaseModel(cfg).to(dev).eval()
+    model.differentiable_attentions = True
+    w_pool = torch.randn(nseq, 768, generator=g).to(dev)
+    for retain in (False, True):
+        def step():
+            seq, pooled, hidden, attn = model(ids, grid, mask)
+            if retain:
+                for t in tuple(hidden) + tuple(attn):
+                    t.retain_grad()
+            (pooled.float() * w_pool).sum().backward()
+        for _ in range(3):
+            step()
+        torch.cuda.synchronize()
+        us = timed(step, 5, args.rounds)
+        line = "  retained: %-32s %10.1f us" % ("12 maps + 13 hidden states" if retain else "none", us)
         print(line, flush=True)
         lines.append(line)
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
