@@ -184,6 +184,157 @@ __global__ void maxpool3x3s2_kernel(const __nv_bfloat16* __restrict__ x, __nv_bf
   *reinterpret_cast<uint4*>(y + pix * C + c8 * 8) = pack8(m);
 }
 
+// Backward of the 3x3 stride-2 pad-1 max pool above fused with the stem's ReLU' (BasicStem relu_ -> max_pool2d(3, 2, 1)), in
+// gather form: every input element visits the <= 4 windows that contain it, recomputes each window's arg-max with the forward's
+// rule (pool_takes: first maximum in window order, last NaN; an all -inf window picks its first pixel, as ATen), sums in fp32 the
+// window gradients that pick it (oy, then ox ascending), rounds once and applies ReLU' = (x > 0). One writer per element.
+// x: the pool input on its (row_pitch, img_pitch) grid; dy: compact [N, Ho, Wo, C]; dx: compact [N, H, W, C].
+__global__ void maxpool3x3s2_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                                        __nv_bfloat16* __restrict__ dx, int N, int H, int W, int C, int Ho, int Wo, int64_t row_pitch,
+                                        int64_t img_pitch) {
+  pdl_wait();
+  pdl_trigger();
+  const int c8n = C / 8;
+  const int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= static_cast<int64_t>(N) * H * W * c8n) return;
+  const int c8 = static_cast<int>(t % c8n);
+  const int64_t pix = t / c8n;
+  const int xx = static_cast<int>(pix % W), yy = static_cast<int>((pix / W) % H);
+  const int n = static_cast<int>(pix / (static_cast<int64_t>(W) * H));
+  const __nv_bfloat16* xn = x + static_cast<int64_t>(n) * img_pitch * C + c8 * 8;
+  float acc[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+  // windows (oy, ox) with 2 oy - 1 <= yy <= 2 oy + 1
+  const int oy0 = yy / 2, oy1 = min((yy + 1) / 2, Ho - 1);
+  const int ox0 = xx / 2, ox1 = min((xx + 1) / 2, Wo - 1);
+  for (int oy = oy0; oy <= oy1; ++oy)
+    for (int ox = ox0; ox <= ox1; ++ox) {
+      float best[8];
+      int arg[8];
+      const int ry0 = max(2 * oy - 1, 0), rx0 = max(2 * ox - 1, 0);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { best[j] = -INFINITY; arg[j] = ry0 * W + rx0; }
+      for (int iy = ry0; iy <= min(2 * oy + 1, H - 1); ++iy)
+        for (int ix = rx0; ix <= min(2 * ox + 1, W - 1); ++ix) {
+          float f[8];
+          unpack8(*reinterpret_cast<const uint4*>(xn + (iy * row_pitch + ix) * C), f);
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (pool_takes(f[j], best[j])) { best[j] = f[j]; arg[j] = iy * W + ix; }
+        }
+      float g[8];
+      unpack8(*reinterpret_cast<const uint4*>(dy + ((static_cast<int64_t>(n) * Ho + oy) * Wo + ox) * C + c8 * 8), g);
+      const int me = yy * W + xx;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (arg[j] == me) acc[j] += g[j];
+    }
+  float a[8];
+  unpack8(*reinterpret_cast<const uint4*>(xn + (yy * row_pitch + xx) * C), a);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = a[j] > 0.f ? acc[j] : 0.f;
+  *reinterpret_cast<uint4*>(dx + pix * C + c8 * 8) = pack8(acc);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Stem input gradient (BasicStem conv1 7x7/s2/p3 of grid_feat.py:92-95, backward to the frames): the transposed convolution
+//   dX_bgr[n, c, y, x] = sum_{k, r, s} dc1[n, (y+3-r)/2, (x+3-s)/2, k] * W'[k, (r*7 + s)*3 + c]
+// over the taps where both halves are integers inside the conv output, written as fp32 NCHW in RGB order (plane 2 - c).
+// Output pixel x = 2i + px takes the taps s = px^1, px^1 + 2, ... at dc1 column ox = i + o, o = (px + 3 - s) / 2 in {-1, 0, 1, 2}
+// (px = 0: s = 5, 3, 1; px = 1: s = 6, 4, 2, 0), rows alike. So for one output row y, one 16-pixel tile of i and one kernel row r,
+// the four dc1 tiles at column offsets o = -1 .. 2 each feed one m16n8k16 product per 16-channel k-step for both phases
+// (o = 2 only px = 1): A = 16 dc1 pixels x 16 channels, B = 16 channels x 8 (BGR + 5 zero columns), fp32 accumulators D0 / D1
+// for px = 0 / 1. A comes straight from global memory (L1 / L2: neighbouring warps read the same dc1 rows) with the k index
+// permuted so that lane (g, t) reads channels 16t .. 16t+15 of its two rows as two 16-byte loads: mma k = 2t, 2t+1, 2t+8, 2t+9 of
+// k-step q are channels 16t + 4q + 0, 1, 2, 3 (the contraction is order-free in k; B uses the same permutation). B fragments of
+// all 49 taps live in shared memory (18.8 KB). Every output element has one writer and a fixed summation order (r, o, q).
+// One warp per (frame, output row, 16-pixel tile), eight warps per CTA; CTAs stride over the tiles.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+constexpr int kStemDgradWarps = 8;
+constexpr int kStemTaps = 49;
+
+__global__ void __launch_bounds__(kStemDgradWarps * 32) stem_dgrad_kernel(const __nv_bfloat16* __restrict__ dc1,
+                                                                          const __nv_bfloat16* __restrict__ w, int w_ld,
+                                                                          float* __restrict__ dx, int N, int H, int W, int Ho, int Wo,
+                                                                          int tiles) {
+  // B fragments: wf[((tap * 4 + q) * 4 + t) * 3 + g] = {W'[16t+4q+0][tap*3+g], W'[+1]}, {W'[+2], W'[+3]} (bf16 pairs, low = lower k)
+  __shared__ uint2 wf[kStemTaps * 4 * 4 * 3];
+  pdl_wait();
+  pdl_trigger();
+  for (int i = threadIdx.x; i < kStemTaps * 4 * 4 * 3; i += blockDim.x) {
+    const int g = i % 3, t = (i / 3) % 4, q = (i / 12) % 4, tap = i / 48;
+    const int ch = 16 * t + 4 * q, col = tap * 3 + g;
+    __nv_bfloat162 p0, p1;
+    p0.x = w[(ch + 0) * w_ld + col]; p0.y = w[(ch + 1) * w_ld + col];
+    p1.x = w[(ch + 2) * w_ld + col]; p1.y = w[(ch + 3) * w_ld + col];
+    wf[i] = make_uint2(*reinterpret_cast<uint32_t*>(&p0), *reinterpret_cast<uint32_t*>(&p1));
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int64_t total = static_cast<int64_t>(N) * H * tiles;
+  for (int64_t task = static_cast<int64_t>(blockIdx.x) * kStemDgradWarps + (threadIdx.x >> 5); task < total;
+       task += static_cast<int64_t>(gridDim.x) * kStemDgradWarps) {
+    const int tile = static_cast<int>(task % tiles);
+    const int y = static_cast<int>((task / tiles) % H);
+    const int n = static_cast<int>(task / (static_cast<int64_t>(tiles) * H));
+    const int i0 = tile * 16;
+    float d0[4] = {0.f, 0.f, 0.f, 0.f}, d1[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int r = (y + 3) & 1; r < 7; r += 2) {
+      const int oy = (y + 3 - r) >> 1;
+      if (oy < 0 || oy >= Ho) continue;
+      const __nv_bfloat16* row = dc1 + (static_cast<int64_t>(n) * Ho + oy) * Wo * 64 + 16 * t;
+#pragma unroll
+      for (int o = -1; o <= 2; ++o) {
+        uint4 lo[2], hi[2];       // rows g and g + 8 of the tile: channels 16t .. 16t+7 and 16t+8 .. 16t+15
+        const int oxg = i0 + g + o, oxh = oxg + 8;
+        const uint4 z = make_uint4(0, 0, 0, 0);
+        const bool vg = oxg >= 0 && oxg < Wo, vh = oxh >= 0 && oxh < Wo;
+        lo[0] = vg ? __ldg(reinterpret_cast<const uint4*>(row + static_cast<int64_t>(oxg) * 64)) : z;
+        lo[1] = vg ? __ldg(reinterpret_cast<const uint4*>(row + static_cast<int64_t>(oxg) * 64 + 8)) : z;
+        hi[0] = vh ? __ldg(reinterpret_cast<const uint4*>(row + static_cast<int64_t>(oxh) * 64)) : z;
+        hi[1] = vh ? __ldg(reinterpret_cast<const uint4*>(row + static_cast<int64_t>(oxh) * 64 + 8)) : z;
+        const uint32_t* wg = reinterpret_cast<const uint32_t*>(lo);
+        const uint32_t* wh = reinterpret_cast<const uint32_t*>(hi);
+        const int s0 = 3 - 2 * o, s1 = 4 - 2 * o;       // px = 0 / px = 1 tap column of this dc1 offset
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const uint32_t a[4] = {wg[2 * q], wh[2 * q], wg[2 * q + 1], wh[2 * q + 1]};
+          if (o <= 1) {
+            uint2 b = make_uint2(0, 0);
+            if (g < 3) b = wf[(((r * 7 + s0) * 4 + q) * 4 + t) * 3 + g];
+            mma_bf16_16816(d0, a, b.x, b.y);
+          }
+          uint2 b = make_uint2(0, 0);
+          if (g < 3) b = wf[(((r * 7 + s1) * 4 + q) * 4 + t) * 3 + g];
+          mma_bf16_16816(d1, a, b.x, b.y);
+        }
+      }
+    }
+    // D[row][col]: c[0], c[1] = row g, cols 2t, 2t+1; c[2], c[3] = row g+8. col = BGR channel -> RGB plane 2 - col
+    if (t < 2) {
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int i = i0 + g + 8 * half;
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc) {
+          const int c = 2 * t + cc;
+          if (c > 2) continue;
+          float* o = dx + ((static_cast<int64_t>(n) * 3 + (2 - c)) * H + y) * W;
+          if (2 * i < W) o[2 * i] = d0[2 * half + cc];
+          if (2 * i + 1 < W) o[2 * i + 1] = d1[2 * half + cc];
+        }
+      }
+    }
+  }
+}
+
 // stride-2 pixel subsample (input of a stride-2 1x1 conv): y[n, oy, ox] = x[n, 2oy, 2ox]
 __global__ void subsample2_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H, int W,
                                   int C, int Ho, int Wo) {
@@ -353,6 +504,42 @@ int cb_maxpool3x3s2_strided(const void* x, void* y, int n, int h, int w, int c, 
 
 int cb_maxpool3x3s2(const void* x, void* y, int n, int h, int w, int c, void* stream) {
   return cb_maxpool3x3s2_strided(x, y, n, h, w, c, w, static_cast<int64_t>(h) * w, stream);
+}
+
+int cb_maxpool3x3s2_bwd_strided(const void* dy, const void* x, void* dx, int n, int h, int w, int c, int64_t row_pitch,
+                                int64_t img_pitch, void* stream) {
+  CB_REQUIRE(dy && x && dx && n > 0 && h > 0 && w > 0 && c > 0 && c % 8 == 0,
+             "cb_maxpool3x3s2_bwd: bad arguments (c must be a multiple of 8)");
+  CB_REQUIRE(row_pitch >= w && img_pitch >= static_cast<int64_t>(h) * row_pitch, "cb_maxpool3x3s2_bwd: pitches smaller than the image");
+  const int ho = (h + 2 - 3) / 2 + 1, wo = (w + 2 - 3) / 2 + 1;
+  const int64_t total = static_cast<int64_t>(n) * h * w * (c / 8);
+  launch_k(maxpool3x3s2_bwd_kernel, ceil_div(total, 256), 256, 0, static_cast<cudaStream_t>(stream), static_cast<const __nv_bfloat16*>(dy),
+           static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(dx), n, h, w, c, ho, wo, row_pitch, img_pitch);
+  return check_launch("cb_maxpool3x3s2_bwd");
+}
+
+int cb_maxpool3x3s2_bwd(const void* dy, const void* x, void* dx, int n, int h, int w, int c, void* stream) {
+  return cb_maxpool3x3s2_bwd_strided(dy, x, dx, n, h, w, c, w, static_cast<int64_t>(h) * w, stream);
+}
+
+int cb_stem_dgrad(const void* dc1, const void* w, int w_ld, float* dx, int n, int h, int w_img, void* stream) {
+  CB_REQUIRE(dc1 && w && dx && n > 0 && h > 0 && w_img > 0, "cb_stem_dgrad: bad arguments");
+  CB_REQUIRE(w_ld >= 147, "cb_stem_dgrad: w_ld must be >= 147 (the 7x7x3 taps of one output channel)");
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(dc1) & 15) == 0, "cb_stem_dgrad: dc1 must be 16-byte aligned");
+  const int ho = (h - 1) / 2 + 1, wo = (w_img - 1) / 2 + 1;
+  const int tiles = ((w_img + 1) / 2 + 15) / 16;
+  const int64_t warps = static_cast<int64_t>(n) * h * tiles;
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (sms <= 0) sms = 132;
+  }
+  const int grid = static_cast<int>(std::min<int64_t>(ceil_div(warps, kStemDgradWarps), static_cast<int64_t>(sms) * 4));
+  launch_k(stem_dgrad_kernel, grid, kStemDgradWarps * 32, 0, static_cast<cudaStream_t>(stream), static_cast<const __nv_bfloat16*>(dc1),
+           static_cast<const __nv_bfloat16*>(w), w_ld, dx, n, h, w_img, ho, wo, tiles);
+  return check_launch("cb_stem_dgrad");
 }
 
 int cb_stem_s2d(const void* x, int in_dtype, void* out, int n, int h, int w, int ld, float mean_r, float mean_g, float mean_b,

@@ -113,10 +113,11 @@ class _GridEncoderConv(nn.Module):
 class _CnnFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, module, images, anchor):
-        grid, stash = module._forward_impl(images, need_backward=True)
+        grid, stash = module._forward_impl(images, need_backward=True, frames_grad=ctx.needs_input_grad[1])
         module._pending_backward += 1
         ctx.module = module
         ctx.stash = stash
+        ctx.frames = (images.shape, images.dtype)
         return grid
 
     @staticmethod
@@ -124,9 +125,13 @@ class _CnnFn(torch.autograd.Function):
         stash, ctx.stash = ctx.stash, None
         m = ctx.module
         m._pending_backward = max(0, m._pending_backward - 1)
+        dx = None
         if stash is not None:
-            m._backward_impl(stash, dgrid, last=m._pending_backward == 0)
-        return None, None, None
+            dx = m._backward_impl(stash, dgrid, last=m._pending_backward == 0)
+        if dx is not None:
+            shape, dtype = ctx.frames
+            dx = dx.view(shape).to(dtype)
+        return None, dx, None
 
 
 class GridFeatBackbone(nn.Module):
@@ -159,7 +164,7 @@ class GridFeatBackbone(nn.Module):
         # d2 FREEZE_AT: stem (1) and res2 (2) get no gradient
         if freeze_at < 1:
             # the reference ships FREEZE_AT: 2 (Base-RCNN-grid.yaml) and only ever freezes more (freeze_cnn_backbone); the
-            # backward of the stem (max-pool scatter + 7x7 wgrad) is not built, and silently returning no gradient is worse
+            # stem's weight gradient (7x7 wgrad over the patch matrix) is not built, and silently returning no gradient is worse
             raise NotImplementedError("GridFeatBackbone: FREEZE_AT = 0 (trainable stem) is not supported on the H100 path")
         bb = self.feature.backbone
         if freeze_at >= 1:
@@ -329,10 +334,11 @@ class GridFeatBackbone(nn.Module):
         """x: (B, T, 3, H, W) RGB, float (mean-subtracted) or uint8 if ``pixel_mean`` is set."""
         _require_cuda(x)
         self._ensure_ready(x.device)
-        if not (torch.is_grad_enabled() and self._any_trainable()):
+        if not (torch.is_grad_enabled() and (x.requires_grad or self._any_trainable())):
             return self._forward_impl(x, need_backward=False)[0]
-        # a trainable parameter is passed only as an autograd anchor so that backward is scheduled
-        anchor = next(m.weight for _, m in self._convs() if m.weight.requires_grad)
+        # a trainable parameter is passed only as an autograd anchor so that backward is scheduled; frames that require grad
+        # (pixel attribution, attacks on the input) anchor the node themselves and receive d grid / d frames
+        anchor = next((m.weight for _, m in self._convs() if m.weight.requires_grad), None)
         return _CnnFn.apply(self, x, anchor)
 
     def _conv1x1(self, m, x, rows, act, residual=None, rowmap=ops.ROWMAP_NONE, hw=None, out=None):
@@ -356,7 +362,9 @@ class GridFeatBackbone(nn.Module):
                  rowmap=ops.ROWMAP_UNPAD, map_h=h, map_w=w)
         return out
 
-    def _forward_impl(self, images, need_backward):
+    def _forward_impl(self, images, need_backward, frames_grad=False):
+        """``frames_grad``: the backward also computes the gradient with respect to the frames, so the stem output and every
+        block's activations (frozen blocks too) are kept."""
         dev = images.device
         bsz, n_frms, c, h, w = images.shape
         assert c == 3
@@ -401,6 +409,7 @@ class GridFeatBackbone(nn.Module):
                 ops.stem_s2d(x, s2d, n, h, w, ld, mean)
                 ops.gemm(**dict(kw, a=s2d, a_ld=ld))
             del s2d
+            pitch = (ws, hs * ws)
             ops.maxpool3x3s2(c1, cur, n, ho, wo, 64, row_pitch=ws, img_pitch=hs * ws)
             if self._capture is not None:
                 self._capture["c1"] = c1.view(n, hs, ws, 64)[:, :ho, :wo]     # the pool's view of the s2d output grid
@@ -412,9 +421,11 @@ class GridFeatBackbone(nn.Module):
             ops.gemm(mode=ops.CB_GEMM_TN, m=n * ho * wo, n=64, k=STEM_KP, a=col, a_rows=n * ho * wo, a_ld=STEM_KP, b=stem._w,
                      b_rows=64, b_ld=STEM_KP, shift=stem._shift, act=ops.ACT_RELU, out=c1, out_ld=64)
             del col
+            pitch = (None, None)
             ops.maxpool3x3s2(c1, cur, n, ho, wo, 64)
             if self._capture is not None:
                 self._capture["c1"] = c1.view(n, ho, wo, 64)
+        frames = dict(c1=c1, pitch=pitch, ho=ho, wo=wo, h=h, w=w) if need_backward and frames_grad else None
         del c1
         if self._capture is not None:
             self._capture["stem"] = cur.view(n, hh, ww, 64)
@@ -449,11 +460,12 @@ class GridFeatBackbone(nn.Module):
                     # clones of the pooled buffers: the pool hands them to a later call
                     self._capture["%s.%d" % (name, bi)] = dict(xs=xs, sc=sc, a_pad=a_pad.clone(), b=b, y=y.clone() if last else y)
                 trainable = blk.conv1.weight.requires_grad
-                if not (need_backward and trainable):
+                keep = need_backward and (trainable or frames is not None)     # a frozen block's dgrad chain leads to the frames
+                if not keep:
                     self._pad_put(a_pad, n, hh, ww)     # consumed by conv2 above; stream order makes the reuse safe
-                if need_backward and trainable:
+                else:
                     blocks.append(dict(name="%s.%d" % (name, bi), blk=blk, x_in=x_in, xs=xs, a_pad=a_pad, b=b, y=y, h=hh, w=ww, h_in=h_in, w_in=w_in,
-                                       first_trainable=not blocks))
+                                       trainable=trainable))
                 cur = y
             if self._capture is not None:
                 self._capture[name] = (cur.view(n, hh + 2, ww + 2, -1)[:, 1:-1, 1:-1] if name == "res5" else cur.view(n, hh, ww, -1))
@@ -469,7 +481,7 @@ class GridFeatBackbone(nn.Module):
         if not need_backward:
             self._pad_put(cur, n, hh, ww)           # res5 output (padded), consumed by the grid_encoder conv
         if need_backward:
-            stash = dict(n=n, h=hh, w=ww, res5_pad=cur, gconv=gconv, blocks=blocks)
+            stash = dict(n=n, h=hh, w=ww, res5_pad=cur, gconv=gconv, blocks=blocks, frames=frames)
             if self._capture is not None:
                 self._capture["stash"] = stash
         return grid, stash
@@ -530,39 +542,48 @@ class GridFeatBackbone(nn.Module):
         if ge.weight.requires_grad:
             sq.run(lambda: self._wgrad(ge, dg_pad, res5_pad, p, ntaps=9, tap_w=w + 2), dg_pad, res5_pad)
         blocks = stash["blocks"]
+        frames = stash["frames"]
         if blocks:
             # grad w.r.t. the pre-ReLU output of the last block, compact
             g = self._dgrad3x3(ge, dg_pad, n, h, w, res5_pad)
         del dg_pad
-        for st in (reversed(blocks) if blocks else ()):
+        for st in reversed(blocks):
             blk, hh, ww = st["blk"], st["h"], st["w"]
             rows = n * hh * ww
             pp = n * (hh + 2) * (ww + 2)
-            # the block's three / four weight gradients as ONE grouped launch on the side queue, issued when its last dY (da) exists
-            wg = [self._wgrad_kw(blk.conv3, g, st["b"], rows)]
+            lowest = st is blocks[0]
             db_pad = self._pad_get(n, hh, ww, blk.mid, dev)
             recycle += [(db_pad, n, hh, ww), (st["a_pad"], n, hh, ww)]
             self._dgrad1x1(blk.conv3, g, rows, aux=st["b"], rowmap=ops.ROWMAP_PAD, hw=(hh, ww), out=db_pad)
-            wg.append(self._wgrad_kw(blk.conv2, db_pad, st["a_pad"], pp, ntaps=9, tap_w=ww + 2))
             da = self._dgrad3x3(blk.conv2, db_pad, n, hh, ww, st["a_pad"])
             if cap is not None:
                 cap[st["name"]] = c = dict(g=g, db_pad=db_pad.clone(), da=da)
-            wg.append(self._wgrad_kw(blk.conv1, da, st["xs"], rows))
+            if st["trainable"]:
+                # the block's three / four weight gradients as ONE grouped launch on the side queue, issued when its last dY (da) exists
+                wg = [self._wgrad_kw(blk.conv3, g, st["b"], rows), self._wgrad_kw(blk.conv2, db_pad, st["a_pad"], pp, ntaps=9, tap_w=ww + 2),
+                      self._wgrad_kw(blk.conv1, da, st["xs"], rows)]
+                if blk.has_shortcut:
+                    wg.append(self._wgrad_kw(blk.shortcut, g, st["xs"], rows))
+                if ops.group_wgrad in (1, 2, 4):
+                    sq.run(lambda: ops.gemm_wgrad_group(wg), g, st["b"], db_pad, st["a_pad"], da, st["xs"])
+                else:
+                    sq.run(lambda: [ops.gemm(**kw) for kw in wg], g, st["b"], db_pad, st["a_pad"], da, st["xs"])
             if blk.has_shortcut:
-                wg.append(self._wgrad_kw(blk.shortcut, g, st["xs"], rows))
-            if ops.group_wgrad in (1, 2, 4):
-                sq.run(lambda: ops.gemm_wgrad_group(wg), g, st["b"], db_pad, st["a_pad"], da, st["xs"])
-            else:
-                sq.run(lambda: [ops.gemm(**kw) for kw in wg], g, st["b"], db_pad, st["a_pad"], da, st["xs"])
-            if blk.has_shortcut:
-                if last and self._bucket_hook is not None and st["name"] == "res5.0":
+                if st["trainable"] and last and self._bucket_hook is not None and st["name"] == "res5.0":
                     # every weight gradient of res5 + grid_encoder (78 % of the CNN's trainable parameters, the tail of the
                     # flat buffer) has been enqueued: its exchange can overlap the res4 / res3 backward
                     self._bucket_hook(self._flat.grad, blk.shortcut._e["offset"], sq.side if sq.forked else None)
-                if st["first_trainable"]:
+                if lowest and frames is None:
                     break                                     # d2 FREEZE_AT: no gradient below this block
                 dxs_sc = self._dgrad1x1(blk.shortcut, g, rows)
                 dxs = self._dgrad1x1(blk.conv1, da, rows, residual=dxs_sc)
+                if lowest:
+                    # res2.0 reads the stem's pooled output: dxs is the gradient at the pool output, whose backward applies the
+                    # stem's ReLU' itself (a pooled value is > 0 exactly where the element it selects is)
+                    g = dxs
+                    if cap is not None:
+                        c.update(dxs_sc=dxs_sc, dxs=dxs)
+                    break
                 g = torch.empty(n * st["h_in"] * st["w_in"], blk.cin, dtype=bf16, device=dev)
                 if blk.stride == 2:
                     ops.unsubsample2_mask(dxs, st["x_in"], g, n, st["h_in"], st["w_in"], blk.cin)
@@ -571,13 +592,24 @@ class GridFeatBackbone(nn.Module):
                 if cap is not None:
                     c.update(dxs_sc=dxs_sc, dxs=dxs, gin=g)
             else:
-                if st["first_trainable"]:
+                if lowest:
                     break
                 g = self._dgrad1x1(blk.conv1, da, rows, residual=g, aux=st["x_in"])
                 if cap is not None:
                     c.update(gin=g)
+        dx = None
+        if frames is not None:
+            # stem backward: pool (+ ReLU') to the conv output, then the transposed 7x7/s2 conv to the frames
+            ho, wo = frames["ho"], frames["wo"]
+            dc1 = torch.empty(n * ho * wo, 64, dtype=bf16, device=dev)
+            ops.maxpool3x3s2_bwd(g, frames["c1"], dc1, n, ho, wo, 64, *frames["pitch"])
+            dx = torch.empty(n, 3, frames["h"], frames["w"], dtype=torch.float32, device=dev)
+            ops.stem_dgrad(dc1, self._stem_w, dx, n, frames["h"], frames["w"])
+            if cap is not None:
+                cap["stem"] = dict(dpool=g, dc1=dc1, dx=dx)
         sq.join()
         for t, tn, th, tw in recycle:
             self._pad_put(t, tn, th, tw)
-        if not self._optimizer_emits_packed:
+        if not self._optimizer_emits_packed and self._any_trainable():
             self._dirty = True   # an optimizer step normally follows: repack bf16 operands on the next forward
+        return dx

@@ -455,7 +455,8 @@ class _ClipBertHeadModel(nn.Module):
         grid = grid.contiguous()
         ids = text_input_ids.contiguous()
         mask = text_input_mask.to(torch.int64).contiguous()
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.parameters())):
+            # a grid that requires grad keeps a fully frozen head on the graph (gradients to the frames), as in _run_base
             anchor = self.bert.pooler.dense.weight
             return _TransformerFn.apply(self, grid, anchor, ids, mask, repeat)
         return self._forward_impl(ids, grid, mask, repeat, need_backward=False)[0]

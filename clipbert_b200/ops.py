@@ -45,6 +45,9 @@ _SIGS = {
     "cb_stem_im2col": [_vp, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp],
     "cb_maxpool3x3s2": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool3x3s2_strided": [_vp, _vp, _i, _i, _i, _i, _i64, _i64, _vp],
+    "cb_maxpool3x3s2_bwd": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
+    "cb_maxpool3x3s2_bwd_strided": [_vp, _vp, _vp, _i, _i, _i, _i, _i64, _i64, _vp],
+    "cb_stem_dgrad": [_vp, _vp, _i, _vp, _i, _i, _i, _vp],
     "cb_stem_s2d": [_vp, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp],
     "cb_resize_pad": [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp],
     "cb_subsample2": [_vp, _vp, _i, _i, _i, _i, _vp],
@@ -645,6 +648,23 @@ def maxpool3x3s2(x, y, n, h, w, c, row_pitch=None, img_pitch=None):
         _call("cb_maxpool3x3s2", _p(x), _p(y), n, h, w, c, _s())
     else:
         _call("cb_maxpool3x3s2_strided", _p(x), _p(y), n, h, w, c, row_pitch, img_pitch, _s())
+
+
+def maxpool3x3s2_bwd(dy, x, dx, n, h, w, c, row_pitch=None, img_pitch=None):
+    """dx (compact [n*h*w, c]) = the pool's backward fused with the stem's ReLU'; x is the pool input on the pitches the forward
+    read it with."""
+    if row_pitch is None:
+        _call("cb_maxpool3x3s2_bwd", _p(dy), _p(x), _p(dx), n, h, w, c, _s())
+    else:
+        _call("cb_maxpool3x3s2_bwd_strided", _p(dy), _p(x), _p(dx), n, h, w, c, row_pitch, img_pitch, _s())
+
+
+def stem_dgrad(dc1, w, dx, n, h, wimg):
+    """dx: fp32 NCHW RGB [n, 3, h, wimg] contiguous = the stem conv's input gradient from dc1 (bf16 [n*ho*wo, 64]) and the stem
+    operand w (bf16 [64, >= 147], row pitch w.stride(0))."""
+    assert dx.dtype == torch.float32 and dx.is_contiguous() and dx.numel() == n * 3 * h * wimg
+    assert w.dtype == torch.bfloat16 and w.stride(1) == 1 and dc1.dtype == torch.bfloat16 and dc1.is_contiguous()
+    _call("cb_stem_dgrad", _p(dc1), _p(w), w.stride(0), _p(dx), n, h, wimg, _s())
 
 
 def subsample2(x, y, n, h, w, c):

@@ -390,6 +390,18 @@ int cb_cast_scale_segments(const float* master, void* packed, const int64_t* seg
  *                           stores every 4-pixel window explicitly. Output rows follow the same (ho+3) x (wo+3) grid.
  *   cb_maxpool3x3s2         BasicStem max_pool2d(3, 2, 1); _strided reads an input whose pixel rows / images are
  *                           row_pitch / img_pitch pixels apart (the (ho+3) x (wo+3) grid of the s2d stem)
+ *   cb_maxpool3x3s2_bwd     the gradient with respect to the frames (grid_feat.py:92-95 -> BasicStem.forward, backward): the
+ *                           pool's backward fused with the stem's ReLU', dx[n*h*w, c] (compact, the gradient at the stem conv's
+ *                           pre-ReLU output) from dy[n*ho*wo, c] and x, the pool input (the post-ReLU stem output; _strided: on
+ *                           the pitches of cb_maxpool3x3s2_strided). Gather form: each element sums, in fp32 and window order, the
+ *                           gradients of the <= 4 windows whose forward arg-max it is (first maximum, last NaN), rounds once and
+ *                           keeps it where x > 0. One writer per element, no zero fill.
+ *   cb_stem_dgrad           then the 7x7/s2/p3 transposed convolution to the frames: dx fp32 NCHW [n, 3, h, w] in RGB order (the
+ *                           BGR flip undone) = sum_{k,r,s} dc1[n, (y+3-r)/2, (x+3-s)/2, k] * w[k, (r*7+s)*3 + c], dc1 bf16 compact
+ *                           [n*ho*wo, 64], w the stem operand of the forward (bf16 [64, w_ld], FrozenBN scale and ImageNorm's
+ *                           1 / std folded in), so dx is the gradient with respect to the frames the stem gather read (raw frames
+ *                           included: the mean subtraction has unit derivative). mma.sync m16n8k16, fp32 accumulation in a fixed
+ *                           order, one writer per element: the same bits on every run.
  *   cb_subsample2           input of a stride-2 1x1 conv (res3/4/5 block 0 conv1 + shortcut)
  *   cb_unsubsample2_mask    its backward fused with the ReLU mask of the producing block
  *   cb_maxpool2x2_relu_fwd  grid_encoder MaxPool2d(2,2) + ReLU (7x7 -> 3x3 at 224 px, 14x14 -> 7x7 at 448)
@@ -414,6 +426,10 @@ int cb_stem_s2d(const void* x, int in_dtype, void* out, int n, int h, int w, int
                 void* stream);
 int cb_maxpool3x3s2(const void* x, void* y, int n, int h, int w, int c, void* stream);
 int cb_maxpool3x3s2_strided(const void* x, void* y, int n, int h, int w, int c, int64_t row_pitch, int64_t img_pitch, void* stream);
+int cb_maxpool3x3s2_bwd(const void* dy, const void* x, void* dx, int n, int h, int w, int c, void* stream);
+int cb_maxpool3x3s2_bwd_strided(const void* dy, const void* x, void* dx, int n, int h, int w, int c, int64_t row_pitch,
+                                int64_t img_pitch, void* stream);
+int cb_stem_dgrad(const void* dc1, const void* w, int w_ld, float* dx, int n, int h, int w_img, void* stream);
 int cb_subsample2(const void* x, void* y, int n, int h, int w, int c, void* stream);
 int cb_unsubsample2_mask(const void* dsub, const void* act, void* dx, int n, int h, int w, int c, void* stream);
 int cb_maxpool2x2_relu_fwd(const void* x, void* y, int n, int h, int w, int c, void* stream);
