@@ -125,6 +125,26 @@ __global__ void __launch_bounds__(256) stem_s2d_kernel(const TIn* __restrict__ x
 // up to max_size x max_size; dataset_base.py:191-195). NCHW in (uint8 or fp32), fp32 NCHW out [n, c, S, S].
 // Source coordinate of output pixel o: max(0, (o + 0.5) * in / out - 0.5) (ATen area_pixel_compute_source_index).
 // ------------------------------------------------------------------------------------------------
+// The source taps of output pixel (oy, ox) of an H x W frame (sh = H / nh, sw = W / nw in fp32): rows y0 <= y1 with weights
+// 1 - ly and ly, columns alike. At the top / left edge the coordinate clamps to 0, so ly = 0 and y0 takes weight 1; at the
+// bottom / right y1 = y0 = H - 1 and the two weights land on one pixel. cb_resize_pad and its adjoint both call this, so they
+// agree on every tap and weight. (The two axes stay in one function: with them written in this order resize_pad_kernel
+// compiles to the same instructions as when it carried these lines itself.)
+__device__ __forceinline__ void resize_taps(int oy, int ox, float sh, float sw, int H, int W, int& y0, int& x0, int& y1, int& x1,
+                                            float& ly, float& lx) {
+  const float fy = fmaxf((oy + 0.5f) * sh - 0.5f, 0.f), fx = fmaxf((ox + 0.5f) * sw - 0.5f, 0.f);
+  y0 = min(static_cast<int>(fy), H - 1), x0 = min(static_cast<int>(fx), W - 1);
+  y1 = min(y0 + 1, H - 1), x1 = min(x0 + 1, W - 1);
+  ly = fy - y0, lx = fx - x0;
+}
+
+// One axis of resize_taps (the other axis' results are unused and compiled away).
+__device__ __forceinline__ void resize_taps_1d(int o, float scale, int n, int& i0, int& i1, float& l) {
+  int j0, j1;
+  float m;
+  resize_taps(o, o, scale, scale, n, n, i0, j0, i1, j1, l, m);
+}
+
 template <typename TIn>
 __global__ void __launch_bounds__(256) resize_pad_kernel(const TIn* __restrict__ x, float* __restrict__ y, int NC, int H, int W, int nh, int nw,
                                                          int S, float sh, float sw) {
@@ -136,16 +156,118 @@ __global__ void __launch_bounds__(256) resize_pad_kernel(const TIn* __restrict__
   const int64_t plane = t / (static_cast<int64_t>(S) * S);
   float v = 0.f;
   if (oy < nh && ox < nw) {
-    const float fy = fmaxf((oy + 0.5f) * sh - 0.5f, 0.f), fx = fmaxf((ox + 0.5f) * sw - 0.5f, 0.f);
-    const int y0 = min(static_cast<int>(fy), H - 1), x0 = min(static_cast<int>(fx), W - 1);
-    const int y1 = min(y0 + 1, H - 1), x1 = min(x0 + 1, W - 1);
-    const float ly = fy - y0, lx = fx - x0;
+    int y0, x0, y1, x1;
+    float ly, lx;
+    resize_taps(oy, ox, sh, sw, H, W, y0, x0, y1, x1, ly, lx);
     const TIn* p = x + plane * H * W;
     const float a = static_cast<float>(p[static_cast<int64_t>(y0) * W + x0]), b = static_cast<float>(p[static_cast<int64_t>(y0) * W + x1]);
     const float c = static_cast<float>(p[static_cast<int64_t>(y1) * W + x0]), d = static_cast<float>(p[static_cast<int64_t>(y1) * W + x1]);
     v = (1.f - ly) * ((1.f - lx) * a + lx * b) + ly * ((1.f - lx) * c + lx * d);
   }
   y[t] = v;
+}
+
+// The output indices o in [0, n_out) whose taps include input index i: those with i0(o) in {i - 1, i}. i0 does not decrease with
+// o, so they form one range [lo, hi] (lo > hi: none). Start from the real-valued inverse of (o + 0.5) * scale - 0.5 and correct
+// it against resize_taps itself, so that fp32 rounding and the edge clamps cannot put a tap outside the range.
+__device__ __forceinline__ int2 resize_tap_range(int i, float scale, float inv_scale, int n_in, int n_out) {
+  auto first = [&](int o) {
+    int i0, i1;
+    float l;
+    resize_taps_1d(o, scale, n_in, i0, i1, l);
+    return i0;
+  };
+  int lo = min(max(static_cast<int>(ceilf((i - 0.5f) * inv_scale - 0.5f)), 0), n_out);
+  while (lo > 0 && first(lo - 1) >= i - 1) --lo;
+  while (lo < n_out && first(lo) < i - 1) ++lo;
+  int hi = min(max(static_cast<int>(ceilf((i + 1.5f) * inv_scale - 0.5f)) - 1, -1), n_out - 1);
+  while (hi < n_out - 1 && first(hi + 1) <= i) ++hi;
+  while (hi >= 0 && first(hi) > i) --hi;
+  return make_int2(lo, hi);
+}
+
+// Adjoint of resize_pad_kernel in gather form: dx[y, x] = sum over the output rows oy that tap y, in ascending order, of
+// w_y(oy) * (sum over the output columns ox that tap x, ascending, of w_x(ox) * dy[oy, ox]), with the forward's weights (1 - l on
+// the first tap, l on the second, both when they land on one pixel). The pad region (oy >= nh or ox >= nw) taps nothing. One
+// writer per element, fp32, a fixed order: the same bits on every run. A CTA covers a 32 x 32 tile of one plane (a warp per row,
+// 4 rows per thread); the output ranges of its rows and columns, and the taps of those outputs, are computed once into shared
+// memory (recomputed instead when an extreme upscale makes a tile's span longer than the table).
+constexpr int kResizeBwdTile = 32;
+constexpr int kResizeBwdTaps = 512;
+
+__global__ void __launch_bounds__(256) resize_pad_bwd_kernel(const float* __restrict__ dy, float* __restrict__ dx, int H, int W, int nh, int nw,
+                                                             int S, float sh, float sw, float inv_sh, float inv_sw, int tiles_w, int tiles_h,
+                                                             int accumulate) {
+  __shared__ int2 col_range[kResizeBwdTile], row_range[kResizeBwdTile];
+  __shared__ int2 xtap[kResizeBwdTaps], ytap[kResizeBwdTaps];     // {i0, l as bits} of output column ox_lo + j / row oy_lo + j
+  pdl_wait();
+  pdl_trigger();
+  const int tile = blockIdx.x % (tiles_w * tiles_h);
+  const int64_t plane = blockIdx.x / (tiles_w * tiles_h);
+  const int cx = (tile % tiles_w) * kResizeBwdTile, cy = (tile / tiles_w) * kResizeBwdTile;
+  const int ncols = min(kResizeBwdTile, W - cx), nrows = min(kResizeBwdTile, H - cy);
+  const int tid = threadIdx.x;
+  if (tid < kResizeBwdTile)
+    col_range[tid] = tid < ncols ? resize_tap_range(cx + tid, sw, inv_sw, W, nw) : make_int2(0, -1);
+  else if (tid >= 128 && tid < 128 + kResizeBwdTile)
+    row_range[tid - 128] = tid - 128 < nrows ? resize_tap_range(cy + tid - 128, sh, inv_sh, H, nh) : make_int2(0, -1);
+  __syncthreads();
+  // every column's range lies inside [first column's lo, last column's hi] (both ends are monotone); rows alike
+  const int ox_lo = col_range[0].x, nx = col_range[ncols - 1].y - ox_lo + 1;
+  const int oy_lo = row_range[0].x, ny = row_range[nrows - 1].y - oy_lo + 1;
+  const bool xtab = nx <= kResizeBwdTaps, ytab = ny <= kResizeBwdTaps;
+  for (int j = tid; j < kResizeBwdTaps && (j < nx || j < ny); j += blockDim.x) {
+    int i0, i1;
+    float l;
+    if (xtab && j < nx) {
+      resize_taps_1d(ox_lo + j, sw, W, i0, i1, l);
+      xtap[j] = make_int2(i0, __float_as_int(l));
+    }
+    if (ytab && j < ny) {
+      resize_taps_1d(oy_lo + j, sh, H, i0, i1, l);
+      ytap[j] = make_int2(i0, __float_as_int(l));
+    }
+  }
+  __syncthreads();
+  const int col = tid % kResizeBwdTile;
+  if (col >= ncols) return;
+  const int x = cx + col;
+  const int2 xr = col_range[col];
+  const float* plane_dy = dy + plane * S * S;
+  for (int row = tid / kResizeBwdTile; row < nrows; row += 256 / kResizeBwdTile) {
+    const int y = cy + row;
+    const int2 yr = row_range[row];
+    float acc = 0.f;
+    for (int oy = yr.x; oy <= yr.y; ++oy) {
+      int y0, y1;
+      float ly;
+      if (ytab) {
+        const int2 e = ytap[oy - oy_lo];
+        y0 = e.x, ly = __int_as_float(e.y), y1 = min(y0 + 1, H - 1);
+      } else {
+        resize_taps_1d(oy, sh, H, y0, y1, ly);
+      }
+      const float* dy_row = plane_dy + static_cast<int64_t>(oy) * S;
+      float r = 0.f;
+      for (int ox = xr.x; ox <= xr.y; ++ox) {
+        int x0, x1;
+        float lx;
+        if (xtab) {
+          const int2 e = xtap[ox - ox_lo];
+          x0 = e.x, lx = __int_as_float(e.y), x1 = min(x0 + 1, W - 1);
+        } else {
+          resize_taps_1d(ox, sw, W, x0, x1, lx);
+        }
+        const float g = __ldg(dy_row + ox);
+        if (x0 == x) r += (1.f - lx) * g;
+        if (x1 == x) r += lx * g;
+      }
+      if (y0 == y) acc += (1.f - ly) * r;
+      if (y1 == y) acc += ly * r;
+    }
+    float* o = dx + (plane * H + y) * W + x;
+    *o = accumulate ? *o + acc : acc;
+  }
 }
 
 // ATen's max-pool update (max_pool2d_with_indices): a value replaces the running maximum when it is larger or NaN, so NaN
@@ -576,6 +698,21 @@ int cb_resize_pad(const void* x, int in_dtype, float* y, int planes, int h, int 
   else
     CB_REQUIRE(false, "cb_resize_pad: in_dtype must be 0 (fp32) or 1 (uint8)");
   return check_launch("cb_resize_pad");
+}
+
+int cb_resize_pad_bwd(const float* dy, float* dx, int planes, int h, int w, int new_h, int new_w, int max_size, int accumulate,
+                      void* stream) {
+  CB_REQUIRE(dy && dx && planes > 0 && h > 0 && w > 0, "cb_resize_pad_bwd: bad arguments");
+  CB_REQUIRE(new_h > 0 && new_w > 0 && new_h <= max_size && new_w <= max_size, "cb_resize_pad_bwd: resized frame %d x %d must fit %d x %d",
+             new_h, new_w, max_size, max_size);
+  CB_REQUIRE(accumulate == 0 || accumulate == 1, "cb_resize_pad_bwd: accumulate must be 0 or 1");
+  const int tiles_w = ceil_div(w, kResizeBwdTile), tiles_h = ceil_div(h, kResizeBwdTile);
+  const int64_t blocks = static_cast<int64_t>(planes) * tiles_w * tiles_h;
+  CB_REQUIRE(blocks <= INT32_MAX, "cb_resize_pad_bwd: %lld tiles of 32 x 32 pixels exceed one launch", static_cast<long long>(blocks));
+  const float sh = static_cast<float>(h) / new_h, sw = static_cast<float>(w) / new_w;
+  launch_k(resize_pad_bwd_kernel, static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream), dy, dx, h, w, new_h, new_w, max_size, sh,
+           sw, static_cast<float>(new_h) / h, static_cast<float>(new_w) / w, tiles_w, tiles_h, accumulate);
+  return check_launch("cb_resize_pad_bwd");
 }
 
 int cb_subsample2(const void* x, void* y, int n, int h, int w, int c, void* stream) {

@@ -50,6 +50,7 @@ _SIGS = {
     "cb_stem_dgrad": [_vp, _vp, _i, _vp, _i, _i, _i, _vp],
     "cb_stem_s2d": [_vp, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp],
     "cb_resize_pad": [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp],
+    "cb_resize_pad_bwd": [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp],
     "cb_subsample2": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_unsubsample2_mask": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool2x2_relu_fwd": [_vp, _vp, _i, _i, _i, _i, _vp],
@@ -641,6 +642,15 @@ def resize_pad(x, y, new_h, new_w):
     """x: (..., h, w) uint8 / fp32 planes; y: (..., S, S) fp32 - bilinear (align_corners=False) resize to new_h x new_w, zero pad to S."""
     dt = 0 if x.dtype == torch.float32 else 1
     _call("cb_resize_pad", _p(x), dt, _p(y), x.numel() // (x.shape[-1] * x.shape[-2]), x.shape[-2], x.shape[-1], new_h, new_w, y.shape[-1], _s())
+
+
+def resize_pad_bwd(dy, dx, new_h, new_w, accumulate=False):
+    """dx: (..., h, w) fp32 = (dx if accumulate else 0) + the adjoint of resize_pad(x, y, new_h, new_w) applied to dy (..., S, S)
+    fp32, the gradient of y: d loss / d x. Both contiguous; the pad region of dy contributes nothing."""
+    assert dy.dtype == torch.float32 and dx.dtype == torch.float32 and dy.is_contiguous() and dx.is_contiguous()
+    planes = dx.numel() // (dx.shape[-1] * dx.shape[-2])
+    assert dy.shape[-1] == dy.shape[-2] and dy.numel() == planes * dy.shape[-1] * dy.shape[-2]
+    _call("cb_resize_pad_bwd", _p(dy), _p(dx), planes, dx.shape[-2], dx.shape[-1], new_h, new_w, dy.shape[-1], int(bool(accumulate)), _s())
 
 
 def maxpool3x3s2(x, y, n, h, w, c, row_pitch=None, img_pitch=None):

@@ -420,6 +420,13 @@ int cb_cast_scale_segments(const float* master, void* packed, const int64_t* seg
  * max_size x max_size; src/datasets/dataset_base.py:191-195). x: `planes` = n * c planes of h x w (in_dtype 0 fp32, 1 uint8),
  * y: fp32 [planes, max_size, max_size]. */
 int cb_resize_pad(const void* x, int in_dtype, float* y, int planes, int h, int w, int new_h, int new_w, int max_size, void* stream);
+/* dy: fp32 [planes, max_size, max_size] (the gradient of cb_resize_pad's output); dx: fp32 [planes, h, w]. Adjoint of
+ * cb_resize_pad with the same (h, w, new_h, new_w, max_size): the pad region (rows >= new_h or columns >= new_w) contributes
+ * nothing. Overwrites dx (every element written once) unless accumulate = 1, which adds into it in fp32. Gather form with the
+ * forward's own taps and weights: each dx element sums its outputs' contributions in a fixed order (output row, then column),
+ * so the bits are the same on every run; no atomics, no alignment requirement. */
+int cb_resize_pad_bwd(const float* dy, float* dx, int planes, int h, int w, int new_h, int new_w, int max_size, int accumulate,
+                      void* stream);
 int cb_stem_im2col(const void* x, int in_dtype, void* out, int n, int h, int w, int kp, float mean_r, float mean_g,
                    float mean_b, void* stream);
 int cb_stem_s2d(const void* x, int in_dtype, void* out, int n, int h, int w, int ld, float mean_r, float mean_g, float mean_b,

@@ -4,9 +4,13 @@ headline shape (128 frames of 224 px) and at 448 px (32 frames), and an eval for
 frozen ClipBert on the retrieval head at the headline shape (32 videos x 2 clips x 2 frames, forward_clips), against the same
 forward with frames that do not require grad, with torch.cuda.max_memory_allocated for both.
 
+The input stage: cb_resize_pad_bwd next to cb_resize_pad at decoded sizes users feed (720p, 240p, 1080p and 2160p sources),
+and the same attribution pass from fp32 frames decoded at 1280 x 720, through input_stage.resize_pad to 224 px.
+
 Per kernel: median over `--rounds` rounds of `--reps` back-to-back launches; compulsory bytes (pool: dy and x read, dx written
-once; stem: dc1 read, fp32 frames written once) over the time, and that as a fraction of 3.35 TB/s (the H100 SXM data-sheet HBM3
-bandwidth, for a card allowed 700 W). The card name, power limit and max SM clock are read in the same run.
+once; stem: dc1 read, fp32 frames written once; resize_pad: the source read, the padded frame written; resize_pad_bwd: the
+new_h x new_w part of dy read, the source-sized dx written) over the time, and that as a fraction of 3.35 TB/s (the H100 SXM
+data-sheet HBM3 bandwidth, for a card allowed 700 W). The card name, power limit and max SM clock are read in the same run.
 Usage: python tools/profile_input_grads.py [--reps 20 --rounds 5 --out tool_out/input_grads.txt]"""
 import argparse
 import os
@@ -21,6 +25,7 @@ import torch  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 SHAPES = [(128, 224, "headline: 128 frames of 224 px"), (32, 448, "native resolution: 32 frames of 448 px")]
+RESIZE_SHAPES = [(64, 720, 1280, 448), (64, 240, 320, 448), (16, 1080, 1920, 768), (16, 2160, 3840, 448)]
 
 
 def card():
@@ -71,6 +76,56 @@ def kernels(out, reps, rounds):
                 name, what, t, b / 1e6, b / t / 1e9, 100.0 * b / HBM_BYTES_PER_S / (t / 1e3), extra))
 
 
+def resize_kernels(out, reps, rounds):
+    from clipbert_b200 import input_stage, ops
+    dev = torch.device("cuda:0")
+    for n, h, w, size in RESIZE_SHAPES:
+        nh, nw = input_stage.get_resize_size(h, w, size)
+        x = torch.rand(n, 3, h, w, device=dev) * 255
+        y = torch.empty(n, 3, size, size, device=dev)
+        dy = torch.randn(n, 3, size, size, device=dev)
+        dx = torch.empty_like(x)
+        t_fwd = timed(lambda: ops.resize_pad(x, y, nh, nw), reps, rounds)
+        t_bwd = timed(lambda: ops.resize_pad_bwd(dy, dx, nh, nw), reps, rounds)
+        what = "%d frames %d x %d -> %d (%d x %d)" % (n, w, h, size, nw, nh)
+        src, dst = 4 * n * 3 * h * w, 4 * n * 3 * size * size
+        for name, t, b in (("cb_resize_pad", t_fwd, src + dst), ("cb_resize_pad_bwd", t_bwd, 4 * n * 3 * nh * nw + src)):
+            out("%-28s %-42s %8.3f ms  %7.1f MB  %6.2f TB/s  %5.1f %% of HBM bound" % (
+                name, what, t, b / 1e6, b / t / 1e9, 100.0 * b / HBM_BYTES_PER_S / (t / 1e3)))
+
+
+def decoded_attribution(out, reps, rounds):
+    """Eval forward + backward to fp32 frames decoded at 1280 x 720, through resize_pad to 224 px, on the fully frozen model."""
+    import clipbert_b200 as cb
+    from clipbert_b200 import input_stage
+    from clipbert_b200.workload import IMAGE_MEAN
+    from oracle import synth
+    from util import make_cfg
+    dev = torch.device("cuda:0")
+    model = cb.ClipBert(make_cfg(), detectron2_model_cfg="R-50-grid.yaml")
+    model.load_state_dict(synth.full_state_dict(42))
+    model = model.to(dev).eval()
+    for p in model.parameters():
+        p.requires_grad_(False)
+    input_stage.set_image_norm(model, IMAGE_MEAN)
+    batch = synth.synth_batch(32, 4, n_ex=1, size=224, seed=1)
+    mb = {k: (v.to(dev) if torch.is_tensor(v) else list(v)) for k, v in batch.items() if k != "visual_inputs"}
+    decoded = torch.randint(0, 256, (32, 4, 3, 720, 1280), device=dev).float()
+
+    def attribution():
+        x = decoded.detach().requires_grad_(True)
+        frames = input_stage.resize_pad(x, 224)
+        score = model.forward_clips(dict(mb, visual_inputs=frames), 2)["logits"][..., 1].sum()
+        return torch.autograd.grad(score, x)[0]
+
+    attribution()
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    t = timed(attribution, reps, rounds)
+    out("%-40s 32 videos x 2 clips x 2 frames decoded at 1280 x 720 -> 224 px: %8.2f ms   max_memory_allocated %.2f GB" % (
+        "eval forward + backward to decoded frames", t, torch.cuda.max_memory_allocated() / 1e9))
+
+
 def end_to_end(out, reps, rounds):
     import clipbert_b200 as cb
     from oracle import synth
@@ -116,7 +171,9 @@ def main():
         lines.append(s)
     out(card())
     kernels(out, args.reps, args.rounds)
+    resize_kernels(out, args.reps, args.rounds)
     end_to_end(out, max(2, args.reps // 4), args.rounds)
+    decoded_attribution(out, max(2, args.reps // 4), args.rounds)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
