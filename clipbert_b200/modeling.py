@@ -285,7 +285,7 @@ class _ClipBertHeadModel(nn.Module):
         self._call_count = 0
         self._seed_base = None
         self._drop_counter = None   # uint64 device word: the dropout stream position, advanced ON THE DEVICE once per training forward
-        self._capture = None     # tests set this to a dict to receive per-layer activations
+        self._capture = None     # tests set this to a dict to receive per-layer activations (and, in backward, gradients)
         self._inject = None      # tests: {layer index: (B', L, 768) hidden state} makes that encoder layer start from the given tensor
         self._pending_backward = 0
         self._grad_ready_hook = None
@@ -555,8 +555,11 @@ class _ClipBertHeadModel(nn.Module):
         ops.embed_text_fwd(ids, word, pos, typ, g_t, b_t, x, st["stats_t"], nseq, lt, L, eps, p_h, seed + 1)
         ops.embed_visual_fwd(grid, s2v, n_ex, row_tab, col_tab, self._emb("vis.type")[0], g_v, b_v,
                              x, st["stats_v"], nseq, T, gh, gw, lt, L, eps, p_h, seed + 2)
-        if self._capture is not None:
-            self._capture["embeddings"] = x.view(nseq, L, H).clone()
+        cap = self._capture
+        if cap is not None:
+            cap["embeddings"] = x.view(nseq, L, H).clone()
+            cap.update(seed=seed, drop_word=drop_word, stats_t=st["stats_t"], stats_v=st["stats_v"], grid=grid,
+                       idx=None if sample is None else sample[0], row_tab=row_tab, col_tab=col_tab)
         # ---- encoder ----
         hidden, attn = [], []
         for i in range(len(self.bert.encoder.layer)):
@@ -596,17 +599,19 @@ class _ClipBertHeadModel(nn.Module):
             ops.layernorm_fwd(s2, g2, b2, y, st2, eps)
             if need_backward:
                 st["layers"].append(dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2, seed=ls))
+            if cap is not None:
+                cap["l%d" % i] = dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, gel=gel, u=u, s2=s2, st2=st2)
             x = y
-            if self._capture is not None:
-                self._capture["layer%d" % i] = x.view(nseq, L, H)
+            if cap is not None:
+                cap["layer%d" % i] = x.view(nseq, L, H)
         st["x_last"] = x
         # ---- pooler on the [CLS] rows (row pitch L*768, no gather) ----
         pl = self._lin["pooler"]
         pooled = new(nseq, H)
         self._gemm_fwd(x, nseq, pl, pooled, a_ld=L * H, act=ops.ACT_TANH)
         st["pooled"] = pooled
-        if self._capture is not None:
-            self._capture["pooled"] = pooled
+        if cap is not None:
+            cap["pooled"] = pooled
         if base is not None:
             if want_hidden:
                 hidden.append(x.view(nseq, L, H))
@@ -630,7 +635,7 @@ class _ClipBertHeadModel(nn.Module):
         self._gemm_fwd(c1, nseq, c2, logits, out_fp32=1)
         st["pd"], st["c1"], st["num_out"] = pd, c1, num_out
         if self._capture is not None:
-            self._capture["c1"] = c1
+            self._capture.update(pd=pd, c1=c1, logits=logits)
         return logits[:, :num_out]
 
     def _head_forward(self, pooled, st, nseq, p_h, seed, need_backward):
@@ -665,6 +670,8 @@ class _ClipBertHeadModel(nn.Module):
         # d(pooler pre-activation) = (dc1 @ W0) * dropout_mask * tanh'(pooled)
         self._dgrad(c0, dc1, nseq, dpooled, dropout_p=st["p_h"], dropout_seed=st["seed"] + 5, aux=st["pooled"], aux_ld=H,
                     aux_mode=ops.AUX_TANH_GRAD)
+        if self._capture is not None:
+            self._capture.setdefault("bwd", {}).update(dl=dl, dc1=dc1)
         return dpooled
 
     def _head_backward(self, st, dout, nseq, H):
@@ -692,6 +699,7 @@ class _ClipBertHeadModel(nn.Module):
             return torch.empty(*shape, dtype=dtype, device=dev)
 
         ops.dropout_offset_bind(st.get("drop_word"))       # regenerate exactly this forward's masks
+        cap = None if self._capture is None else self._capture.setdefault("bwd", {})
         sq = ops.SideQueue()                               # wgrad GEMMs / bias sums run beside the dgrad chain
         base = st.get("base_grads")                        # ClipBertBaseModel.forward: (d sequence, d pooled, d hidden states)
         dhidden = dattn = None
@@ -709,10 +717,14 @@ class _ClipBertHeadModel(nn.Module):
         if dpre is not None:
             self._dgrad(pl, dpre, nseq, dx, out_ld=L * H)  # scatters into the [CLS] rows
         extra = self._extra_sequence_grad(st) if base is None else dseq
+        if cap is not None:      # clones where an add below writes the tensor in place
+            cap.update(dpre=dpre, extra=extra, dx_pooler=dx.clone() if extra is not None or dhidden is not None else dx)
         if extra is not None:
             dx += extra
         for i in reversed(range(len(st["layers"]))):
             if dhidden is not None and dhidden[i + 1] is not None:     # output of layer i = hidden_states[i + 1]
+                if cap is not None and i + 1 < len(st["layers"]):
+                    cap["l%d" % (i + 1)]["dxn"] = dx.clone()
                 dx += dhidden[i + 1]
             if ret_hidden is not None:
                 _set_retained_hidden_grad(ret_hidden[i + 1], dx, nseq, L, H)
@@ -758,6 +770,8 @@ class _ClipBertHeadModel(nn.Module):
             ops.attention_bwd(ly["qkv"], st["mask"], ly["ctx"], dctx, ly["lse"], dqkv, nseq, L, lt, heads, p_a, ls + 1)
             if dattn is not None and dattn[i] is not None:      # a loss on attentions[i]: its dQ / dK added into dqkv
                 drow = new(nseq, heads, L, dtype=f32)
+                if cap is not None:
+                    cap.setdefault("l%d" % i, {})["dqkv_attn"] = dqkv.clone()
                 ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn[i], drow, dqkv, nseq, L, lt, heads, p_a, ls + 1)
             if ret_attn is not None and ret_attn[i] is not None:
                 _add_retained_attention_grad(ret_attn[i], ly["qkv"], dctx, nseq, L, heads)
@@ -768,9 +782,15 @@ class _ClipBertHeadModel(nn.Module):
                 sq.run(lambda: (ops.gemm(**wg[3]), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
             dxn = new(M, H)
             self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
+            if cap is not None:
+                c = cap.setdefault("l%d" % i, {})
+                c.update(dx=dx, ds2=ds2, ds2d=ds2d, du=du, da=da, ds1=ds1, ds1d=ds1d, dctx=dctx, dqkv=dqkv)
+                c.setdefault("dxn", dxn)
             dx = dxn
             st["layers"][i] = None     # free this layer's stash
         if dhidden is not None and dhidden[0] is not None:                 # hidden_states[0] = the embedding output
+            if cap is not None and len(st["layers"]):
+                cap["l0"]["dxn"] = dx.clone()
             dx += dhidden[0]
         if ret_hidden is not None:
             _set_retained_hidden_grad(ret_hidden[0], dx, nseq, L, H)
@@ -800,6 +820,8 @@ class _ClipBertHeadModel(nn.Module):
                 full.index_copy_(2, idx, dgrid.view(nvid, T, gh, H))
                 dgrid = full.view(nvid, T, gh0, gw0, H)
         sq.join()          # every weight gradient is in the flat buffer before the caller (all-reduce hook, optimizer) sees it
+        if cap is not None:
+            cap.update(dx_emb=dx, dgrid=dgrid)
         if not self._optimizer_emits_packed:
             self._dirty = True
         return dgrid
@@ -1120,6 +1142,8 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
         ops.gemm(mode=ops.CB_GEMM_TN, m=R, n=vp, k=H, a=t2, a_rows=R, a_ld=H, b=self._word_bf16, b_rows=vp, b_ld=H, shift=bias,
                  out=scores, out_ld=vp, out_fp32=1)
         st.update(xt=xt, mlm_u=u, mlm_t1=t1, mlm_t2=t2, mlm_stats=stats)
+        if self._capture is not None:
+            self._capture.update(itm=itm, xt=xt, mlm_u=u, t1=t1, t2=t2, mlm_stats=stats, scores=scores)
         v = _cfg(self.config, "vocab_size")
         return itm[:, :2], scores.view(nseq, lt, vp)[:, :, :v]
 
@@ -1130,6 +1154,7 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
         nseq_, nvid, T, gh, gw, lt, L = st["dims"]
         R = nseq * lt
         itm_l, t_l = self._lin["itm"], self._lin["mlm_t"]
+        cap = None if self._capture is None else self._capture.setdefault("bwd", {})
         dpre = torch.zeros(nseq, H, dtype=bf16, device=dev)
         if ditm is not None:
             dl = torch.empty(nseq, itm_l.n, dtype=bf16, device=dev)
@@ -1137,6 +1162,8 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
             self._wgrad(itm_l, dl, st["pooled"], nseq)
             ops.colsum(dl, itm_l.gb, nseq, itm_l.n)
             self._dgrad(itm_l, dl, nseq, dpre, aux=st["pooled"], aux_ld=H, aux_mode=ops.AUX_TANH_GRAD)
+            if cap is not None:
+                cap["dl"] = dl
         st["mlm_dx"] = None
         if dscores is not None:
             vp = self._word_bf16.shape[0]
@@ -1163,6 +1190,8 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
             dxt = torch.empty(R, H, dtype=bf16, device=dev)
             self._dgrad(t_l, du, R, dxt)
             st["mlm_dx"] = dxt
+            if cap is not None:
+                cap.update(ds=ds, dt2=dt2, dt1=dt1, mlm_du=du, dxt=dxt)
         return dpre
 
     def _extra_sequence_grad(self, st):

@@ -36,9 +36,10 @@ NAN_PAD = 64                # NaN floats before and after the dprobs / lse windo
 
 
 # ------------------------------------------------------------------------------------------------ reference
-def probs_bwd_ref(q, k, madd, lse, r, Gr, dq0, dk0):
+def probs_bwd_ref(q, k, madd, lse, r, Gr, dq0, dk0, rounded=True):
     """[(dQ, bound), (dK, bound)] as [NSEQ, H, L, 64] float64, from the bf16 Q / K, the kernel's lse, the multipliers r and the
-    upstream gradient Gr (float64 of the fp32 values), added to dq0 / dk0."""
+    upstream gradient Gr (float64 of the fp32 values), added to dq0 / dk0. rounded: dS is rounded to bf16 before the products,
+    as the tensor-core kernel does (False: the CPU emulator, which keeps it unrounded)."""
     L = q.shape[2]
     S, eS = A._scores(q, k, madd)
     lse = lse.detach().cpu().double()[..., None]
@@ -51,7 +52,7 @@ def probs_bwd_ref(q, k, madd, lse, r, Gr, dq0, dk0):
     gd = g - Dv
     dS = P * gd
     edS = P * (eg + eD + U * gd.abs()) + eP * gd.abs() + U * dS.abs()
-    dSX, amb = A._inter(dS, edS, True)
+    dSX, amb = A._inter(dS, edS, rounded)
     depth = 3.0 * (L + 1)
     out = []
     for Am, ambm, B, old in ((dSX, amb, k, dq0), (dSX.transpose(-1, -2), amb.transpose(-1, -2), q, dk0)):
