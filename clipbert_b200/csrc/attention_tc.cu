@@ -963,7 +963,23 @@ __device__ __forceinline__ void tc_acc_add_global(const float (&acc)[8][4], __nv
   }
 }
 
-// dQ of one 64-query tile; writes D of its rows to drow [nseq, heads, l]
+// dst (bf16, 16 rows r0 + lane / 4, + 8 of a 64-column block, row pitch ld) = acc * mul, rounded once; rows >= nrows are not
+// touched and nothing is read
+__device__ __forceinline__ void tc_acc_store_global(const float (&acc)[8][4], __nv_bfloat16* dst, int64_t ld, int r0, int lane, int nrows,
+                                                    float mul) {
+  const int r = r0 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    if (r + 8 * half < nrows) {
+      uint32_t* row = reinterpret_cast<uint32_t*>(dst + static_cast<int64_t>(r + 8 * half) * ld + c);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) row[j * 4] = pack_bf16x2(acc[j][2 * half] * mul, acc[j][2 * half + 1] * mul);
+    }
+  }
+}
+
+// dQ of one 64-query tile; writes D of its rows to drow [nseq, heads, l]. STORE: dQ is written, not added (a fresh dqkv)
+template <bool STORE>
 __global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_bwd_q_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                                                          int64_t ld_qkv, const int64_t* __restrict__ text_mask,
                                                                          const float* __restrict__ lse, const float* __restrict__ dprobs,
@@ -1032,10 +1048,16 @@ __global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_bwd_q_kernel(const _
       }
     }
   }
-  if (live) tc_acc_add_global(acc, dq + (row0 + q0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nq, scale);
+  if (live) {
+    if (STORE)
+      tc_acc_store_global(acc, dq + (row0 + q0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nq, scale);
+    else
+      tc_acc_add_global(acc, dq + (row0 + q0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nq, scale);
+  }
 }
 
-// dK of one 64-key tile, with D from drow
+// dK of one 64-key tile, with D from drow. STORE: dK is written, not added
+template <bool STORE>
 __global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_bwd_k_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                                                          int64_t ld_qkv, const int64_t* __restrict__ text_mask,
                                                                          const float* __restrict__ lse, const float* __restrict__ dprobs,
@@ -1098,7 +1120,94 @@ __global__ void __launch_bounds__(TC_THREADS) attn_tc_probs_bwd_k_kernel(const _
     __syncthreads();
     if (warp < nks) tc_mm_atb_live(dkacc, dSs, Qs, r0, lane, nqs);   // this warp's 16 key rows: dK += dS^T Q
   }
-  if (warp < nks) tc_acc_add_global(dkacc, dk + (row0 + k0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nk, scale);
+  if (warp < nks) {
+    if (STORE)
+      tc_acc_store_global(dkacc, dk + (row0 + k0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nk, scale);
+    else
+      tc_acc_add_global(dkacc, dk + (row0 + k0) * ld_dqkv + h * 64, ld_dqkv, r0, lane, nk, scale);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ dV alone
+// dV_j = sum_i P_ij r_ij dO_i of one 64-key tile, for the backward split at a differentiable attention map (the context product's
+// share of the attention backward; dQ / dK come from the map's gradient through cb_attention_probs_bwd_store). P is rebuilt from
+// Q, K and the saved lse as attn_tc_probs_kernel forms it, with the forward's dropout multipliers r; the returned map is never
+// read. The layout of attn_tc_bwd_kv_kernel without dS: K and the key mask stay in smem; per query tile, phase 1 (each warp: 16
+// query rows x 64 keys) forms P r and stages it as bf16, phase 2 (each warp: 16 key rows) accumulates dV += (P r)^T dO in
+// registers. dV is written once to the V block: one writer per element, no atomics.
+__global__ void __launch_bounds__(TC_THREADS) attn_tc_bwd_dv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                                    int64_t ld_qkv, const int64_t* __restrict__ text_mask,
+                                                                    const __nv_bfloat16* __restrict__ dctx, int64_t ld_ctx,
+                                                                    const float* __restrict__ lse, __nv_bfloat16* __restrict__ dv,
+                                                                    int64_t ld_dqkv, int L, int Lt, int H, float scale, TcDrop dc_in) {
+  pdl_wait();
+  const TcDrop dc = drop_resolve(dc_in);   // seed + device-side offset (read after the wait)
+  pdl_trigger();
+  extern __shared__ __align__(16) uint8_t tc_smem[];
+  __nv_bfloat16* Ks = reinterpret_cast<__nv_bfloat16*>(tc_smem);
+  __nv_bfloat16* Qs = Ks + TC_TILE;
+  __nv_bfloat16* dOs = Qs + TC_TILE;
+  __nv_bfloat16* Ps = dOs + TC_TILE;     // dropped probabilities [query][key], then the dV tile
+  float* madd = reinterpret_cast<float*>(Ps + TC_TILE);
+  float* lses = madd + 64;
+  const int kb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int k0 = kb * 64;
+  const int nk = min(64, L - k0), nks = tc_live_slabs(nk);
+  const int64_t row0 = static_cast<int64_t>(b) * L;
+  const uint64_t bh0 = (static_cast<uint64_t>(b) * H + h) * L;         // row of query 0 in P viewed as [nseq*H*L, L]
+  tc_load_tile(Ks, k + (row0 + k0) * ld_qkv + h * 64, ld_qkv, nk);
+  tc_key_mask(madd, text_mask, b, k0, L, Lt);
+  const int r0 = warp * 16;
+  const int rq = r0 + (lane >> 2), cq = 2 * (lane & 3);
+  float dvacc[8][4];
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) dvacc[j][e] = 0.f;
+  const int nqb = (L + 63) / 64;
+  for (int qb = 0; qb < nqb; ++qb) {
+    const int q0 = qb * 64, nq = min(64, L - q0);
+    const int nqs = tc_live_slabs(nq);
+    __syncthreads();                     // phase 2 of the previous query tile is done with Qs, dOs and Ps
+    tc_load_tile(Qs, q + (row0 + q0) * ld_qkv + h * 64, ld_qkv, nq);
+    tc_load_tile(dOs, dctx + (row0 + q0) * ld_ctx + h * 64, ld_ctx, nq);
+    if (threadIdx.x < 64) lses[threadIdx.x] = static_cast<int>(threadIdx.x) < nq ? lse[bh0 + q0 + threadIdx.x] : 0.f;
+    __syncthreads();
+    if (warp < nqs) {
+      float s[8][4];
+      tc_mm_abt_live(s, Qs, Ks, r0, lane, nks);
+      const bool ok0 = rq < nq, ok1 = rq + 8 < nq;
+      const float l0 = lses[rq], l1 = lses[rq + 8];
+      const uint64_t e0 = (bh0 + q0 + rq) * L + k0, e1 = e0 + static_cast<uint64_t>(8) * L;   // dropout index of (row, k0)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float m0 = madd[j * 8 + cq], m1 = madd[j * 8 + cq + 1];
+        float p0 = ok0 ? __expf(s[j][0] * scale + m0 - l0) : 0.f, p1 = ok0 ? __expf(s[j][1] * scale + m1 - l0) : 0.f;
+        float p2 = ok1 ? __expf(s[j][2] * scale + m0 - l1) : 0.f, p3 = ok1 ? __expf(s[j][3] * scale + m1 - l1) : 0.f;
+        if (dc.thresh) {
+          float r_0, r_1, r_2, r_3;
+          dropout_mult2(dc.seed, e0 + j * 8 + cq, dc.thresh, dc.inv_keep, r_0, r_1);
+          dropout_mult2(dc.seed, e1 + j * 8 + cq, dc.thresh, dc.inv_keep, r_2, r_3);
+          p0 *= r_0; p1 *= r_1; p2 *= r_2; p3 *= r_3;
+        }
+        *reinterpret_cast<uint32_t*>(Ps + rq * TC_LD + j * 8 + cq) = pack_bf16x2(p0, p1);
+        *reinterpret_cast<uint32_t*>(Ps + (rq + 8) * TC_LD + j * 8 + cq) = pack_bf16x2(p2, p3);
+      }
+    } else {                             // all 16 query rows beyond L: P = 0
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        *reinterpret_cast<uint32_t*>(Ps + rq * TC_LD + j * 8 + cq) = 0u;
+        *reinterpret_cast<uint32_t*>(Ps + (rq + 8) * TC_LD + j * 8 + cq) = 0u;
+      }
+    }
+    __syncthreads();
+    if (warp < nks) tc_mm_atb_live(dvacc, Ps, dOs, r0, lane, nqs);   // this warp's 16 key rows: dV += (P r)^T dO
+  }
+  __syncthreads();                       // P fully consumed: stage dV in its tile
+  tc_acc_to_smem(dvacc, Ps, r0, lane, 1.0f);
+  __syncthreads();
+  tc_store_tile(Ps, dv + (row0 + k0) * ld_dqkv + h * 64, ld_dqkv, nk);
 }
 
 static TcDrop make_tc_drop(float p, uint64_t seed) { return make_drop(p, seed); }
@@ -1237,20 +1346,22 @@ extern "C" int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t
   return check_launch("cb_attention_probs");
 }
 
-extern "C" int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const float* dprobs,
-                                      float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
-                                      float dropout_p, uint64_t seed, void* stream) {
-  using namespace cb;
-  CB_REQUIRE(head_dim == 64, "cb_attention_probs_bwd: head_dim %d unsupported (built for 64)", head_dim);
+namespace cb {
+// cb_attention_probs_bwd (STORE = false: added to dQ / dK) and cb_attention_probs_bwd_store (written)
+template <bool STORE>
+static int attention_probs_bwd(const char* name, const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse,
+                               const float* dprobs, float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads,
+                               int head_dim, float dropout_p, uint64_t seed, void* stream) {
+  CB_REQUIRE(head_dim == 64, "%s: head_dim %d unsupported (built for 64)", name, head_dim);
   CB_REQUIRE(qkv && text_mask && lse && dprobs && drow && dqkv && nseq > 0 && l > 0 && lt >= 0 && lt <= l && heads > 0 && nseq <= 65535 &&
                  heads <= 65535,
-             "cb_attention_probs_bwd: bad arguments");
+             "%s: bad arguments", name);
   CB_REQUIRE(ld_qkv % 8 == 0 && ld_dqkv % 8 == 0 && ld_qkv >= 3 * static_cast<int64_t>(heads) * 64 &&
                  ld_dqkv >= 3 * static_cast<int64_t>(heads) * 64,
-             "cb_attention_probs_bwd: row pitches must be multiples of 8 and hold Q | K | V");
+             "%s: row pitches must be multiples of 8 and hold Q | K | V", name);
   CB_REQUIRE(reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(dqkv) % 16 == 0 &&
                  reinterpret_cast<uintptr_t>(dprobs) % 16 == 0,
-             "cb_attention_probs_bwd: qkv, dqkv and dprobs must be 16-byte aligned");
+             "%s: qkv, dqkv and dprobs must be 16-byte aligned", name);
   // q kernel: Q, K tiles + key mask, lse = 18.5 KB; k kernel: K, Q, dS tiles + key mask, lse, D = 27.8 KB
   const int smem_q = 2 * TC_TILE * 2 + 2 * 64 * 4;
   const int smem_k = 3 * TC_TILE * 2 + 3 * 64 * 4;
@@ -1260,13 +1371,51 @@ extern "C" int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int
   const TcDrop dc = make_tc_drop(dropout_p, seed);
   const dim3 grid(ceil_div(l, 64), heads, nseq);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  launch_k(attn_tc_probs_bwd_q_kernel, grid, TC_THREADS, smem_q, st, base, base + hid, ld_qkv, text_mask, lse, dprobs, drow, dbase, ld_dqkv,
-           l, lt, heads, 0.125f, dc);
-  int rc = check_launch("cb_attention_probs_bwd(q)");
+  launch_k(attn_tc_probs_bwd_q_kernel<STORE>, grid, TC_THREADS, smem_q, st, base, base + hid, ld_qkv, text_mask, lse, dprobs, drow, dbase,
+           ld_dqkv, l, lt, heads, 0.125f, dc);
+  int rc = check_launch(STORE ? "cb_attention_probs_bwd_store(q)" : "cb_attention_probs_bwd(q)");
   if (rc) return rc;
-  launch_k(attn_tc_probs_bwd_k_kernel, grid, TC_THREADS, smem_k, st, base, base + hid, ld_qkv, text_mask, lse, dprobs,
+  launch_k(attn_tc_probs_bwd_k_kernel<STORE>, grid, TC_THREADS, smem_k, st, base, base + hid, ld_qkv, text_mask, lse, dprobs,
            static_cast<const float*>(drow), dbase + hid, ld_dqkv, l, lt, heads, 0.125f, dc);
-  return check_launch("cb_attention_probs_bwd(k)");
+  return check_launch(STORE ? "cb_attention_probs_bwd_store(k)" : "cb_attention_probs_bwd(k)");
+}
+}  // namespace cb
+
+extern "C" int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const float* dprobs,
+                                      float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
+                                      float dropout_p, uint64_t seed, void* stream) {
+  return cb::attention_probs_bwd<false>("cb_attention_probs_bwd", qkv, ld_qkv, text_mask, lse, dprobs, drow, dqkv, ld_dqkv, nseq, l, lt,
+                                        heads, head_dim, dropout_p, seed, stream);
+}
+
+extern "C" int cb_attention_probs_bwd_store(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse,
+                                            const float* dprobs, float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt,
+                                            int heads, int head_dim, float dropout_p, uint64_t seed, void* stream) {
+  return cb::attention_probs_bwd<true>("cb_attention_probs_bwd_store", qkv, ld_qkv, text_mask, lse, dprobs, drow, dqkv, ld_dqkv, nseq, l,
+                                       lt, heads, head_dim, dropout_p, seed, stream);
+}
+
+extern "C" int cb_attention_bwd_dv(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const void* dctx,
+                                   int64_t ld_ctx, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
+                                   float dropout_p, uint64_t seed, void* stream) {
+  using namespace cb;
+  CB_REQUIRE(head_dim == 64, "cb_attention_bwd_dv: head_dim %d unsupported (built for 64)", head_dim);
+  CB_REQUIRE(qkv && text_mask && lse && dctx && dqkv && nseq > 0 && l > 0 && lt >= 0 && lt <= l && heads > 0 && nseq <= 65535 &&
+                 heads <= 65535,
+             "cb_attention_bwd_dv: bad arguments");
+  CB_REQUIRE(ld_qkv % 8 == 0 && ld_ctx % 8 == 0 && ld_dqkv % 8 == 0 && ld_qkv >= 3 * static_cast<int64_t>(heads) * 64 &&
+                 ld_dqkv >= 3 * static_cast<int64_t>(heads) * 64 && ld_ctx >= static_cast<int64_t>(heads) * 64,
+             "cb_attention_bwd_dv: row pitches must be multiples of 8 and hold Q | K | V and the merged heads");
+  CB_REQUIRE(reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(dctx) % 16 == 0 &&
+                 reinterpret_cast<uintptr_t>(dqkv) % 16 == 0,
+             "cb_attention_bwd_dv: qkv, dctx and dqkv must be 16-byte aligned");
+  const int smem = 4 * TC_TILE * 2 + 2 * 64 * 4;                  // K, Q, dO, P tiles (bf16) + key mask, lse (fp32): 37 KB
+  const __nv_bfloat16* base = static_cast<const __nv_bfloat16*>(qkv);
+  const int hid = heads * 64;
+  launch_k(attn_tc_bwd_dv_kernel, dim3(ceil_div(l, 64), heads, nseq), TC_THREADS, smem, static_cast<cudaStream_t>(stream), base,
+           base + hid, ld_qkv, text_mask, static_cast<const __nv_bfloat16*>(dctx), ld_ctx, lse,
+           static_cast<__nv_bfloat16*>(dqkv) + 2 * hid, ld_dqkv, l, lt, heads, 0.125f, make_tc_drop(dropout_p, seed));
+  return check_launch("cb_attention_bwd_dv");
 }
 
 extern "C" int cb_attention_dprobs(const void* qkv, int64_t ld_qkv, const void* dctx, int64_t ld_ctx, float* dprobs, int accumulate,

@@ -18,6 +18,7 @@ is the hand-written sm_90a kernels behind libclipbert_sm90.so:
                  cb_gemm WGRAD accumulating fp32 into the flat gradient buffer, activation
                  derivatives and dropout masks fused into the dgrad / LayerNorm-backward epilogues.
 """
+import contextlib
 import weakref
 
 import torch
@@ -147,12 +148,23 @@ class ClipBertBaseModel(nn.Module):
     included); ``hidden_states[k].grad`` is the full gradient at the input of layer k, and ``sequence_output.grad`` (the
     same tensor as hidden_states[12] in the reference) the full top gradient, pooler path included; ``pooled_output.grad``
     is its direct term, which is its full gradient. A pass with nothing retained issues the same launches as without.
-    Unsupported: ``torch.autograd.grad(score, attentions)`` (or hidden states), and tensor hooks on the maps or hidden
-    states. The whole pass is one autograd node, and a tensor's hooks fire before that node runs, so they see only the
-    loss's direct term; ``.grad`` of a retained tensor is completed inside the node.
+
+    By default the whole pass is one autograd node: a tensor hook on a map or hidden state fires before that node runs and sees
+    only the loss's direct term, and ``torch.autograd.grad(score, attentions)`` (or hidden states) returns only that term.
+    ``model.layerwise_autograd = True`` (default False; also on ``head.bert``) makes a pass that records autograd a chain of
+    nodes - the embeddings, one node per encoder layer (two when the maps are differentiable: A_k, hidden_states[k] ->
+    attentions[k], and C_k, (hidden_states[k], attentions[k]) -> hidden_states[k + 1], the reference's dataflow) and the
+    pooler - with sequence_output the same tensor as hidden_states[12]. Tensor hooks, ``torch.autograd.grad``,
+    ``retain_grad()`` and ``backward(inputs=...)`` on any map or hidden state then follow torch's semantics, and a hook that
+    rewrites a map's gradient changes every gradient below that layer. Parameter gradients too: a node writes them only when
+    the backward accumulates into the parameters (``autograd.grad`` leaves the flat gradient buffer as it was), and
+    ``retain_graph=True`` allows a second backward. The forward issues the launches of the default; so does the backward of a
+    layer whose map is not differentiable. Refused together with the overlapped data-parallel exchange
+    (``enable_overlapped_allreduce``): the switch is for analysis, not training.
     """
 
     differentiable_attentions = False
+    layerwise_autograd = False
 
     def __init__(self, config, _engine=None):
         super().__init__()
@@ -171,7 +183,7 @@ class ClipBertBaseModel(nn.Module):
 
     def forward(self, text_input_ids, visual_inputs, attention_mask):
         return self._engine._run_base(text_input_ids, visual_inputs, attention_mask, self.output_hidden_states, self.output_attentions,
-                                      self.differentiable_attentions)
+                                      self.differentiable_attentions, self.layerwise_autograd)
 
 
 def _require_cuda(t):
@@ -270,6 +282,153 @@ class _BaseModelFn(torch.autograd.Function):
         if outs[0] is not None:
             at_input[n_layers].append(outs[0])
         return at_input, (attn if any(t is not None for t in attn) else None)
+
+
+_LAYER_STASH = ("x", "qkv", "ctx", "lse", "s1", "st1", "a", "u", "gel", "s2", "st2")
+
+
+class _LayerwisePass:
+    """What the nodes of one layerwise bert(...) pass share: the engine, the pass's stash (its per-layer activations move into the
+    nodes' saved tensors) and the hand-over from C_k to A_k of a map-split layer (dqkv with its V block, ds1)."""
+
+    def __init__(self, module, st):
+        self.module, self.st, self.handover = module, st, {}
+
+    def dims(self):
+        nseq, _, _, _, _, _, L = self.st["dims"]
+        return nseq, L, _cfg(self.module.config, "hidden_size")
+
+    def dense(self, g):
+        """An upstream gradient of a hidden state as the engine's [nseq * L, H] contiguous bf16 operand."""
+        nseq, L, H = self.dims()
+        return g.reshape(nseq * L, H).to(torch.bfloat16).contiguous()
+
+    def hidden(self, i):
+        """hidden_states[i] as a fresh view: the input of layer i, or the top of the encoder."""
+        nseq, L, H = self.dims()
+        layers = self.st["layers"]
+        return (layers[i]["x"] if i < len(layers) else self.st["x_last"]).view(nseq, L, H)
+
+
+def _will_execute(ctx, k):
+    """Whether the engine runs, in the current backward, the node behind tensor input k of this node (False when that input
+    takes no gradient). For a parameter anchor: whether this backward accumulates into the parameters - backward() does;
+    torch.autograd.grad() and backward(inputs=...) without the parameter do not."""
+    node = ctx.next_functions[k][0]
+    if node is None:
+        return False
+    try:
+        return bool(torch._C._will_engine_execute_node(node))
+    except RuntimeError:        # autograd.grad() with the anchor parameter among its inputs: no accumulation into .grad
+        return False
+
+
+class _EmbeddingNode(torch.autograd.Function):
+    """(visual_inputs, anchor) -> hidden_states[0]."""
+
+    @staticmethod
+    def forward(ctx, ps, grid, anchor):
+        st = ps.st
+        ctx.ps = ps
+        ctx.save_for_backward(st.pop("ids"), st.pop("grid"), st.pop("stats_t"), st.pop("stats_v"))
+        return ps.hidden(0)
+
+    @staticmethod
+    def backward(ctx, dh):
+        ids, grid, stats_t, stats_v = ctx.saved_tensors
+        ps = ctx.ps
+        grads, need_grid = _will_execute(ctx, 1), _will_execute(ctx, 0)
+        if not (grads or need_grid):
+            return None, None, None
+        st = dict(ps.st, ids=ids, grid=grid, stats_t=stats_t, stats_v=stats_v)
+        with ps.module._node_backward(st, grads):
+            dgrid = ps.module._embedding_backward(st, ps.dense(dh), need_grid, grads)
+        return None, dgrid, None
+
+
+class _LayerNode(torch.autograd.Function):
+    """Encoder layer i, hidden_states[i] -> hidden_states[i + 1] (maps not differentiable)."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, anchor):
+        ly = ps.st["layers"][i]
+        ctx.ps, ctx.i, ctx.seed = ps, i, ly["seed"]
+        ctx.save_for_backward(*(ly[k] for k in _LAYER_STASH))
+        return ps.hidden(i + 1)
+
+    @staticmethod
+    def backward(ctx, dy):
+        ly = dict(zip(_LAYER_STASH, ctx.saved_tensors), seed=ctx.seed)
+        ps, grads = ctx.ps, _will_execute(ctx, 1)
+        with ps.module._node_backward(ps.st, grads) as sq:
+            dxn = ps.module._layer_backward(ps.st, ctx.i, ly, ps.dense(dy), sq, grads=grads)
+        return None, None, dxn.view(*ps.dims()), None
+
+
+class _MapNode(torch.autograd.Function):
+    """A_k: hidden_states[k] -> attentions[k]. Its backward receives the map's full gradient G (the direct term, C_k's dO V^T and
+    whatever hooks made of them) and finishes layer k: dQ / dK from G, the QKV weight gradient, the dgrad to hidden_states[k]."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, anchor):
+        ly = ps.st["layers"][i]
+        ctx.ps, ctx.i, ctx.seed = ps, i, ly["seed"]
+        ctx.save_for_backward(ly["x"], ly["qkv"], ly["lse"])
+        return ps.st["attn"][i]
+
+    @staticmethod
+    def backward(ctx, G):
+        x, qkv, lse = ctx.saved_tensors
+        ps, grads = ctx.ps, _will_execute(ctx, 1)
+        handover = ps.handover.pop(ctx.i, None)
+        with ps.module._node_backward(ps.st, grads) as sq:
+            dxn = ps.module._map_backward(ps.st, ctx.i, dict(x=x, qkv=qkv, lse=lse, seed=ctx.seed), G.to(torch.float32).contiguous(),
+                                          handover, sq, grads)
+        return None, None, dxn.view(*ps.dims()), None
+
+
+class _ContextNode(torch.autograd.Function):
+    """C_k: (hidden_states[k], attentions[k]) -> hidden_states[k + 1], the reference's dataflow past the map (ctx = A V, output
+    projection, LN1, FFN, LN2). Its backward returns d A = dO V^T for the map and nothing for hidden_states[k]: dV and the
+    residual ds1 are handed to A_k, which produces the whole gradient at hidden_states[k]."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, a, anchor):
+        ly = ps.st["layers"][i]
+        ctx.ps, ctx.i, ctx.seed = ps, i, ly["seed"]
+        ctx.save_for_backward(*(ly[k] for k in _LAYER_STASH))
+        return ps.hidden(i + 1)
+
+    @staticmethod
+    def backward(ctx, dy):
+        ly = dict(zip(_LAYER_STASH, ctx.saved_tensors), seed=ctx.seed)
+        ps, grads = ctx.ps, _will_execute(ctx, 2)
+        split = "with_map" if _will_execute(ctx, 1) else "map_only"       # A_k runs in this backward: hand dV and ds1 over
+        with ps.module._node_backward(ps.st, grads) as sq:
+            dmap, handover = ps.module._layer_backward(ps.st, ctx.i, ly, ps.dense(dy), sq, grads=grads, split=split)
+        if handover is not None:
+            ps.handover[ctx.i] = handover
+        return None, None, None, dmap, None
+
+
+class _PoolerNode(torch.autograd.Function):
+    """hidden_states[-1] (= sequence_output) -> pooled_output."""
+
+    @staticmethod
+    def forward(ctx, ps, h, anchor):
+        ctx.ps = ps
+        pooled = ps.st.pop("pooled")
+        ctx.save_for_backward(ps.st.pop("x_last"), pooled)
+        return pooled
+
+    @staticmethod
+    def backward(ctx, dpooled):
+        x_last, pooled = ctx.saved_tensors
+        ps, grads = ctx.ps, _will_execute(ctx, 1)
+        nseq, L, H = ps.dims()
+        with ps.module._node_backward(ps.st, grads):
+            dx = ps.module._pooler_backward(_pooler_pre_grad(pooled, dpooled), x_last, nseq, L, H, grads)
+        return None, dx.view(nseq, L, H), None
 
 
 class _ClipBertHeadModel(nn.Module):
@@ -461,7 +620,7 @@ class _ClipBertHeadModel(nn.Module):
             return _TransformerFn.apply(self, grid, anchor, ids, mask, repeat)
         return self._forward_impl(ids, grid, mask, repeat, need_backward=False)[0]
 
-    def _run_base(self, text_input_ids, visual_inputs, attention_mask, want_hidden, want_attn, diff_attn=False):
+    def _run_base(self, text_input_ids, visual_inputs, attention_mask, want_hidden, want_attn, diff_attn=False, layerwise=False):
         """ClipBertBaseModel.forward on this engine (the head itself is not run). visual_inputs: (B', T, h, w, 768)."""
         _require_cuda(text_input_ids)
         self._ensure_ready(text_input_ids.device)
@@ -471,7 +630,9 @@ class _ClipBertHeadModel(nn.Module):
         ids = text_input_ids.contiguous()
         mask = attention_mask.to(torch.int64).contiguous()
         flags = (bool(want_hidden), bool(want_attn), bool(want_attn and diff_attn))
-        if torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters())):
+        if torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters())) and layerwise:
+            seq, pooled, hidden, attn = self._run_layerwise(ids, grid, mask, flags)
+        elif torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters())):
             outs = _BaseModelFn.apply(self, grid, self.bert.pooler.dense.weight, ids, mask, flags)
             n_hidden = len(self.bert.encoder.layer) + 1 if flags[0] else 0
             seq, pooled, hidden, attn = outs[0], outs[1], outs[2:2 + n_hidden], outs[2 + n_hidden:]
@@ -483,6 +644,51 @@ class _ClipBertHeadModel(nn.Module):
         if flags[1]:
             out = out + (tuple(attn),)
         return out
+
+    def _run_layerwise(self, ids, grid, mask, flags):
+        """ClipBertBaseModel.forward with layerwise_autograd: the pass runs as _forward_impl runs it (same launches, same bits),
+        then its outputs are handed out through a chain of autograd nodes - the embeddings, one node per encoder layer (two, A_k
+        and C_k, when the maps are differentiable) and the pooler - so that tensor hooks, torch.autograd.grad and
+        backward(inputs=...) on any hidden state or map follow torch's own semantics. Returns (sequence_output, pooled_output,
+        hidden_states, attentions) as _forward_impl does."""
+        if self._grad_ready_hook is not None:
+            raise RuntimeError("ClipBertBaseModel.layerwise_autograd is for analysis, not data-parallel training: it cannot run while "
+                               "the overlapped gradient exchange (enable_overlapped_allreduce) is enabled")
+        with torch.no_grad():
+            (_, _, _, attn), st = self._forward_impl(ids, grid, mask, (1, None, None), need_backward=True, base=flags)
+        st["attn"] = attn
+        ps = _LayerwisePass(self, st)
+        bert = self.bert
+        h = _EmbeddingNode.apply(ps, grid, bert.embeddings.word_embeddings.weight)
+        hidden, maps = [h], []
+        for i, layer in enumerate(bert.encoder.layer):
+            if flags[2]:
+                a = _MapNode.apply(ps, i, h, layer.attention.self.query.weight)
+                h = _ContextNode.apply(ps, i, h, a, layer.attention.output.dense.weight)
+                maps.append(a)
+            else:
+                h = _LayerNode.apply(ps, i, h, layer.attention.self.query.weight)
+            hidden.append(h)
+        pooled = _PoolerNode.apply(ps, h, bert.pooler.dense.weight)
+        st["layers"] = st["attn"] = None    # each layer's activations are saved tensors of its node(s) now, released with them
+        return h, pooled, (hidden if flags[0] else []), (maps if flags[2] else attn)
+
+    @contextlib.contextmanager
+    def _node_backward(self, st, grads):
+        """Around the backward of one layerwise node: the pass's dropout word bound (its masks regenerated) and unbound on the way
+        out, the node's side-queue weight gradients joined before it returns (a partial backward may run no later node), and,
+        when it writes parameter gradients, the flat buffer attached and the bf16 operands due a repack."""
+        ops.dropout_offset_bind(st["drop_word"])
+        sq = ops.SideQueue()
+        try:
+            if grads:
+                self._flat.attach_grads()
+            yield sq
+            if grads and not self._optimizer_emits_packed:
+                self._dirty = True
+        finally:
+            sq.join()
+            ops.dropout_offset_bind(None)
 
     def _backward_done(self):
         self._pending_backward = max(0, self._pending_backward - 1)
@@ -686,18 +892,9 @@ class _ClipBertHeadModel(nn.Module):
     def _backward_body(self, st, dout, grid_needs_grad):
         self._flat.attach_grads()
         dev = st["x_last"].device
-        cfg = self.config
-        H = _cfg(cfg, "hidden_size")
-        heads = _cfg(cfg, "num_attention_heads")
+        H = _cfg(self.config, "hidden_size")
         nseq, nvid, T, gh, gw, lt, L = st["dims"]
         M = nseq * L
-        p_h, p_a = st["p_h"], st["p_a"]
-        bf16, f32 = torch.bfloat16, torch.float32
-        n_ex, s2v, starts = st["repeat"]
-
-        def new(*shape, dtype=bf16):
-            return torch.empty(*shape, dtype=dtype, device=dev)
-
         ops.dropout_offset_bind(st.get("drop_word"))       # regenerate exactly this forward's masks
         cap = None if self._capture is None else self._capture.setdefault("bwd", {})
         sq = ops.SideQueue()                               # wgrad GEMMs / bias sums run beside the dgrad chain
@@ -708,14 +905,7 @@ class _ClipBertHeadModel(nn.Module):
             dpre = self._head_backward(st, dout, nseq, H)  # grad w.r.t. pooler pre-activation
         else:
             dpre, dseq, dhidden, dattn = self._base_output_grads(st, base, M, H)
-        pl = self._lin["pooler"]
-        x_last = st["x_last"]
-        if dpre is not None:
-            self._wgrad(pl, dpre, x_last, nseq, x_ld=L * H)
-            ops.colsum(dpre, pl.gb, nseq, H)
-        dx = torch.zeros(M, H, dtype=bf16, device=dev)
-        if dpre is not None:
-            self._dgrad(pl, dpre, nseq, dx, out_ld=L * H)  # scatters into the [CLS] rows
+        dx = self._pooler_backward(dpre, st["x_last"], nseq, L, H)
         extra = self._extra_sequence_grad(st) if base is None else dseq
         if cap is not None:      # clones where an add below writes the tensor in place
             cap.update(dpre=dpre, extra=extra, dx_pooler=dx.clone() if extra is not None or dhidden is not None else dx)
@@ -728,65 +918,8 @@ class _ClipBertHeadModel(nn.Module):
                 dx += dhidden[i + 1]
             if ret_hidden is not None:
                 _set_retained_hidden_grad(ret_hidden[i + 1], dx, nseq, L, H)
-            ly = st["layers"][i]
-            ls = ly["seed"]
-            qkv_l, ao_l, in_l, out_l = (self._lin["l%d.%s" % (i, k)] for k in ("qkv", "ao", "inter", "out"))
-            g1, _, dg1, db1 = self._ln("l%d.ln1" % i)
-            g2, _, dg2, db2 = self._ln("l%d.ln2" % i)
-            # y = LN2(s2), s2 = dropout(gel @ Wo^T + bo) + a
-            ds2 = new(M, H)
-            ds2d = new(M, H) if p_h > 0 else None
-            ops.layernorm_bwd(dx, ly["s2"], ly["st2"], g2, ds2, ds2d, dg2, db2, out_l.gb, p_h, ls + 3)
-            dd = ds2d if ds2d is not None else ds2
-            gmode = ops.group_wgrad      # the layer's four weight gradients as ONE launch (issued when the last dY, dqkv, exists) or two pairs
-            group = gmode in (1, 3, 4)
-            pairs = gmode == 4
-            wg = [self._wgrad_kw(out_l, dd, ly["gel"], M)]
-            if not group:
-                sq.run(lambda: ops.gemm(**wg[0]), dd, ly["gel"])
-            du = new(M, in_l.n)
-            self._dgrad(out_l, dd, M, du, aux=ly["u"], aux_ld=in_l.n, aux_mode=ops.AUX_MUL)
-            wg.append(self._wgrad_kw(in_l, du, ly["a"], M))
-            if pairs:
-                wg_ffn, wg = wg, []
-                sq.run(lambda: (ops.gemm_wgrad_group(wg_ffn), ops.colsum(du, in_l.gb, M, in_l.n)), dd, ly["gel"], du, ly["a"])
-            elif group:
-                sq.run(lambda: ops.colsum(du, in_l.gb, M, in_l.n), du)
-            else:
-                sq.run(lambda: (ops.gemm(**wg[1]), ops.colsum(du, in_l.gb, M, in_l.n)), du, ly["a"])
-            da = new(M, H)
-            self._dgrad(in_l, du, M, da, residual=ds2, res_ld=H)
-            # a = LN1(s1), s1 = dropout(ctx @ Wao^T + b) + x
-            ds1 = new(M, H)
-            ds1d = new(M, H) if p_h > 0 else None
-            ops.layernorm_bwd(da, ly["s1"], ly["st1"], g1, ds1, ds1d, dg1, db1, ao_l.gb, p_h, ls + 2)
-            dd1 = ds1d if ds1d is not None else ds1
-            wg.append(self._wgrad_kw(ao_l, dd1, ly["ctx"], M))
-            if not group:
-                sq.run(lambda: ops.gemm(**wg[2]), dd1, ly["ctx"])
-            dctx = new(M, H)
-            self._dgrad(ao_l, dd1, M, dctx)
-            dqkv = new(M, 3 * H)
-            ops.attention_bwd(ly["qkv"], st["mask"], ly["ctx"], dctx, ly["lse"], dqkv, nseq, L, lt, heads, p_a, ls + 1)
-            if dattn is not None and dattn[i] is not None:      # a loss on attentions[i]: its dQ / dK added into dqkv
-                drow = new(nseq, heads, L, dtype=f32)
-                if cap is not None:
-                    cap.setdefault("l%d" % i, {})["dqkv_attn"] = dqkv.clone()
-                ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn[i], drow, dqkv, nseq, L, lt, heads, p_a, ls + 1)
-            if ret_attn is not None and ret_attn[i] is not None:
-                _add_retained_attention_grad(ret_attn[i], ly["qkv"], dctx, nseq, L, heads)
-            wg.append(self._wgrad_kw(qkv_l, dqkv, ly["x"], M))
-            if group:
-                sq.run(lambda: (ops.gemm_wgrad_group(wg), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dd, ly["gel"], du, ly["a"], dd1, ly["ctx"], dqkv, ly["x"])
-            else:
-                sq.run(lambda: (ops.gemm(**wg[3]), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
-            dxn = new(M, H)
-            self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
-            if cap is not None:
-                c = cap.setdefault("l%d" % i, {})
-                c.update(dx=dx, ds2=ds2, ds2d=ds2d, du=du, da=da, ds1=ds1, ds1d=ds1d, dctx=dctx, dqkv=dqkv)
-                c.setdefault("dxn", dxn)
-            dx = dxn
+            dx = self._layer_backward(st, i, st["layers"][i], dx, sq, cap, None if dattn is None else dattn[i],
+                                      None if ret_attn is None else ret_attn[i])
             st["layers"][i] = None     # free this layer's stash
         if dhidden is not None and dhidden[0] is not None:                 # hidden_states[0] = the embedding output
             if cap is not None and len(st["layers"]):
@@ -794,15 +927,170 @@ class _ClipBertHeadModel(nn.Module):
             dx += dhidden[0]
         if ret_hidden is not None:
             _set_retained_hidden_grad(ret_hidden[0], dx, nseq, L, H)
-        # ---- embeddings ----
+        dgrid = self._embedding_backward(st, dx, grid_needs_grad)
+        sq.join()          # every weight gradient is in the flat buffer before the caller (all-reduce hook, optimizer) sees it
+        if cap is not None:
+            cap.update(dx_emb=dx, dgrid=dgrid)
+        if not self._optimizer_emits_packed:
+            self._dirty = True
+        return dgrid
+
+    def _pooler_backward(self, dpre, x_last, nseq, L, H, grads=True):
+        """d pooler pre-activation (None: no gradient) -> the gradient at the top of the encoder, [nseq * L, H] bf16 with the [CLS]
+        rows filled; grads: the pooler's weight and bias gradients into the flat buffer."""
+        pl = self._lin["pooler"]
+        if dpre is not None and grads:
+            self._wgrad(pl, dpre, x_last, nseq, x_ld=L * H)
+            ops.colsum(dpre, pl.gb, nseq, H)
+        dx = torch.zeros(nseq * L, H, dtype=torch.bfloat16, device=x_last.device)
+        if dpre is not None:
+            self._dgrad(pl, dpre, nseq, dx, out_ld=L * H)  # scatters into the [CLS] rows
+        return dx
+
+    def _layer_backward(self, st, i, ly, dx, sq, cap=None, dattn=None, ret_attn=None, grads=True, split=None):
+        """Encoder layer i from the gradient at its output dx ([nseq * L, H] bf16, not written) to the gradient at its input, with
+        the layer's stash ly; weight gradients on the side queue sq. dattn: a loss term on the layer's returned attention map,
+        ret_attn: the map when retained. grads = False: no parameter gradient is written (a backward that does not accumulate
+        into the parameters). split (the backward split at a differentiable map, ClipBertBaseModel.layerwise_autograd): stop at
+        the attention and return (d map = dO V^T, hand-over) - the hand-over (dqkv with its V block written, ds1) when split is
+        "with_map" (the map's node runs next and finishes the layer in _map_backward), None when it is "map_only"."""
+        dev = dx.device
+        H = _cfg(self.config, "hidden_size")
+        heads = _cfg(self.config, "num_attention_heads")
+        nseq, nvid, T, gh, gw, lt, L = st["dims"]
+        M = nseq * L
+        p_h, p_a = st["p_h"], st["p_a"]
+        bf16, f32 = torch.bfloat16, torch.float32
+
+        def new(*shape, dtype=bf16):
+            return torch.empty(*shape, dtype=dtype, device=dev)
+
+        ls = ly["seed"]
+        qkv_l, ao_l, in_l, out_l = (self._lin["l%d.%s" % (i, k)] for k in ("qkv", "ao", "inter", "out"))
+        g1, _, dg1, db1 = self._ln("l%d.ln1" % i)
+        g2, _, dg2, db2 = self._ln("l%d.ln2" % i)
+        dbo, dbao = out_l.gb, ao_l.gb
+        if not grads:
+            dg1 = db1 = dg2 = db2 = dbo = dbao = None
+        # y = LN2(s2), s2 = dropout(gel @ Wo^T + bo) + a
+        ds2 = new(M, H)
+        ds2d = new(M, H) if p_h > 0 else None
+        ops.layernorm_bwd(dx, ly["s2"], ly["st2"], g2, ds2, ds2d, dg2, db2, dbo, p_h, ls + 3)
+        dd = ds2d if ds2d is not None else ds2
+        gmode = ops.group_wgrad      # the layer's four weight gradients as ONE launch (issued when the last dY, dqkv, exists) or two pairs
+        group = gmode in (1, 3, 4)
+        pairs = gmode == 4
+        wg = [self._wgrad_kw(out_l, dd, ly["gel"], M)]
+        if grads and not group:
+            sq.run(lambda: ops.gemm(**wg[0]), dd, ly["gel"])
+        du = new(M, in_l.n)
+        self._dgrad(out_l, dd, M, du, aux=ly["u"], aux_ld=in_l.n, aux_mode=ops.AUX_MUL)
+        wg.append(self._wgrad_kw(in_l, du, ly["a"], M))
+        if not grads:
+            pass
+        elif pairs:
+            wg_ffn, wg = wg, []
+            sq.run(lambda: (ops.gemm_wgrad_group(wg_ffn), ops.colsum(du, in_l.gb, M, in_l.n)), dd, ly["gel"], du, ly["a"])
+        elif group:
+            sq.run(lambda: ops.colsum(du, in_l.gb, M, in_l.n), du)
+        else:
+            sq.run(lambda: (ops.gemm(**wg[1]), ops.colsum(du, in_l.gb, M, in_l.n)), du, ly["a"])
+        da = new(M, H)
+        self._dgrad(in_l, du, M, da, residual=ds2, res_ld=H)
+        # a = LN1(s1), s1 = dropout(ctx @ Wao^T + b) + x
+        ds1 = new(M, H)
+        ds1d = new(M, H) if p_h > 0 else None
+        ops.layernorm_bwd(da, ly["s1"], ly["st1"], g1, ds1, ds1d, dg1, db1, dbao, p_h, ls + 2)
+        dd1 = ds1d if ds1d is not None else ds1
+        wg.append(self._wgrad_kw(ao_l, dd1, ly["ctx"], M))
+        if grads and not group:
+            sq.run(lambda: ops.gemm(**wg[2]), dd1, ly["ctx"])
+        dctx = new(M, H)
+        self._dgrad(ao_l, dd1, M, dctx)
+        if split is not None:
+            if grads and group and wg:           # the weight gradients still pending here; the map's node issues the QKV one
+                sq.run(lambda: ops.gemm_wgrad_group(wg), dd, ly["gel"], du, ly["a"], dd1, ly["ctx"])
+            dmap = new(nseq, heads, L, L, dtype=f32)
+            ops.attention_dprobs(ly["qkv"], dctx, dmap, False, nseq, L, heads)
+            if split != "with_map":
+                return dmap, None
+            dqkv = new(M, 3 * H)
+            ops.attention_bwd_dv(ly["qkv"], st["mask"], ly["lse"], dctx, dqkv, nseq, L, lt, heads, p_a, ls + 1)
+            return dmap, (dqkv, ds1)
+        dqkv = new(M, 3 * H)
+        ops.attention_bwd(ly["qkv"], st["mask"], ly["ctx"], dctx, ly["lse"], dqkv, nseq, L, lt, heads, p_a, ls + 1)
+        if dattn is not None:      # a loss on attentions[i]: its dQ / dK added into dqkv
+            drow = new(nseq, heads, L, dtype=f32)
+            if cap is not None:
+                cap.setdefault("l%d" % i, {})["dqkv_attn"] = dqkv.clone()
+            ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn, drow, dqkv, nseq, L, lt, heads, p_a, ls + 1)
+        if ret_attn is not None:
+            _add_retained_attention_grad(ret_attn, ly["qkv"], dctx, nseq, L, heads)
+        wg.append(self._wgrad_kw(qkv_l, dqkv, ly["x"], M))
+        if not grads:
+            pass
+        elif group:
+            sq.run(lambda: (ops.gemm_wgrad_group(wg), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dd, ly["gel"], du, ly["a"], dd1, ly["ctx"], dqkv, ly["x"])
+        else:
+            sq.run(lambda: (ops.gemm(**wg[3]), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
+        dxn = new(M, H)
+        self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
+        if cap is not None:
+            c = cap.setdefault("l%d" % i, {})
+            c.update(dx=dx, ds2=ds2, ds2d=ds2d, du=du, da=da, ds1=ds1, ds1d=ds1d, dctx=dctx, dqkv=dqkv)
+            c.setdefault("dxn", dxn)
+        return dxn
+
+    def _map_backward(self, st, i, ly, G, handover, sq, grads=True):
+        """The rest of encoder layer i's backward from G, the full gradient of its attention map (fp32 [nseq, heads, L, L]), when
+        the backward is split at the map: dQ / dK written from G (cb_attention_probs_bwd_store), then the QKV weight gradient and
+        the dgrad to the layer input with the residual ds1. handover = (dqkv with its V block, ds1) from _layer_backward, or None
+        when the layer's output got no gradient (dV = 0, no residual)."""
+        H = _cfg(self.config, "hidden_size")
+        heads = _cfg(self.config, "num_attention_heads")
+        nseq, nvid, T, gh, gw, lt, L = st["dims"]
+        M = nseq * L
+        dev = G.device
+        qkv_l = self._lin["l%d.qkv" % i]
+        if handover is None:
+            dqkv, ds1 = torch.empty(M, 3 * H, dtype=torch.bfloat16, device=dev), None
+            dqkv[:, 2 * H:].zero_()
+        else:
+            dqkv, ds1 = handover
+        drow = torch.empty(nseq, heads, L, dtype=torch.float32, device=dev)
+        ops.attention_probs_bwd_store(ly["qkv"], st["mask"], ly["lse"], G, drow, dqkv, nseq, L, lt, heads, st["p_a"], ly["seed"] + 1)
+        if grads:
+            kw = self._wgrad_kw(qkv_l, dqkv, ly["x"], M)
+            sq.run(lambda: (ops.gemm(**kw), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
+        dxn = torch.empty(M, H, dtype=torch.bfloat16, device=dev)
+        if ds1 is None:
+            self._dgrad(qkv_l, dqkv, M, dxn)
+        else:
+            self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
+        return dxn
+
+    def _embedding_backward(self, st, dx, grid_needs_grad, grads=True):
+        """The text and visual embeddings from the gradient at their output dx; returns d visual_inputs (None unless
+        grid_needs_grad). grads = False: no parameter gradient is written (the visual kernel's go to scratch)."""
+        dev = dx.device
+        H = _cfg(self.config, "hidden_size")
+        nseq, nvid, T, gh, gw, lt, L = st["dims"]
+        p_h = st["p_h"]
+        bf16 = torch.bfloat16
+        n_ex, s2v, starts = st["repeat"]
         g_t, _, dg_t, db_t = self._ln("emb.ln")
         g_v, _, dg_v, db_v = self._ln("vis.ln")
         (word, dword), (pos, dpos), (typ, dtyp) = self._emb("emb.word"), self._emb("emb.pos"), self._emb("emb.type")
-        ops.embed_text_bwd(dx, st["ids"], word, pos, typ, g_t, st["stats_t"], dword, dpos, dtyp, dg_t, db_t, nseq, lt, L, p_h,
-                           st["seed"] + 1)
+        if grads:
+            ops.embed_text_bwd(dx, st["ids"], word, pos, typ, g_t, st["stats_t"], dword, dpos, dtyp, dg_t, db_t, nseq, lt, L, p_h,
+                               st["seed"] + 1)
         (row, drow), (col, dcol), (vtyp, dvtyp) = self._emb("vis.row"), self._emb("vis.col"), self._emb("vis.type")
-        dv_tmp = new(nseq * gh * gw, H, dtype=f32)
-        dgrid = new(nvid, T, gh, gw, H) if grid_needs_grad else None
+        if not grads:
+            if not grid_needs_grad:
+                return None
+            drow, dcol, dvtyp, dg_v, db_v = (torch.zeros_like(t) for t in (drow, dcol, dvtyp, dg_v, db_v))
+        dv_tmp = torch.empty(nseq * gh * gw, H, dtype=torch.float32, device=dev)
+        dgrid = torch.empty(nvid, T, gh, gw, H, dtype=bf16, device=dev) if grid_needs_grad else None
         sample = st.get("sample")
         if sample is None:
             ops.embed_visual_bwd(dx, st["grid"], s2v, starts, n_ex, row, col, vtyp, g_v, st["stats_v"], dv_tmp, dgrid, drow, dcol, dvtyp,
@@ -813,17 +1101,13 @@ class _ClipBertHeadModel(nn.Module):
             drow_s, dcol_s = torch.zeros_like(row_s), torch.zeros_like(col_s)
             ops.embed_visual_bwd(dx, st["grid"], s2v, starts, n_ex, row_s, col_s, vtyp, g_v, st["stats_v"], dv_tmp, dgrid, drow_s, dcol_s,
                                  dvtyp, dg_v, db_v, nseq, nvid, T, gh, gw, lt, L, p_h, st["seed"] + 2)
-            drow.index_add_(0, idx // gw0, drow_s)         # d(row[r] + col[c]) goes to both tables
-            dcol.index_add_(0, idx % gw0, drow_s)
+            if grads:
+                drow.index_add_(0, idx // gw0, drow_s)         # d(row[r] + col[c]) goes to both tables
+                dcol.index_add_(0, idx % gw0, drow_s)
             if dgrid is not None:
                 full = torch.zeros(nvid, T, gh0 * gw0, H, dtype=bf16, device=dev)
                 full.index_copy_(2, idx, dgrid.view(nvid, T, gh, H))
                 dgrid = full.view(nvid, T, gh0, gw0, H)
-        sq.join()          # every weight gradient is in the flat buffer before the caller (all-reduce hook, optimizer) sees it
-        if cap is not None:
-            cap.update(dx_emb=dx, dgrid=dgrid)
-        if not self._optimizer_emits_packed:
-            self._dirty = True
         return dgrid
 
     def _extra_sequence_grad(self, st):
@@ -840,10 +1124,7 @@ class _ClipBertHeadModel(nn.Module):
         def dense(g):
             return None if g is None else g.reshape(M, H).to(bf16).contiguous()
 
-        dpre = None
-        if dpooled is not None:
-            pooled = st["pooled"].float()
-            dpre = (dpooled.float() * (1.0 - pooled * pooled)).to(bf16)
+        dpre = None if dpooled is None else _pooler_pre_grad(st["pooled"], dpooled)
         dattn = None
         if any(g is not None for g in da):
             dattn = [None if g is None else g.to(torch.float32).contiguous() for g in da]
@@ -855,6 +1136,12 @@ class _ClipBertHeadModel(nn.Module):
             self._flat.zero_grad()
         else:
             super().zero_grad(set_to_none=set_to_none)
+
+
+def _pooler_pre_grad(pooled, dpooled):
+    """d pooler pre-activation (bf16) = d pooled * tanh' = d pooled (1 - pooled^2), as one product on the (B', 768) rows."""
+    p = pooled.float()
+    return (dpooled.float() * (1.0 - p * p)).to(torch.bfloat16)
 
 
 def _set_retained_hidden_grad(tensors, dx, nseq, L, H):

@@ -42,6 +42,8 @@ _SIGS = {
     "cb_attention_probs": [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_attention_probs_bwd": [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_attention_dprobs": [_vp, _i64, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp],
+    "cb_attention_probs_bwd_store": [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
+    "cb_attention_bwd_dv": [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _f, _u64, _vp],
     "cb_stem_im2col": [_vp, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp],
     "cb_maxpool3x3s2": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool3x3s2_strided": [_vp, _vp, _i, _i, _i, _i, _i64, _i64, _vp],
@@ -614,6 +616,20 @@ def attention_probs_bwd(qkv, text_mask, lse, dprobs, drow, dqkv, nseq, l, lt, he
     assert dprobs.dtype == torch.float32 and dprobs.is_contiguous() and dprobs.numel() == nseq * heads * l * l
     assert drow.dtype == torch.float32 and drow.numel() >= nseq * heads * l
     _call("cb_attention_probs_bwd", _p(qkv), qkv.shape[1], _p(text_mask), _p(lse), _p(dprobs), _p(drow), _p(dqkv), dqkv.shape[1],
+          nseq, l, lt, heads, 64, p, seed, _s())
+
+
+def attention_probs_bwd_store(qkv, text_mask, lse, dprobs, drow, dqkv, nseq, l, lt, heads, p, seed):
+    """attention_probs_bwd with dQ / dK written to dqkv's Q and K blocks instead of added (their old contents are never read)."""
+    assert dprobs.dtype == torch.float32 and dprobs.is_contiguous() and dprobs.numel() == nseq * heads * l * l
+    assert drow.dtype == torch.float32 and drow.numel() >= nseq * heads * l
+    _call("cb_attention_probs_bwd_store", _p(qkv), qkv.shape[1], _p(text_mask), _p(lse), _p(dprobs), _p(drow), _p(dqkv),
+          dqkv.shape[1], nseq, l, lt, heads, 64, p, seed, _s())
+
+
+def attention_bwd_dv(qkv, text_mask, lse, dctx, dqkv, nseq, l, lt, heads, p, seed):
+    """dV = (P r)^T dO per head, written to dqkv's V block (Q and K blocks untouched), P rebuilt from qkv, the mask and lse."""
+    _call("cb_attention_bwd_dv", _p(qkv), qkv.shape[1], _p(text_mask), _p(lse), _p(dctx), dctx.shape[1], _p(dqkv), dqkv.shape[1],
           nseq, l, lt, heads, 64, p, seed, _s())
 
 

@@ -330,6 +330,26 @@ int cb_attention_probs(const void* qkv, int64_t ld_qkv, const int64_t* text_mask
 int cb_attention_probs_bwd(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const float* dprobs,
                            float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
                            float dropout_p, uint64_t seed, void* stream);
+/* cb_attention_probs_bwd with dQ and dK WRITTEN to the Q and K column blocks (dQ_i = sum_j dS_ij K_j / 8, dK_j = sum_i dS_ij
+ * Q_i / 8, each rounded to bf16 once) instead of added: for a dqkv whose Q and K blocks hold nothing yet, the backward split at a
+ * differentiable attention map (ClipBertBaseModel.layerwise_autograd), where G is the map's full gradient. Nothing is read from
+ * dqkv; the V block, the pitch padding and everything outside the window are not touched. Same arguments, checks, rounding and
+ * kernels (their store instantiations). */
+int cb_attention_probs_bwd_store(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse,
+                                 const float* dprobs, float* drow, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt,
+                                 int heads, int head_dim, float dropout_p, uint64_t seed, void* stream);
+/* The value gradient of the attention backward alone, for the same split: with dO = dctx [nseq * l, >= heads * 64] bf16 (row
+ * pitch ld_ctx) and P rebuilt from qkv, the mask and lse as cb_attention_probs forms it (same seed, same bound device word,
+ * dropout multipliers r),
+ *   dV_j = sum_i P_ij r_ij dO_i       per (sequence, head), every j < l
+ * WRITTEN to the V column block of dqkv (bf16, rounded once); the Q and K blocks, the pitch padding and everything outside the
+ * window are not touched. P r is rounded to bf16 before the product, as cb_attention_bwd does. Tensor cores (mma.sync), one CTA
+ * per (64-key tile, head, sequence), one writer per element: no atomics, bit-identical from run to run. Arguments are checked as
+ * for cb_attention_bwd (pitches multiples of 8 holding Q | K | V and heads x 64; qkv, dctx, dqkv 16-byte aligned); nothing is
+ * launched otherwise. */
+int cb_attention_bwd_dv(const void* qkv, int64_t ld_qkv, const int64_t* text_mask, const float* lse, const void* dctx,
+                        int64_t ld_ctx, void* dqkv, int64_t ld_dqkv, int nseq, int l, int lt, int heads, int head_dim,
+                        float dropout_p, uint64_t seed, void* stream);
 /* The gradient the returned probabilities A receive from the context product ctx = A V (transformers.py:271-277), for
  * retain_grad() on the attentions: dctx [nseq * l, >= heads * 64] bf16 with row pitch ld_ctx (d loss / d context), V the third
  * column block of qkv;
