@@ -2,6 +2,8 @@
 // src/modeling/grid_feat.py:89-105 -> detectron2 BasicStem / BottleneckBlock / MaxPool, and the
 // grid_encoder MaxPool2d+ReLU at grid_feat.py:43-48). Activations are NHWC bf16; every thread moves
 // 8 channels with one 128-bit access. All convolution FLOPs run in gemm.cu (wgmma).
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 #include "host_util.h"
 
@@ -498,6 +500,148 @@ __global__ void unsubsample2_mask_kernel(const __nv_bfloat16* __restrict__ dsub,
   *reinterpret_cast<uint4*>(dx + pix * C + c8 * 8) = o;
 }
 
+// the mask-free form of the above (act == NULL): dx[n,y,x] = (y,x even ? dsub[n,y/2,x/2] : 0). A kernel of its own so that the
+// masked one keeps its instructions.
+__global__ void unsubsample2_kernel(const __nv_bfloat16* __restrict__ dsub, __nv_bfloat16* __restrict__ dx, int N, int H, int W,
+                                    int C, int Ho, int Wo) {
+  pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
+  pdl_trigger();
+  const int c8n = C / 8;
+  const int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= static_cast<int64_t>(N) * H * W * c8n) return;
+  const int c8 = static_cast<int>(t % c8n);
+  const int64_t pix = t / c8n;
+  const int xx = static_cast<int>(pix % W), yy = static_cast<int>((pix / W) % H);
+  const int n = static_cast<int>(pix / (static_cast<int64_t>(W) * H));
+  uint4 o = make_uint4(0, 0, 0, 0);
+  if ((yy & 1) == 0 && (xx & 1) == 0)
+    o = *reinterpret_cast<const uint4*>(dsub + ((static_cast<int64_t>(n) * Ho + yy / 2) * Wo + xx / 2) * C + c8 * 8);
+  *reinterpret_cast<uint4*>(dx + pix * C + c8 * 8) = o;
+}
+
+// ---- cb_nhwc_intake: a strided (n, c, h, w) tensor into the engine's NHWC bf16 layout, optionally masked by (act > 0) ----
+template <typename T>
+__device__ __forceinline__ float intake_ld(const T* p);
+template <>
+__device__ __forceinline__ float intake_ld<float>(const float* p) { return __ldg(p); }
+template <>
+__device__ __forceinline__ float intake_ld<__half>(const __half* p) { return __half2float(__ldg(p)); }
+template <>
+__device__ __forceinline__ float intake_ld<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+
+// 8 contiguous channels as fp32
+__device__ __forceinline__ void intake_ld8(const float* p, float (&v)[8]) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+__device__ __forceinline__ void intake_ld8(const __nv_bfloat16* p, float (&v)[8]) { unpack8(__ldg(reinterpret_cast<const uint4*>(p)), v); }
+__device__ __forceinline__ void intake_ld8(const __half* p, float (&v)[8]) {
+  const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+  const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 f = __half22float2(h2[j]);
+    v[2 * j] = f.x;
+    v[2 * j + 1] = f.y;
+  }
+}
+
+// the engine row of pixel (n, y, x): compact, or the interior of the zero-bordered [n, h+2, w+2] grid
+__device__ __forceinline__ int64_t intake_row(int64_t pix, int H, int W, bool bordered) {
+  if (!bordered) return pix;
+  const int64_t xx = pix % W, r = pix / W;
+  const int64_t yy = r % H, n = r / H;
+  return (n * (H + 2) + yy + 1) * (W + 2) + xx + 1;
+}
+
+// 8 channels of one pixel: mask (act > 0 ? v : +0), one rounding to bf16, one 16-byte store
+__device__ __forceinline__ void intake_store8(float (&v)[8], const __nv_bfloat16* __restrict__ act, bool act_bordered,
+                                              __nv_bfloat16* __restrict__ out, bool out_bordered, int64_t pix, int c, int H, int W,
+                                              int C) {
+  if (act != nullptr) {
+    float a[8];
+    unpack8(__ldg(reinterpret_cast<const uint4*>(act + intake_row(pix, H, W, act_bordered) * C + c)), a);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = a[j] > 0.f ? v[j] : 0.f;
+  }
+  *reinterpret_cast<uint4*>(out + intake_row(pix, H, W, out_bordered) * C + c) = pack8(v);
+}
+
+// one thread per (pixel, 8 channels). kVec: the 8 channels are contiguous and 16-byte aligned (channels-last input)
+template <typename T, bool kVec>
+__global__ void nhwc_intake_kernel(const T* __restrict__ x, int64_t sn, int64_t sc, int64_t sh, int64_t sw,
+                                   const __nv_bfloat16* __restrict__ act, int act_bordered, __nv_bfloat16* __restrict__ out,
+                                   int out_bordered, int N, int C, int H, int W) {
+  pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
+  pdl_trigger();
+  const int c8n = C / 8;
+  const int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= static_cast<int64_t>(N) * H * W * c8n) return;
+  const int c = static_cast<int>(t % c8n) * 8;
+  const int64_t pix = t / c8n;
+  const int64_t xx = pix % W, yy = (pix / W) % H, n = pix / (static_cast<int64_t>(W) * H);
+  const T* p = x + n * sn + yy * sh + xx * sw + c * sc;
+  float v[8];
+  if (kVec) {
+    intake_ld8(p, v);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = intake_ld(p + j * sc);
+  }
+  intake_store8(v, act, act_bordered, out, out_bordered, pix, c, H, W, C);
+}
+
+// contiguous NCHW planes (sw = 1, sh = w, sc = h * w): a 32-channel x 64-pixel tile through shared memory, so that the loads run
+// along pixels and the 16-byte stores along channels
+constexpr int kIntakeTileP = 64, kIntakeTileC = 32;
+template <typename T>
+__global__ void __launch_bounds__(256) nhwc_intake_nchw_kernel(const T* __restrict__ x, int64_t sn, const __nv_bfloat16* __restrict__ act,
+                                                               int act_bordered, __nv_bfloat16* __restrict__ out, int out_bordered, int C,
+                                                               int H, int W) {
+  __shared__ float tile[kIntakeTileC][kIntakeTileP + 1];
+  pdl_wait();      // PDL: everything above ran while the previous kernel drained; no global access before this
+  pdl_trigger();
+  const int64_t hw = static_cast<int64_t>(H) * W;
+  const int64_t p0 = static_cast<int64_t>(blockIdx.x) * kIntakeTileP;
+  const int c0 = blockIdx.y * kIntakeTileC, n = blockIdx.z;
+  const int tp = threadIdx.x % kIntakeTileP, tc = threadIdx.x / kIntakeTileP;     // 64 pixels x 4 channel rows per pass
+  const T* xn = x + n * sn;
+#pragma unroll
+  for (int j = 0; j < kIntakeTileC / 4; ++j) {
+    const int c = c0 + tc + 4 * j;
+    const int64_t p = p0 + tp;
+    tile[tc + 4 * j][tp] = (c < C && p < hw) ? intake_ld(xn + c * hw + p) : 0.f;
+  }
+  __syncthreads();
+  const int op = threadIdx.x / 4, oc = (threadIdx.x % 4) * 8;      // each thread: one pixel, 8 channels
+  const int64_t p = p0 + op;
+  if (p < hw && c0 + oc < C) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = tile[oc + j][op];
+    intake_store8(v, act, act_bordered, out, out_bordered, n * hw + p, c0 + oc, H, W, C);
+  }
+}
+
+template <typename T>
+static void launch_intake(const void* xv, int64_t sn, int64_t sc, int64_t sh, int64_t sw, const __nv_bfloat16* act, int act_bordered,
+                          __nv_bfloat16* out, int out_bordered, int n, int c, int h, int w, cudaStream_t st) {
+  const T* x = static_cast<const T*>(xv);
+  const bool aligned = (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  if (sc == 1 && aligned && sn % 8 == 0 && sh % 8 == 0 && sw % 8 == 0) {
+    const int64_t total = static_cast<int64_t>(n) * h * w * (c / 8);
+    launch_k(nhwc_intake_kernel<T, true>, ceil_div(total, 256), 256, 0, st, x, sn, sc, sh, sw, act, act_bordered, out, out_bordered, n, c,
+             h, w);
+  } else if (sw == 1 && sh == w && sc == static_cast<int64_t>(h) * w && n <= 65535) {
+    const dim3 grid(static_cast<unsigned>(ceil_div(static_cast<int64_t>(h) * w, kIntakeTileP)), ceil_div(c, kIntakeTileC), n);
+    launch_k(nhwc_intake_nchw_kernel<T>, grid, 256, 0, st, x, sn, act, act_bordered, out, out_bordered, c, h, w);
+  } else {
+    const int64_t total = static_cast<int64_t>(n) * h * w * (c / 8);
+    launch_k(nhwc_intake_kernel<T, false>, ceil_div(total, 256), 256, 0, st, x, sn, sc, sh, sw, act, act_bordered, out, out_bordered, n,
+             c, h, w);
+  }
+}
+
 // grid_encoder tail: MaxPool2d(2,2) (floor) then ReLU, NHWC compact -> NHWC compact
 __global__ void maxpool2x2_relu_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H,
                                            int W, int C, int Ho, int Wo) {
@@ -726,13 +870,39 @@ int cb_subsample2(const void* x, void* y, int n, int h, int w, int c, void* stre
 
 /* dsub: [n, ho, wo, c]; act, dx: [n, h, w, c] */
 int cb_unsubsample2_mask(const void* dsub, const void* act, void* dx, int n, int h, int w, int c, void* stream) {
-  CB_REQUIRE(dsub && act && dx && n > 0 && h > 0 && w > 0 && c > 0 && c % 8 == 0, "cb_unsubsample2_mask: bad arguments");
+  CB_REQUIRE(dsub && dx && n > 0 && h > 0 && w > 0 && c > 0 && c % 8 == 0, "cb_unsubsample2_mask: bad arguments");
   const int ho = (h - 1) / 2 + 1, wo = (w - 1) / 2 + 1;
   const int64_t total = static_cast<int64_t>(n) * h * w * (c / 8);
-  launch_k(unsubsample2_mask_kernel, ceil_div(total, 256), 256, 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const __nv_bfloat16*>(dsub), static_cast<const __nv_bfloat16*>(act), static_cast<__nv_bfloat16*>(dx), n, h, w, c,
-      ho, wo);
+  if (act == nullptr)
+    launch_k(unsubsample2_kernel, ceil_div(total, 256), 256, 0, static_cast<cudaStream_t>(stream), static_cast<const __nv_bfloat16*>(dsub),
+             static_cast<__nv_bfloat16*>(dx), n, h, w, c, ho, wo);
+  else
+    launch_k(unsubsample2_mask_kernel, ceil_div(total, 256), 256, 0, static_cast<cudaStream_t>(stream),
+        static_cast<const __nv_bfloat16*>(dsub), static_cast<const __nv_bfloat16*>(act), static_cast<__nv_bfloat16*>(dx), n, h, w, c,
+        ho, wo);
   return check_launch("cb_unsubsample2_mask");
+}
+
+int cb_nhwc_intake(const void* x, int in_dtype, int64_t sn, int64_t sc, int64_t sh, int64_t sw, int n, int c, int h, int w, const void* act,
+                   int act_bordered, void* out, int out_bordered, void* stream) {
+  CB_REQUIRE(x && out && n > 0 && c > 0 && h > 0 && w > 0 && c % 8 == 0, "cb_nhwc_intake: bad arguments (c must be a multiple of 8)");
+  CB_REQUIRE(sn >= 0 && sc >= 0 && sh >= 0 && sw >= 0, "cb_nhwc_intake: negative stride");
+  CB_REQUIRE((act_bordered == 0 || act_bordered == 1) && (out_bordered == 0 || out_bordered == 1),
+             "cb_nhwc_intake: act_bordered and out_bordered must be 0 or 1");
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(act) & 15) == 0,
+             "cb_nhwc_intake: out and act must be 16-byte aligned");
+  const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(act);
+  __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (in_dtype == 0)
+    launch_intake<float>(x, sn, sc, sh, sw, a, act_bordered, o, out_bordered, n, c, h, w, st);
+  else if (in_dtype == 2)
+    launch_intake<__nv_bfloat16>(x, sn, sc, sh, sw, a, act_bordered, o, out_bordered, n, c, h, w, st);
+  else if (in_dtype == 3)
+    launch_intake<__half>(x, sn, sc, sh, sw, a, act_bordered, o, out_bordered, n, c, h, w, st);
+  else
+    CB_REQUIRE(false, "cb_nhwc_intake: in_dtype must be 0 (fp32), 2 (bf16) or 3 (fp16)");
+  return check_launch("cb_nhwc_intake");
 }
 
 int cb_maxpool2x2_relu_fwd(const void* x, void* y, int n, int h, int w, int c, void* stream) {

@@ -58,6 +58,7 @@ _SIGS = {
     "cb_maxpool2x2_relu_fwd": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool2x2_relu_bwd": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "cb_relu_mask": [_vp, _vp, _vp, _i64, _vp],
+    "cb_nhwc_intake": [_vp, _i, _i64, _i64, _i64, _i64, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp],
     # deterministic variants: the arguments of the plain entry point, then (scratch, scratch_bytes) before the stream
     "cb_layernorm_bwd_det": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _u64, _vp, _i64, _vp],
     "cb_embed_text_bwd_det": [_vp] * 12 + [_i, _i, _i, _i, _i, _f, _u64, _vp, _i64, _vp],
@@ -698,6 +699,7 @@ def subsample2(x, y, n, h, w, c):
 
 
 def unsubsample2_mask(dsub, act, dx, n, h, w, c):
+    """act None: the mask-free scatter (the gradient's mask is applied by the block that produced x)."""
     _call("cb_unsubsample2_mask", _p(dsub), _p(act), _p(dx), n, h, w, c, _s())
 
 
@@ -711,3 +713,21 @@ def maxpool2x2_relu_bwd(dy, x, dx_pad, n, h, w, c):
 
 def relu_mask(dy, act, dx):
     _call("cb_relu_mask", _p(dy), _p(act), _p(dx), dy.numel(), _s())
+
+
+INTAKE_DTYPES = {torch.float32: 0, torch.bfloat16: 2, torch.float16: 3}
+
+
+def nhwc_intake(x, out, act=None, out_bordered=False, act_bordered=False):
+    """cb_nhwc_intake: x (n, c, h, w), any strides, fp32 / bf16 / fp16 -> out, bf16 NHWC compact [n*h*w, c] or (out_bordered) the
+    interior of a zero-bordered [n*(h+2)*(w+2), c]; act (bf16 NHWC, compact or act_bordered): out = (act > 0) ? x : +0."""
+    if x.dtype not in INTAKE_DTYPES:
+        raise TypeError("nhwc_intake: dtype %s is not fp32, bf16 or fp16" % x.dtype)
+    n, c, h, w = x.shape
+    rows = n * (h + 2) * (w + 2) if out_bordered else n * h * w
+    assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() == rows * c and x.device == out.device
+    if act is not None:
+        arows = n * (h + 2) * (w + 2) if act_bordered else n * h * w
+        assert act.dtype == torch.bfloat16 and act.is_contiguous() and act.numel() == arows * c and act.device == out.device
+    _call("cb_nhwc_intake", _p(x), INTAKE_DTYPES[x.dtype], *x.stride(), n, c, h, w, _p(act), int(bool(act_bordered)), _p(out),
+          int(bool(out_bordered)), _s())

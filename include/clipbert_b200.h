@@ -423,7 +423,9 @@ int cb_cast_scale_segments(const float* master, void* packed, const int64_t* seg
  *                           included: the mean subtraction has unit derivative). mma.sync m16n8k16, fp32 accumulation in a fixed
  *                           order, one writer per element: the same bits on every run.
  *   cb_subsample2           input of a stride-2 1x1 conv (res3/4/5 block 0 conv1 + shortcut)
- *   cb_unsubsample2_mask    its backward fused with the ReLU mask of the producing block
+ *   cb_unsubsample2_mask    its backward fused with the ReLU mask of the producing block; act = NULL: the mask-free scatter
+ *                           (dx = dsub at even pixels, +0 elsewhere), for a gradient whose mask the producing block applies
+ *                           itself (cb_nhwc_intake)
  *   cb_maxpool2x2_relu_fwd  grid_encoder MaxPool2d(2,2) + ReLU (7x7 -> 3x3 at 224 px, 14x14 -> 7x7 at 448)
  *   cb_maxpool2x2_relu_bwd  its backward, written into the zero-bordered layout read by the 3x3 dgrad/wgrad
  *   cb_relu_mask            dx = dy * (act > 0)
@@ -462,6 +464,17 @@ int cb_unsubsample2_mask(const void* dsub, const void* act, void* dx, int n, int
 int cb_maxpool2x2_relu_fwd(const void* x, void* y, int n, int h, int w, int c, void* stream);
 int cb_maxpool2x2_relu_bwd(const void* dy, const void* x, void* dx_pad, int n, int h, int w, int c, void* stream);
 int cb_relu_mask(const void* dy, const void* act, void* dx, int64_t n, void* stream);
+/* A strided 4-D tensor into the engine's NHWC bf16 layout: out[pixel (n, y, x), ch] = bf16(x[n, ch, y, x]), element (n, ch, y, x)
+ * of x at element offset n*sn + ch*sc + y*sh + x*sw (any non-negative strides: channels-last, contiguous NCHW, permuted, sliced
+ * or expanded views); in_dtype 0 = fp32, 2 = bf16, 3 = fp16. out is compact [n*h*w, c] (out_bordered = 0) or the interior of a
+ * zero-bordered [n, h+2, w+2, c] (out_bordered = 1: border rows are never written). act != NULL: out = (act > 0) ? bf16(x) : +0,
+ * with act bf16 NHWC [n, h, w, c] in the same two layouts (act_bordered): the ReLU' of the block whose output gradient x is,
+ * applied where it enters the block's backward (GridFeatBackbone's module path; a NaN passes where act > 0). One rounding,
+ * one writer per element, no atomics: the same bits on every run. c % 8 == 0; out and act 16-byte aligned. Channels-last x
+ * (sc = 1, 16-byte aligned 8-channel groups) takes 16-byte loads, contiguous NCHW planes a shared-memory transpose, anything
+ * else a generic gather. Bound by HBM: x and act read once, out written once. */
+int cb_nhwc_intake(const void* x, int in_dtype, int64_t sn, int64_t sc, int64_t sh, int64_t sw, int n, int c, int h, int w, const void* act,
+                   int act_bordered, void* out, int out_bordered, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Clip-level score aggregation + loss of the training loops, pool_method "lse"
