@@ -249,7 +249,10 @@ __global__ void __launch_bounds__(128) ln_bwd_kernel(const __nv_bfloat16* __rest
 
 // ------------------------------------------------------------------------------------------------
 // Text embeddings: out[b*L + t] = dropout(LN(word[id] + pos[t] + type[0]))   (t < Lt)
+// VEC: the word vectors come from the caller, row r = b * Lt + t at word + r * vocab (vocab is then the row pitch in floats, ids
+// is not read): the forward of a hooked word_embeddings. The VEC = false instantiation is the kernel of before.
 // ------------------------------------------------------------------------------------------------
+template <bool VEC>
 __global__ void __launch_bounds__(128) embed_text_fwd_kernel(const int64_t* __restrict__ ids, const float* word,
                                                              const float* pos, const float* type0,
                                                              const float* gamma, const float* beta,
@@ -262,10 +265,14 @@ __global__ void __launch_bounds__(128) embed_text_fwd_kernel(const int64_t* __re
   const int64_t r = static_cast<int64_t>(blockIdx.x) * ROWS_PER_BLOCK + warp;
   if (r >= static_cast<int64_t>(nseq) * Lt) return;
   const int b = static_cast<int>(r / Lt), t = static_cast<int>(r - static_cast<int64_t>(b) * Lt);
-  int64_t id = ids[r];
-  id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
   float v[CH][8], p[CH][8], ty[CH][8];
-  load_row_f32(word + id * HID, lane, v);
+  if constexpr (VEC) {
+    load_row_f32(word + r * vocab, lane, v);
+  } else {
+    int64_t id = ids[r];
+    id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
+    load_row_f32(word + id * HID, lane, v);
+  }
   load_row_f32(pos + static_cast<int64_t>(t) * HID, lane, p);
   load_row_f32(type0, lane, ty);
 #pragma unroll
@@ -288,7 +295,9 @@ __global__ void __launch_bounds__(128) embed_text_fwd_kernel(const int64_t* __re
 // Lt rows of dpos made this kernel 82 us at 64 sequences); the word rows go out as 16-byte reductions.
 // DET: the parameter partials go to scratch (slots dgamma, dbeta, d type/pos) and row r's word gradient to drows[r] (fp32), which
 // word_scatter_ordered_kernel adds into the table afterwards.
-template <bool DET>
+// VEC: the forward's word vectors came from the caller (see embed_text_fwd_kernel; e is read from word + r * vocab) and row r's
+// gradient is the output: stored to drows[r], as DET stores it, never added into a table.
+template <bool DET, bool VEC>
 __global__ void __launch_bounds__(128) embed_text_bwd_kernel(const __nv_bfloat16* __restrict__ dh,
                                                              const int64_t* __restrict__ ids, const float* word,
                                                              const float* pos, const float* type0, const float* gamma,
@@ -315,13 +324,16 @@ __global__ void __launch_bounds__(128) embed_text_bwd_kernel(const __nv_bfloat16
     }
   for (int b = blockIdx.x * ROWS_PER_BLOCK + warp; b < nseq; b += gridDim.x * ROWS_PER_BLOCK) {
     const int64_t r = static_cast<int64_t>(b) * Lt + t;
-    int64_t id = ids[r];
-    id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
+    int64_t id = 0;
+    if constexpr (!VEC) {
+      id = ids[r];
+      id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
+    }
     const int64_t orow = static_cast<int64_t>(b) * L + t;
     float g[CH][8], e[CH][8];
     load_row_bf16(dh + orow * HID, lane, g);
     apply_dropout_row(g, dc, orow, lane);
-    load_row_f32(word + id * HID, lane, e);
+    load_row_f32(VEC ? word + r * vocab : word + id * HID, lane, e);
 #pragma unroll
     for (int c = 0; c < CH; ++c)
 #pragma unroll
@@ -342,13 +354,13 @@ __global__ void __launch_bounds__(128) embed_text_bwd_kernel(const __nv_bfloat16
         ag[c][j] += gsave[c][j] * e[c][j];
         at[c][j] += g[c][j];
       }
-      if constexpr (!DET) {
+      if constexpr (!DET && !VEC) {
         float* wrow = dword + id * HID + c * 256 + lane * 8;
         red_add_f32x4(wrow, make_float4(g[c][0], g[c][1], g[c][2], g[c][3]));
         red_add_f32x4(wrow + 4, make_float4(g[c][4], g[c][5], g[c][6], g[c][7]));
       }
     }
-    if constexpr (DET) store_row_f32(drows + r * HID, lane, g);
+    if constexpr (DET || VEC) store_row_f32(drows + r * HID, lane, g);
   }
   if constexpr (DET) {      // one partial of d type[0] serves d type[0] and d pos[t] (see ordered reduction in cb_embed_text_bwd_det)
     block_store(ag, red, part_row(part, 0), warp, lane);
@@ -865,7 +877,7 @@ int cb_embed_text_fwd(const int64_t* ids, const float* word, const float* pos, c
                       float eps, float dropout_p, uint64_t seed, void* stream) {
   CB_REQUIRE(hidden == HID, "cb_embed_text_fwd: hidden size %d unsupported", hidden);
   CB_REQUIRE(ids && word && pos && type0 && out && stats && nseq > 0 && lt > 0 && l >= lt, "cb_embed_text_fwd: bad arguments");
-  launch_k(embed_text_fwd_kernel, ceil_div(static_cast<int64_t>(nseq) * lt, ROWS_PER_BLOCK), 128, 0, static_cast<cudaStream_t>(stream), 
+  launch_k(embed_text_fwd_kernel<false>, ceil_div(static_cast<int64_t>(nseq) * lt, ROWS_PER_BLOCK), 128, 0, static_cast<cudaStream_t>(stream), 
       ids, word, pos, type0, gamma, beta, static_cast<__nv_bfloat16*>(out), stats, nseq, lt, l, vocab, eps,
       make_drop(dropout_p, seed));
   return check_launch("cb_embed_text_fwd");
@@ -880,7 +892,7 @@ int cb_embed_text_bwd(const void* dh, const int64_t* ids, const float* word, con
   CB_REQUIRE(nseq > 0 && lt > 0 && lt <= 65535, "cb_embed_text_bwd: bad sizes");
   CB_REQUIRE_NONDET("cb_embed_text_bwd");
   const int per_pos = embed_bwd_per_pos(nseq);      // two (up to five at 640 sequences) rows per warp
-  launch_k(embed_text_bwd_kernel<false>, dim3(per_pos, lt), 128, 0, static_cast<cudaStream_t>(stream), 
+  launch_k(embed_text_bwd_kernel<false, false>, dim3(per_pos, lt), 128, 0, static_cast<cudaStream_t>(stream), 
       static_cast<const __nv_bfloat16*>(dh), ids, word, pos, type0, gamma, stats, dword, dpos, dtype0, dgamma, dbeta,
       nseq, lt, l, vocab, make_drop(dropout_p, seed), static_cast<float*>(nullptr), static_cast<float*>(nullptr));
   return check_launch("cb_embed_text_bwd");
@@ -903,7 +915,7 @@ int cb_embed_text_bwd_det(const void* dh, const int64_t* ids, const float* word,
   const int64_t nb = static_cast<int64_t>(per_pos) * lt;
   float* drows = scratch + 3 * nb * HID;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  launch_k(embed_text_bwd_kernel<true>, dim3(per_pos, lt), 128, 0, st, static_cast<const __nv_bfloat16*>(dh), ids, word, pos, type0,
+  launch_k(embed_text_bwd_kernel<true, false>, dim3(per_pos, lt), 128, 0, st, static_cast<const __nv_bfloat16*>(dh), ids, word, pos, type0,
            gamma, stats, dword, dpos, dtype0, dgamma, dbeta, nseq, lt, l, vocab, make_drop(dropout_p, seed), scratch, drows);
   int rc = check_launch("cb_embed_text_bwd_det");
   if (rc != CB_OK) return rc;
@@ -917,6 +929,84 @@ int cb_embed_text_bwd_det(const void* dh, const int64_t* ids, const float* word,
   launch_k(word_scatter_ordered_kernel, static_cast<int>(static_cast<int64_t>(nseq) * lt), HID / 4, 0, st, ids, drows, dword,
            nseq * lt, vocab);
   return check_launch("cb_embed_text_bwd_det(word scatter)");
+}
+
+// ---- word vectors from the caller (a hooked word_embeddings) ----
+static int check_vectors(const char* who, const float* vec, int64_t vec_ld) {
+  CB_REQUIRE(vec && vec_ld >= HID && vec_ld % 4 == 0 && vec_ld <= INT32_MAX, "%s: vec must be non-null with a row pitch >= %d, a multiple "
+             "of 4 floats (got %lld)", who, HID, static_cast<long long>(vec_ld));
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(vec) & 15) == 0, "%s: vec must be 16-byte aligned", who);
+  return CB_OK;
+}
+
+int cb_embed_text_fwd_vectors(const float* vec, int64_t vec_ld, const float* pos, const float* type0, const float* gamma,
+                              const float* beta, void* out, float* stats, int nseq, int lt, int l, int hidden, float eps,
+                              float dropout_p, uint64_t seed, void* stream) {
+  CB_REQUIRE(hidden == HID, "cb_embed_text_fwd_vectors: hidden size %d unsupported", hidden);
+  CB_REQUIRE(pos && type0 && gamma && beta && out && stats && nseq > 0 && lt > 0 && l >= lt, "cb_embed_text_fwd_vectors: bad arguments");
+  const int rc = check_vectors("cb_embed_text_fwd_vectors", vec, vec_ld);
+  if (rc != CB_OK) return rc;
+  launch_k(embed_text_fwd_kernel<true>, ceil_div(static_cast<int64_t>(nseq) * lt, ROWS_PER_BLOCK), 128, 0, static_cast<cudaStream_t>(stream),
+           static_cast<const int64_t*>(nullptr), vec, pos, type0, gamma, beta, static_cast<__nv_bfloat16*>(out), stats, nseq, lt, l,
+           static_cast<int>(vec_ld), eps, make_drop(dropout_p, seed));
+  return check_launch("cb_embed_text_fwd_vectors");
+}
+
+int cb_embed_text_bwd_vectors(const void* dh, const float* vec, int64_t vec_ld, const float* pos, const float* type0,
+                              const float* gamma, const float* stats, float* dvec, float* dpos, float* dtype0, float* dgamma,
+                              float* dbeta, int nseq, int lt, int l, int hidden, float dropout_p, uint64_t seed, void* stream) {
+  CB_REQUIRE(hidden == HID, "cb_embed_text_bwd_vectors: hidden size %d unsupported", hidden);
+  CB_REQUIRE(dh && pos && type0 && gamma && stats && dvec && dpos && dtype0 && dgamma && dbeta, "cb_embed_text_bwd_vectors: bad arguments");
+  CB_REQUIRE(nseq > 0 && lt > 0 && lt <= 65535 && l >= lt, "cb_embed_text_bwd_vectors: bad sizes");
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(dvec) & 15) == 0, "cb_embed_text_bwd_vectors: dvec must be 16-byte aligned");
+  CB_REQUIRE_NONDET("cb_embed_text_bwd_vectors");
+  const int rc = check_vectors("cb_embed_text_bwd_vectors", vec, vec_ld);
+  if (rc != CB_OK) return rc;
+  launch_k(embed_text_bwd_kernel<false, true>, dim3(embed_bwd_per_pos(nseq), lt), 128, 0, static_cast<cudaStream_t>(stream),
+           static_cast<const __nv_bfloat16*>(dh), static_cast<const int64_t*>(nullptr), vec, pos, type0, gamma, stats,
+           static_cast<float*>(nullptr), dpos, dtype0, dgamma, dbeta, nseq, lt, l, static_cast<int>(vec_ld), make_drop(dropout_p, seed),
+           static_cast<float*>(nullptr), dvec);
+  return check_launch("cb_embed_text_bwd_vectors");
+}
+
+int64_t cb_embed_text_bwd_vectors_scratch_bytes(int nseq, int lt) {
+  if (nseq <= 0 || lt <= 0) return 0;
+  return 3ll * embed_bwd_per_pos(nseq) * lt * HID * 4;
+}
+
+int cb_embed_text_bwd_vectors_det(const void* dh, const float* vec, int64_t vec_ld, const float* pos, const float* type0,
+                                  const float* gamma, const float* stats, float* dvec, float* dpos, float* dtype0, float* dgamma,
+                                  float* dbeta, int nseq, int lt, int l, int hidden, float dropout_p, uint64_t seed, float* scratch,
+                                  int64_t scratch_bytes, void* stream) {
+  CB_REQUIRE(hidden == HID, "cb_embed_text_bwd_vectors_det: hidden size %d unsupported", hidden);
+  CB_REQUIRE(dh && pos && type0 && gamma && stats && dvec && dpos && dtype0 && dgamma && dbeta, "cb_embed_text_bwd_vectors_det: bad arguments");
+  CB_REQUIRE(nseq > 0 && lt > 0 && lt <= 65535 && l >= lt, "cb_embed_text_bwd_vectors_det: bad sizes");
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(dvec) & 15) == 0, "cb_embed_text_bwd_vectors_det: dvec must be 16-byte aligned");
+  CB_REQUIRE_SCRATCH("cb_embed_text_bwd_vectors_det", scratch, scratch_bytes, cb_embed_text_bwd_vectors_scratch_bytes(nseq, lt));
+  int rc = check_vectors("cb_embed_text_bwd_vectors_det", vec, vec_ld);
+  if (rc != CB_OK) return rc;
+  const int per_pos = embed_bwd_per_pos(nseq);
+  const int64_t nb = static_cast<int64_t>(per_pos) * lt;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  launch_k(embed_text_bwd_kernel<true, true>, dim3(per_pos, lt), 128, 0, st, static_cast<const __nv_bfloat16*>(dh),
+           static_cast<const int64_t*>(nullptr), vec, pos, type0, gamma, stats, static_cast<float*>(nullptr), dpos, dtype0, dgamma,
+           dbeta, nseq, lt, l, static_cast<int>(vec_ld), make_drop(dropout_p, seed), scratch, dvec);
+  rc = check_launch("cb_embed_text_bwd_vectors_det");
+  if (rc != CB_OK) return rc;
+  // the partials and their order of cb_embed_text_bwd_det
+  ColRed r = {HID, 4, {colred_all(dgamma, scratch, static_cast<int>(nb), HID), colred_all(dbeta, scratch + nb * HID, static_cast<int>(nb), HID),
+                       colred_all(dtype0, scratch + 2 * nb * HID, static_cast<int>(nb), HID),
+                       {dpos, scratch + 2 * nb * HID, lt, HID, static_cast<int64_t>(per_pos) * HID, 1, 0, per_pos, HID}}};
+  return launch_ordered_colsum(r, st, "cb_embed_text_bwd_vectors_det(reduce)");
+}
+
+int cb_embed_word_scatter(const int64_t* ids, const float* dvec, float* dword, int rows, int vocab, int hidden, void* stream) {
+  CB_REQUIRE(hidden == HID, "cb_embed_word_scatter: hidden size %d unsupported", hidden);
+  CB_REQUIRE(ids && dvec && dword && rows > 0 && vocab > 0, "cb_embed_word_scatter: bad arguments");
+  CB_REQUIRE((reinterpret_cast<uintptr_t>(dvec) & 15) == 0 && (reinterpret_cast<uintptr_t>(dword) & 15) == 0,
+             "cb_embed_word_scatter: dvec and dword must be 16-byte aligned");
+  launch_k(word_scatter_ordered_kernel, rows, HID / 4, 0, static_cast<cudaStream_t>(stream), ids, dvec, dword, rows, vocab);
+  return check_launch("cb_embed_word_scatter");
 }
 
 int cb_embed_visual_fwd(const void* grid, const int32_t* seq2vid, int n_ex, const float* rowemb, const float* colemb,

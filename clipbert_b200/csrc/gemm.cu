@@ -1566,6 +1566,18 @@ extern "C" int cb_gemm_wgrad_group(const cb_gemm_desc* descs, int n, void* strea
   return launch_wgrad(descs, n, gp.bn, gp.split, static_cast<cudaStream_t>(stream_v), "cb_gemm_wgrad_group");
 }
 
+/* The launch plan cb_gemm_wgrad_group runs the problems with: tile width and K-split per problem, or 0 and 0 when they are not
+   grouped (each then runs as its own cb_gemm). A single weight gradient with block_n / split_k set to these runs each output
+   element's sum in the group's order. */
+extern "C" int cb_gemm_wgrad_group_plan(const cb_gemm_desc* descs, int n, int* bn, int* split) {
+  using namespace cb;
+  CB_REQUIRE(descs != nullptr && n >= 1 && bn != nullptr && split != nullptr, "cb_gemm_wgrad_group_plan: bad arguments");
+  const GroupPlan gp = group_plan(descs, n, plan_sm_count());
+  *bn = gp.groupable ? gp.bn : 0;
+  *split = gp.groupable ? real_splits(ceil_div(descs[0].k, BK), gp.split) : 0;
+  return CB_OK;
+}
+
 extern "C" int cb_gemm_tile_width(const cb_gemm_desc* d) {
   using namespace cb;
   if (d == nullptr || d->m <= 0 || d->n <= 0 || d->k <= 0) return 0;

@@ -4,7 +4,8 @@ Mirrors the reference classes in ``src/modeling/modeling.py`` / ``src/modeling/t
 (ClipBertBaseModel, ClipBertForVideoTextRetrieval, ClipBertForSequenceClassification,
 ClipBertForMultipleChoice, ClipBertForPreTraining): same constructor (a BertConfig-like object),
 same forward signatures and return dicts, same state_dict keys (SURVEY.md App. B). The torch.nn
-modules below are PARAMETER CONTAINERS only — their own ``forward`` is never called. All arithmetic
+modules below are parameter containers whose ``forward`` runs only on the module path: when a hook is registered on bert or a
+module below it, bert(...) and the heads call them (_BertPass), each running its part of the engine. All arithmetic
 is the hand-written sm_90a kernels behind libclipbert_sm90.so:
 
   embeddings     cb_embed_text_fwd / cb_embed_visual_fwd (gather + sum + LN + dropout; the visual
@@ -40,14 +41,24 @@ def _cfg(config, name, default=None):
 # ----------------------------------------------------------------------------------------------------
 # parameter containers (names = reference attribute names => identical state_dict keys)
 # ----------------------------------------------------------------------------------------------------
+class BertWordEmbeddings(nn.Embedding):
+    """BertEmbeddings.word_embeddings: on the module path (a hook on it) input_ids -> word[input_ids], fp32 (B', Lt, 768)."""
+
+    def forward(self, input_ids):
+        return _bert_pass(self).word(self, input_ids)
+
+
 class BertEmbeddings(nn.Module):
     def __init__(self, config):
         super().__init__()
         h = _cfg(config, "hidden_size")
-        self.word_embeddings = nn.Embedding(_cfg(config, "vocab_size"), h, padding_idx=_cfg(config, "pad_token_id", 0))
+        self.word_embeddings = BertWordEmbeddings(_cfg(config, "vocab_size"), h, padding_idx=_cfg(config, "pad_token_id", 0))
         self.position_embeddings = nn.Embedding(_cfg(config, "max_position_embeddings"), h)
         self.token_type_embeddings = nn.Embedding(_cfg(config, "type_vocab_size"), h)
         self.LayerNorm = nn.LayerNorm(h, eps=_cfg(config, "layer_norm_eps"))
+
+    def forward(self, input_ids):
+        return _bert_pass(self).text(self, input_ids)
 
 
 class VisualInputEmbedding(nn.Module):
@@ -60,12 +71,18 @@ class VisualInputEmbedding(nn.Module):
         self.token_type_embeddings = nn.Embedding(1, h)
         self.LayerNorm = nn.LayerNorm(h, eps=_cfg(config, "layer_norm_eps"))
 
+    def forward(self, grid):
+        return _bert_pass(self).visual(self, grid)
+
 
 class BertSelfAttention(nn.Module):
     def __init__(self, config):
         super().__init__()
         h = _cfg(config, "hidden_size")
         self.query, self.key, self.value = nn.Linear(h, h), nn.Linear(h, h), nn.Linear(h, h)
+
+    def forward(self, hidden_states, attention_mask=None, head_mask=None):
+        return _bert_pass(self).self_attention(self, hidden_states, attention_mask, head_mask)
 
 
 class BertSelfOutput(nn.Module):
@@ -75,6 +92,9 @@ class BertSelfOutput(nn.Module):
         self.dense = nn.Linear(h, h)
         self.LayerNorm = nn.LayerNorm(h, eps=_cfg(config, "layer_norm_eps"))
 
+    def forward(self, hidden_states, input_tensor):
+        return _bert_pass(self).self_output(self, hidden_states, input_tensor)
+
 
 class BertAttention(nn.Module):
     def __init__(self, config):
@@ -82,11 +102,17 @@ class BertAttention(nn.Module):
         self.self = BertSelfAttention(config)
         self.output = BertSelfOutput(config)
 
+    def forward(self, hidden_states, attention_mask=None, head_mask=None):
+        return _bert_pass(self).attention(self, hidden_states, attention_mask, head_mask)
+
 
 class BertIntermediate(nn.Module):
     def __init__(self, config):
         super().__init__()
         self.dense = nn.Linear(_cfg(config, "hidden_size"), _cfg(config, "intermediate_size"))
+
+    def forward(self, hidden_states):
+        return _bert_pass(self).intermediate(self, hidden_states)
 
 
 class BertOutput(nn.Module):
@@ -94,6 +120,9 @@ class BertOutput(nn.Module):
         super().__init__()
         self.dense = nn.Linear(_cfg(config, "intermediate_size"), _cfg(config, "hidden_size"))
         self.LayerNorm = nn.LayerNorm(_cfg(config, "hidden_size"), eps=_cfg(config, "layer_norm_eps"))
+
+    def forward(self, hidden_states, input_tensor):
+        return _bert_pass(self).output(self, hidden_states, input_tensor)
 
 
 class BertLayer(nn.Module):
@@ -103,11 +132,17 @@ class BertLayer(nn.Module):
         self.intermediate = BertIntermediate(config)
         self.output = BertOutput(config)
 
+    def forward(self, hidden_states, attention_mask=None, head_mask=None):
+        return _bert_pass(self).layer(self, hidden_states, attention_mask, head_mask)
+
 
 class BertEncoder(nn.Module):
     def __init__(self, config):
         super().__init__()
         self.layer = nn.ModuleList([BertLayer(config) for _ in range(_cfg(config, "num_hidden_layers"))])
+
+    def forward(self, hidden_states, attention_mask=None, head_mask=None):
+        return _bert_pass(self).encoder(self, hidden_states, attention_mask, head_mask)
 
 
 class BertPooler(nn.Module):
@@ -115,6 +150,9 @@ class BertPooler(nn.Module):
         super().__init__()
         h = _cfg(config, "hidden_size")
         self.dense = nn.Linear(h, h)
+
+    def forward(self, hidden_states):
+        return _bert_pass(self).pooler(self, hidden_states)
 
 
 class ClipBertBaseModel(nn.Module):
@@ -161,6 +199,11 @@ class ClipBertBaseModel(nn.Module):
     ``retain_graph=True`` allows a second backward. The forward issues the launches of the default; so does the backward of a
     layer whose map is not differentiable. Refused together with the overlapped data-parallel exchange
     (``enable_overlapped_allreduce``): the switch is for analysis, not training.
+
+    A hook on this model or a module below it (or a global module hook) runs the pass through the modules - embeddings,
+    visual_embeddings, encoder, each layer's attention (self, output), intermediate and output, pooler - so torch's hooks on them
+    fire, and a forward hook or pre-hook may replace what they return or receive. The backward is a chain of nodes split at the
+    hooked modules. INTEGRATION.md lists what each module hands to its hooks and the hooks that are refused.
     """
 
     differentiable_attentions = False
@@ -182,8 +225,16 @@ class ClipBertBaseModel(nn.Module):
         self.__dict__["_engine"] = _engine
 
     def forward(self, text_input_ids, visual_inputs, attention_mask):
-        return self._engine._run_base(text_input_ids, visual_inputs, attention_mask, self.output_hidden_states, self.output_attentions,
-                                      self.differentiable_attentions, self.layerwise_autograd)
+        eng = self._engine
+        ps = _BERT_PASSES[-1] if _BERT_PASSES and _BERT_PASSES[-1].awaits(eng) else None
+        if ps is None:
+            hooked = eng._bert_hooked()
+            if not hooked:
+                return eng._run_base(text_input_ids, visual_inputs, attention_mask, self.output_hidden_states, self.output_attentions,
+                                     self.differentiable_attentions, self.layerwise_autograd)
+            with _BertPass(eng, hooked) as ps:
+                return ps.base(text_input_ids, visual_inputs, attention_mask)
+        return ps.base(text_input_ids, visual_inputs, attention_mask)
 
 
 def _require_cuda(t):
@@ -431,6 +482,779 @@ class _PoolerNode(torch.autograd.Function):
         return None, dx.view(nseq, L, H), None
 
 
+# ----------------------------------------------------------------------------------------------------
+# module path: hooks on bert and the modules below it
+# ----------------------------------------------------------------------------------------------------
+_BERT_PASSES = []     # the module-path passes running (_BertPass), innermost last
+_BERT_SITES = (BertEmbeddings, BertWordEmbeddings, VisualInputEmbedding, BertEncoder, BertLayer, BertAttention, BertSelfAttention, BertSelfOutput,
+               BertIntermediate, BertOutput, BertPooler, ClipBertBaseModel)
+
+
+def _bert_pass(module):
+    """The module-path pass that is calling ``module``: bert's modules run only inside bert(...) or a head's forward."""
+    if not _BERT_PASSES:
+        raise RuntimeError("%s of ClipBertBaseModel runs only inside bert(...) or a head's forward (call the ClipBertBaseModel or its "
+                           "head; calling its embeddings, encoder, layers or their sub-modules directly is not supported)"
+                           % type(module).__name__)
+    return _BERT_PASSES[-1]
+
+
+def _has_hooks(mod):
+    return bool(mod._forward_hooks or mod._forward_pre_hooks or mod._backward_hooks or mod._backward_pre_hooks)
+
+
+def _global_hooks():
+    g = torch.nn.modules.module
+    return any(getattr(g, k, None) for k in ("_global_forward_hooks", "_global_forward_pre_hooks", "_global_backward_hooks",
+                                             "_global_backward_pre_hooks"))
+
+
+def _input_needed(ctx, k):
+    """Whether tensor input k of this node (a data input, not a parameter anchor) takes a gradient in the current backward: as
+    _will_execute, but a leaf that torch.autograd.grad() was asked for does."""
+    node = ctx.next_functions[k][0]
+    if node is None:
+        return False
+    try:
+        return bool(torch._C._will_engine_execute_node(node))
+    except RuntimeError:        # a captured input of autograd.grad()
+        return True
+
+
+def _engine_executes(node):
+    """Whether the engine runs ``node`` (a grad_fn) in the current backward."""
+    try:
+        return bool(torch._C._will_engine_execute_node(node))
+    except RuntimeError:
+        return False
+
+
+class _BertPass:
+    """One bert(...) pass on the module path (a hook on bert or a module below it): each module the forward calls runs its part of
+    the engine here, from the tensor it was handed (the previous module's output, or what a hook replaced it with) to a view of
+    the bf16 buffer it writes. A pass that records autograd runs each part as a node whose activations are its saved tensors:
+    one node per encoder layer unless a sub-module of that layer is hooked, then the attention (or, with its self-attention or
+    output hooked, _SelfNode + _SelfOutputNode) and the FFN (or, with intermediate or output hooked, _InterNode + _OutNode)."""
+
+    def __init__(self, eng, hooked, repeat=None, given=None):
+        self.eng, self.hooked = eng, hooked
+        self.repeat = (1, None, None) if repeat is None else repeat
+        self.head = repeat is not None          # a head's pass: bert(...) is called by the head and returns to it
+        self.given = given                      # head: (the visual_inputs it hands to bert, the grid behind them)
+        self.waiting = self.head                # the head's bert(...) call has not started yet
+        self.st = None
+        self.own = {}                           # id(tensor handed out) -> (tensor, the engine's [B' * L, H] rows behind it)
+        self.fwd = {}                           # forward-only bookkeeping, dropped when the pass ends (it refers to outputs)
+        self.handover = {}                      # backward: residual gradients handed to the node that owns the other term
+
+    def __enter__(self):
+        _BERT_PASSES.append(self)
+        return self
+
+    def __exit__(self, *exc):
+        _BERT_PASSES.pop()
+        self.own, self.fwd = {}, {}
+        ops.dropout_offset_bind(None)
+
+    def awaits(self, eng):
+        return self.waiting and self.eng is eng
+
+    # ---- shared helpers ------------------------------------------------------------------------------------------------
+    def bind(self):
+        ops.dropout_offset_bind(self.st["drop_word"])       # a hook may have run another pass in between
+
+    def dims(self):
+        nseq, _, _, _, _, lt, L = self.st["dims"]
+        return nseq, lt, L, self.st["H"]
+
+    def is_hooked(self, *mods):
+        return any(m in self.hooked for m in mods)
+
+    def give(self, t, rows):
+        self.own[id(t)] = (t, rows)
+        return t
+
+    def rows(self, t, what):
+        """A tensor a module was handed, as the engine's [B' * L, H] contiguous bf16 rows: the buffer behind it when it is the
+        tensor the pass handed out, else a copy (a hook's replacement, any strides, bf16, fp16 or fp32)."""
+        own = self.own.get(id(t))
+        if own is not None and own[0] is t:
+            return own[1]
+        nseq, _, L, H = self.dims()
+        if tuple(t.shape) != (nseq, L, H):
+            raise RuntimeError("ClipBertBaseModel: %s must be a (%d, %d, %d) tensor, got %s" % (what, nseq, L, H, tuple(t.shape)))
+        return t.detach().to(torch.bfloat16).reshape(nseq * L, H).contiguous()
+
+    def dense(self, g):
+        """An upstream gradient of a hidden state as the engine's [B' * L, H] contiguous bf16 operand."""
+        nseq, _, L, H = self.dims()
+        return g.reshape(nseq * L, H).to(torch.bfloat16).contiguous()
+
+    def view(self, rows):
+        nseq, _, L, H = self.dims()
+        return rows.view(nseq, L, H)
+
+    def layer_index(self, mod):
+        return self.eng._bert_site_index()[mod]
+
+    def check_mask(self, mod, attention_mask, head_mask):
+        if attention_mask is not self.fwd.get("ext_mask"):
+            raise RuntimeError("ClipBertBaseModel: the attention_mask %s received is not the extended mask of the pass: a hook that "
+                               "changes the mask is not supported (the kernels read the text mask of the call)" % type(mod).__name__)
+        if head_mask is not None:
+            raise RuntimeError("ClipBertBaseModel: %s received a head_mask: head masks are not supported (ablate a head with a "
+                               "pre-hook on attention.output that zeroes its 64 context columns)" % type(mod).__name__)
+
+    # ---- ClipBertBaseModel ---------------------------------------------------------------------------------------------
+    def base(self, ids, visual_inputs, attention_mask):
+        """ClipBertBaseModel.forward through its modules (modeling.py:201-238)."""
+        eng = self.eng
+        bert = eng.bert
+        self.waiting = False
+        _require_cuda(ids)
+        eng._ensure_ready(ids.device)
+        src = visual_inputs
+        if self.head and visual_inputs is self.given[0]:
+            src = self.given[1]                 # the head's grid, repeated by the visual-embedding kernel
+        else:
+            self.repeat = (1, None, None)
+            assert visual_inputs.shape[0] == ids.shape[0], "visual_inputs must have one row per text example"
+        grid = src.detach()
+        grid = (grid if grid.dtype == torch.bfloat16 else grid.to(torch.bfloat16)).contiguous()
+        mask = attention_mask.to(torch.int64).contiguous()
+        self.want_hidden, self.want_attn = bert.output_hidden_states, bert.output_attentions
+        self.diff_attn = self.want_attn and bert.differentiable_attentions
+        self.need_backward = torch.is_grad_enabled()
+        self.st = eng._pass_state(ids.contiguous(), grid, mask, self.repeat, bert.training)
+        self.fwd["grid"], self.fwd["grid_src"] = visual_inputs, src
+        nseq, lt, L, H = self.dims()
+        self.x = torch.empty(nseq * L, H, dtype=torch.bfloat16, device=ids.device)
+        t = bert.embeddings(ids)
+        v = bert.visual_embeddings(visual_inputs)
+        x = self.give(_JoinNode.apply(self, t, v), self.fwd.pop("x_rows"))
+        ext = None
+        enc_mods = [bert.encoder] + [m for ly in bert.encoder.layer for m in (ly, ly.attention, ly.attention.self)]
+        if self.is_hooked(*enc_mods):         # the reference's extended additive mask, for the hooks that can see it
+            full = torch.cat([mask, mask.new_ones(nseq, L - lt)], 1)
+            ext = (1.0 - full[:, None, None, :].to(torch.float32)) * -10000.0
+        self.fwd["ext_mask"] = ext
+        enc = bert.encoder(x, ext)
+        made = self.fwd.pop("encoder_out")
+        if len(enc) != len(made) or any(a is not b for a, b in zip(enc[1:], made[1:])):
+            raise RuntimeError("ClipBertBaseModel: a hook on bert.encoder replaced a member of its output other than [0] (the last "
+                               "hidden state): not supported; replace a layer's output instead")
+        pooled = bert.pooler(enc[0])
+        return (enc[0], pooled) + tuple(enc[1:])
+
+    # ---- embeddings ------------------------------------------------------------------------------------------------------
+    def text(self, mod, ids):
+        if ids.dtype not in (torch.int64, torch.int32) or tuple(ids.shape) != tuple(self.st["ids"].shape):
+            raise RuntimeError("ClipBertBaseModel: bert.embeddings takes (%d, %d) token ids" % tuple(self.st["ids"].shape))
+        ids = ids.to(torch.int64).contiguous()
+        if self.is_hooked(mod.word_embeddings):
+            vec = mod.word_embeddings(ids)
+            return self.give(_TextVectorsNode.apply(self, vec, mod.word_embeddings.weight), self.x)
+        return self.give(_TextNode.apply(self, ids, mod.word_embeddings.weight), self.x)
+
+    def word(self, mod, ids):
+        if ids.dtype not in (torch.int64, torch.int32) or tuple(ids.shape) != tuple(self.st["ids"].shape):
+            raise RuntimeError("ClipBertBaseModel: bert.embeddings.word_embeddings takes (%d, %d) token ids" % tuple(self.st["ids"].shape))
+        return _WordNode.apply(self, ids.to(torch.int64).contiguous(), mod.weight)
+
+    def visual(self, mod, grid):
+        st = self.st
+        if grid is self.fwd["grid"]:
+            g, repeat, grid = st["grid"], self.repeat, self.fwd["grid_src"]
+        else:                                   # a replacement: one row per sequence, sampled as the pass samples
+            nseq, nvid, T, gh, gw, _, _ = st["dims"]
+            g = grid.detach()
+            g = (g if g.dtype == torch.bfloat16 else g.to(torch.bfloat16)).contiguous()
+            sample = st["sample"]
+            shape = (nseq, T, gh * gw, 1, st["H"]) if sample is not None else (nseq, T, gh, gw, st["H"])
+            if sample is not None:
+                if g.shape[0] != nseq or g.dim() != 5 or g.shape[2] * g.shape[3] != sample[1] * sample[2]:
+                    raise RuntimeError("ClipBertBaseModel: visual_inputs replaced with a tensor of the wrong shape %s" % (tuple(grid.shape),))
+                g = g.view(nseq, T, -1, st["H"]).index_select(2, sample[0]).view(nseq, T, gh, gw, st["H"])
+            elif tuple(g.shape) != (nseq, T, gh, gw, st["H"]):
+                raise RuntimeError("ClipBertBaseModel: visual_inputs must be %s per sequence, got %s" % (shape, tuple(grid.shape)))
+            repeat = (1, None, None)
+        return self.give(_VisualNode.apply(self, grid, g, repeat, mod.LayerNorm.weight), self.x)
+
+    # ---- encoder -----------------------------------------------------------------------------------------------------------
+    def encoder(self, mod, h, attention_mask, head_mask):
+        self.check_mask(mod, attention_mask, head_mask)
+        hidden, attn = [], []
+        for layer in mod.layer:
+            if self.want_hidden:
+                hidden.append(h)
+            outs = layer(h, attention_mask, None)
+            h = outs[0]
+            if self.want_attn:
+                attn.append(outs[1])
+        if self.want_hidden:
+            hidden.append(h)
+        out = (h,) + ((tuple(hidden),) if self.want_hidden else ()) + ((tuple(attn),) if self.want_attn else ())
+        self.fwd["encoder_out"] = out
+        return out
+
+    def _maps(self, outs, probs):
+        return outs + ((probs,) if self.want_attn else ())
+
+    def layer(self, mod, h, attention_mask, head_mask):
+        self.check_mask(mod, attention_mask, head_mask)
+        i = self.layer_index(mod)
+        att = mod.attention
+        if not self.is_hooked(att, att.self, att.output, mod.intermediate, mod.output):
+            y, probs = _LayerModNode.apply(self, i, h, att.self.query.weight)
+            return self._maps((self.give(y, self.fwd.pop("y_rows")),), probs)
+        ao = att(h, attention_mask, None)
+        a = ao[0]
+        if self.is_hooked(mod.intermediate, mod.output):
+            y = mod.output(mod.intermediate(a), a)
+        else:
+            y = self.give(_FfnNode.apply(self, i, a, mod.intermediate.dense.weight), self.fwd.pop("y_rows"))
+        return (y,) + tuple(ao[1:])
+
+    def attention(self, mod, h, attention_mask, head_mask):
+        self.check_mask(mod, attention_mask, head_mask)
+        i = self.layer_index(mod)
+        if self.is_hooked(mod.self, mod.output):
+            so = mod.self(h, attention_mask, None)
+            return (mod.output(so[0], h),) + tuple(so[1:])
+        a, probs = _AttentionNode.apply(self, i, h, mod.self.query.weight)
+        return self._maps((self.give(a, self.fwd.pop("a_rows")),), probs)
+
+    def self_attention(self, mod, h, attention_mask, head_mask):
+        self.check_mask(mod, attention_mask, head_mask)
+        i = self.layer_index(mod)
+        ctx, probs = _SelfNode.apply(self, i, h, mod.query.weight)
+        self.fwd[("self", i)] = (h, ctx.grad_fn)
+        return self._maps((self.give(ctx, self.fwd.pop("ctx_rows")),), probs)
+
+    def self_output(self, mod, ctx, h):
+        i = self.layer_index(mod)
+        h_self, node = self.fwd.pop(("self", i), (None, None))
+        partner = node if (h_self is h and node is not None) else None
+        a = _SelfOutputNode.apply(self, i, ctx, h, mod.dense.weight, partner)
+        return self.give(a, self.fwd.pop("a_rows"))
+
+    def intermediate(self, mod, a):
+        i = self.layer_index(mod)
+        gel = _InterNode.apply(self, i, a, mod.dense.weight)
+        self.fwd[("inter", i)] = (a, gel.grad_fn)
+        return gel
+
+    def output(self, mod, gel, a):
+        i = self.layer_index(mod)
+        a_inter, node = self.fwd.pop(("inter", i), (None, None))
+        partner = node if (a_inter is a and node is not None) else None
+        y = _OutNode.apply(self, i, gel, a, mod.dense.weight, partner)
+        return self.give(y, self.fwd.pop("y_rows"))
+
+    # ---- pooler and head -----------------------------------------------------------------------------------------------
+    def split_head(self):
+        """Whether the head's part runs as a node of its own after the pooler (pooled_output visible to a hook), rather than
+        together with the pooler's backward (its tanh' fused into the head's dgrad epilogue, as on the default path)."""
+        return self.is_hooked(self.eng.bert, self.eng.bert.pooler)
+
+    def pooler(self, mod, h):
+        self.fwd["seq"] = h
+        if self.head and not self.split_head():
+            x = self.rows(h, "the input of bert.pooler")
+            self.fwd["seq_rows"] = x
+            self.bind()
+            return self.eng._pooler_fwd(self.st, x)           # the head's node runs the pooler's backward
+        return _PoolerModNode.apply(self, h, mod.dense.weight)
+
+    def run_head(self, seq, pooled):
+        eng = self.eng
+        anchor = next(lin for _, lin in eng._head_linears()).weight
+        if self.split_head():
+            outs = _HeadNode.apply(self, seq, pooled, anchor)
+        else:
+            outs = _HeadPoolerNode.apply(self, seq, pooled.detach(), anchor)
+        return outs
+
+
+def _alias(t):
+    """t as a tensor of its own on the same memory: not an autograd view of the encoder-input buffer, which the other embedding
+    kernel writes after t is handed out."""
+    return torch.empty(0, dtype=t.dtype, device=t.device).set_(t.untyped_storage(), t.storage_offset(), t.shape, t.stride())
+
+
+def _layer_seed(ps, i):
+    return ps.st["seed"] + 16 * (i + 1)
+
+
+def _ly(names, tensors, seed):
+    return dict(zip(names, tensors), seed=seed)
+
+
+class _TextNode(torch.autograd.Function):
+    """bert.embeddings: input_ids -> the text rows of the encoder input, (B', Lt, H)."""
+
+    @staticmethod
+    def forward(ctx, ps, ids, anchor):
+        ps.bind()
+        ps.eng._text_fwd(ps.st, ids, ps.x)
+        ctx.ps = ps
+        ctx.save_for_backward(ids)
+        return _alias(ps.view(ps.x)[:, :ps.dims()[1]])
+
+    @staticmethod
+    def backward(ctx, dt):
+        ps = ctx.ps
+        if dt is None or not _will_execute(ctx, 1):
+            return None, None, None
+        ids, = ctx.saved_tensors
+        with ps.eng._node_backward(ps.st, True):
+            ps.eng._text_embedding_backward(ps.st, ids, _JoinNode.full(ps, dt, True))
+        return None, None, None
+
+
+class _WordNode(torch.autograd.Function):
+    """bert.embeddings.word_embeddings: input_ids -> word[input_ids], fp32 (B', Lt, H), materialised for the hooks. Its backward
+    adds the per-token vector gradients into the table rows (cb_embed_word_scatter: one writer and one order per row)."""
+
+    @staticmethod
+    def forward(ctx, ps, ids, anchor):
+        word = ps.eng._emb("emb.word")[0]
+        ctx.ps = ps
+        ctx.save_for_backward(ids)
+        nseq, lt, _, H = ps.dims()
+        return word.index_select(0, ids.reshape(-1).clamp(0, word.shape[0] - 1)).view(nseq, lt, H)
+
+    @staticmethod
+    def backward(ctx, dvec):
+        ps = ctx.ps
+        if dvec is None or not _will_execute(ctx, 1):
+            return None, None, None
+        ids, = ctx.saved_tensors
+        nseq, lt, _, H = ps.dims()
+        with ps.eng._node_backward(ps.st, True):
+            ops.embed_word_scatter(ids, dvec.reshape(nseq * lt, H).to(torch.float32).contiguous(), ps.eng._emb("emb.word")[1])
+        return None, None, None
+
+
+class _TextVectorsNode(torch.autograd.Function):
+    """bert.embeddings with word_embeddings hooked: the word vectors (its output, or a hook's replacement) -> the text rows of the
+    encoder input (cb_embed_text_fwd_vectors); the backward returns d vectors (cb_embed_text_bwd_vectors)."""
+
+    @staticmethod
+    def forward(ctx, ps, vec, anchor):
+        nseq, lt, _, H = ps.dims()
+        if tuple(vec.shape) != (nseq, lt, H):
+            raise RuntimeError("ClipBertBaseModel: the word vectors handed to bert.embeddings must be (%d, %d, %d), got %s"
+                               % (nseq, lt, H, tuple(vec.shape)))
+        v = vec.detach().to(torch.float32).reshape(nseq * lt, H)
+        if v.stride(1) != 1 or v.stride(0) % 4 or v.data_ptr() % 16:
+            v = v.contiguous()
+        ps.bind()
+        ps.eng._text_vectors_fwd(ps.st, v, ps.x)
+        ctx.ps = ps
+        ctx.save_for_backward(v)
+        return _alias(ps.view(ps.x)[:, :lt])
+
+    @staticmethod
+    def backward(ctx, dt):
+        ps = ctx.ps
+        need_vec, grads = _input_needed(ctx, 0), _will_execute(ctx, 1)
+        if dt is None or not (need_vec or grads):
+            return None, None, None
+        v, = ctx.saved_tensors
+        with ps.eng._node_backward(ps.st, grads):
+            dvec = ps.eng._text_vectors_backward(ps.st, v, _JoinNode.full(ps, dt, True), grads)
+        nseq, lt, _, H = ps.dims()
+        return None, dvec.view(nseq, lt, H), None
+
+
+class _VisualNode(torch.autograd.Function):
+    """bert.visual_embeddings: visual_inputs -> the visual rows of the encoder input, (B', Lv, H)."""
+
+    @staticmethod
+    def forward(ctx, ps, grid, g, repeat, anchor):
+        ps.bind()
+        ps.eng._visual_fwd(ps.st, g, repeat, ps.x)
+        ctx.ps, ctx.repeat, ctx.grid = ps, repeat, (grid.shape, grid.dtype)
+        ctx.save_for_backward(g)
+        return _alias(ps.view(ps.x)[:, ps.dims()[1]:])
+
+    @staticmethod
+    def backward(ctx, dv):
+        ps = ctx.ps
+        need_grid, grads = _input_needed(ctx, 0), _will_execute(ctx, 2)
+        if dv is None or not (need_grid or grads):
+            return None, None, None, None, None
+        g, = ctx.saved_tensors
+        with ps.eng._node_backward(ps.st, grads):
+            dgrid = ps.eng._visual_embedding_backward(ps.st, g, ctx.repeat, _JoinNode.full(ps, dv, False), need_grid, grads)
+        if dgrid is not None:
+            dgrid = dgrid.view(ctx.grid[0])
+        return None, dgrid, None, None, None
+
+
+class _JoinNode(torch.autograd.Function):
+    """torch.cat([text, visual], 1) (modeling.py:217-220): zero-copy when both are the rows the embeddings wrote."""
+
+    @staticmethod
+    def forward(ctx, ps, t, v):
+        nseq, lt, L, H = ps.dims()
+        ctx.ps = ps
+        ot, ov = ps.own.get(id(t)), ps.own.get(id(v))
+        if ot is not None and ot[0] is t and ov is not None and ov[0] is v:
+            x = ps.x
+        else:
+            x = torch.empty_like(ps.x)
+            xv = x.view(nseq, L, H)
+            for part, src, n in ((xv[:, :lt], t, lt), (xv[:, lt:], v, L - lt)):
+                if tuple(src.shape) != (nseq, n, H):
+                    raise RuntimeError("ClipBertBaseModel: a replaced embedding output must be (%d, %d, %d), got %s"
+                                       % (nseq, n, H, tuple(src.shape)))
+                part.copy_(src.detach())
+        ps.fwd["x_rows"] = x
+        return x.view(nseq, L, H)
+
+    @staticmethod
+    def backward(ctx, dx):
+        ps = ctx.ps
+        nseq, lt, L, H = ps.dims()
+        g = ps.dense(dx)
+        ps.handover["emb"] = g
+        gv = g.view(nseq, L, H)
+        return None, gv[:, :lt], gv[:, lt:]
+
+    @staticmethod
+    def full(ps, g, text):
+        """The [B' * L, H] gradient buffer whose text (or visual) rows hold g, for the embedding kernels' row pitch."""
+        full = ps.handover.get("emb")
+        nseq, lt, L, H = ps.dims()
+        if (full is not None and g.dtype == torch.bfloat16 and g.stride() == (L * H, H, 1)
+                and g.data_ptr() == full.data_ptr() + (0 if text else lt * H * full.element_size())):
+            return full
+
+        buf = torch.zeros(nseq * L, H, dtype=torch.bfloat16, device=g.device)
+        v = buf.view(nseq, L, H)
+        (v[:, :lt] if text else v[:, lt:]).copy_(g)
+        return buf
+
+
+def _map_outputs(ctx, ps, probs):
+    if probs is None:
+        probs = torch.empty(0, device=ps.x.device)
+    if not ps.diff_attn:
+        ctx.mark_non_differentiable(probs)
+    return probs
+
+
+def _dmap(ps, dprobs):
+    return None if (dprobs is None or not ps.diff_attn) else dprobs.to(torch.float32).contiguous()
+
+
+class _LayerModNode(torch.autograd.Function):
+    """encoder.layer[i] with none of its sub-modules hooked: hidden_states -> (layer_output, probabilities)."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, anchor):
+        eng, st = ps.eng, ps.st
+        ps.bind()
+        x = ps.rows(h, "the input of encoder.layer[%d]" % i)
+        qkv, c, lse, probs = eng._self_fwd(st, i, x, ps.need_backward, ps.want_attn)
+        s1, st1, a = eng._attn_out_fwd(st, i, c, x)
+        gel, u = eng._inter_fwd(st, i, a, ps.need_backward)
+        s2, st2, y = eng._out_fwd(st, i, gel, a)
+        ctx.ps, ctx.i = ps, i
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, qkv, c, lse, s1, st1, a, u, gel, s2, st2)
+        ps.fwd["y_rows"] = y
+        return ps.view(y), _map_outputs(ctx, ps, probs)
+
+    @staticmethod
+    def backward(ctx, dy, dprobs):
+        ps, i = ctx.ps, ctx.i
+        grads, need_dx = _will_execute(ctx, 1), _input_needed(ctx, 0)
+        dattn = _dmap(ps, dprobs)
+        if not (grads or need_dx) or (dy is None and dattn is None):
+            return None, None, None, None
+        ly = _ly(_LAYER_STASH, ctx.saved_tensors, _layer_seed(ps, i))
+        dy = torch.zeros_like(ly["x"]) if dy is None else ps.dense(dy)
+        with ps.eng._node_backward(ps.st, grads) as sq:
+            dxn = ps.eng._layer_backward(ps.st, i, ly, dy, sq, dattn=dattn, grads=grads)
+        return None, None, ps.view(dxn), None
+
+
+class _AttentionNode(torch.autograd.Function):
+    """layer[i].attention with neither sub-module hooked: hidden_states -> (attention_output (post-LN1), probabilities)."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, anchor):
+        eng, st = ps.eng, ps.st
+        ps.bind()
+        x = ps.rows(h, "the input of layer[%d].attention" % i)
+        qkv, c, lse, probs = eng._self_fwd(st, i, x, ps.need_backward, ps.want_attn)
+        s1, st1, a = eng._attn_out_fwd(st, i, c, x)
+        ctx.ps, ctx.i = ps, i
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, qkv, c, lse, s1, st1)
+        ps.fwd["a_rows"] = a
+        return ps.view(a), _map_outputs(ctx, ps, probs)
+
+    @staticmethod
+    def backward(ctx, da, dprobs):
+        ps, i = ctx.ps, ctx.i
+        grads, need_dx = _will_execute(ctx, 1), _input_needed(ctx, 0)
+        dattn = _dmap(ps, dprobs)
+        if not (grads or need_dx) or (da is None and dattn is None):
+            return None, None, None, None
+        ly = _ly(("x", "qkv", "ctx", "lse", "s1", "st1"), ctx.saved_tensors, _layer_seed(ps, i))
+        da = torch.zeros_like(ly["x"]) if da is None else ps.dense(da)
+        eng = ps.eng
+        with eng._node_backward(ps.st, grads) as sq:
+            dctx, ds1 = eng._self_output_backward(ps.st, i, ly, da, sq, grads)
+            dxn = eng._self_attention_backward(ps.st, i, ly, dctx, dattn, sq, grads, ds1)
+        return None, None, ps.view(dxn), None
+
+
+class _FfnNode(torch.autograd.Function):
+    """layer[i].intermediate + layer[i].output, neither hooked: attention_output -> layer_output (gelu' fused into the dgrad)."""
+
+    @staticmethod
+    def forward(ctx, ps, i, a, anchor):
+        eng, st = ps.eng, ps.st
+        ps.bind()
+        ar = ps.rows(a, "the attention output of layer[%d]" % i)
+        gel, u = eng._inter_fwd(st, i, ar, ps.need_backward)
+        s2, st2, y = eng._out_fwd(st, i, gel, ar)
+        ctx.ps, ctx.i = ps, i
+        ctx.save_for_backward(ar, u, gel, s2, st2)
+        ps.fwd["y_rows"] = y
+        return ps.view(y)
+
+    @staticmethod
+    def backward(ctx, dy):
+        ps, i = ctx.ps, ctx.i
+        grads, need_dx = _will_execute(ctx, 1), _input_needed(ctx, 0)
+        if not (grads or need_dx):
+            return None, None, None, None
+        ly = _ly(("a", "u", "gel", "s2", "st2"), ctx.saved_tensors, _layer_seed(ps, i))
+        eng = ps.eng
+        with eng._node_backward(ps.st, grads) as sq:
+            du, ds2 = eng._output_backward(ps.st, i, ly, ps.dense(dy), sq, grads, fused=True)
+            da = eng._intermediate_backward(ps.st, i, ly, du, sq, grads, ds2)
+        return None, None, ps.view(da), None
+
+
+class _SelfNode(torch.autograd.Function):
+    """layer[i].attention.self: hidden_states -> (context, probabilities). Its backward runs the attention backward with the
+    forward's own context (the D = rowsum(dO o O) term belongs to the attention), then the QKV dgrad with the residual gradient
+    the attention.output node handed over, if any."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, anchor):
+        ps.bind()
+        x = ps.rows(h, "the input of layer[%d].attention.self" % i)
+        qkv, c, lse, probs = ps.eng._self_fwd(ps.st, i, x, ps.need_backward, ps.want_attn)
+        ctx.ps, ctx.i = ps, i
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, qkv, c, lse)
+        ps.fwd["ctx_rows"] = c
+        return ps.view(c), _map_outputs(ctx, ps, probs)
+
+    @staticmethod
+    def backward(ctx, dctx, dprobs):
+        ps, i = ctx.ps, ctx.i
+        residual = ps.handover.pop(("ds1", i), None)
+        grads = _will_execute(ctx, 1)
+        dattn = _dmap(ps, dprobs)
+        ly = _ly(("x", "qkv", "ctx", "lse"), ctx.saved_tensors, _layer_seed(ps, i))
+        if dctx is None and dattn is None:
+            return None, None, (None if residual is None else ps.view(residual)), None
+        dctx = torch.zeros_like(ly["x"]) if dctx is None else ps.dense(dctx)
+        with ps.eng._node_backward(ps.st, grads) as sq:
+            dxn = ps.eng._self_attention_backward(ps.st, i, ly, dctx, dattn, sq, grads, residual)
+        return None, None, ps.view(dxn), None
+
+
+class _SelfOutputNode(torch.autograd.Function):
+    """layer[i].attention.output: (context, hidden_states) -> attention_output = LN1(dropout(context Wao^T + b) + hidden_states).
+    The residual's gradient goes to the self-attention node when that node received the same hidden_states and runs in this
+    backward, so that its QKV dgrad adds it in the epilogue (one rounding, as on the default path); else it is returned."""
+
+    @staticmethod
+    def forward(ctx, ps, i, c, h, anchor, partner):
+        ps.bind()
+        cr = ps.rows(c, "the context handed to layer[%d].attention.output" % i)
+        x = ps.rows(h, "the hidden states handed to layer[%d].attention.output" % i)
+        s1, st1, a = ps.eng._attn_out_fwd(ps.st, i, cr, x)
+        ctx.ps, ctx.i, ctx.partner = ps, i, partner
+        ctx.save_for_backward(cr, s1, st1)
+        ps.fwd["a_rows"] = a
+        return ps.view(a)
+
+    @staticmethod
+    def backward(ctx, da):
+        ps, i = ctx.ps, ctx.i
+        grads = _will_execute(ctx, 2)
+        ly = _ly(("ctx", "s1", "st1"), ctx.saved_tensors, _layer_seed(ps, i))
+        with ps.eng._node_backward(ps.st, grads) as sq:
+            dctx, ds1 = ps.eng._self_output_backward(ps.st, i, ly, ps.dense(da), sq, grads)
+        if ctx.partner is not None and _engine_executes(ctx.partner):
+            ps.handover[("ds1", i)] = ds1
+            return None, None, ps.view(dctx), None, None, None
+        return None, None, ps.view(dctx), ps.view(ds1), None, None
+
+
+class _InterNode(torch.autograd.Function):
+    """layer[i].intermediate: attention_output -> GELU output. Its backward multiplies the incoming gradient by the stashed gelu'
+    (one bf16 rounding more than the fused dgrad epilogue of the default path), then runs the FFN-up dgrad with the residual
+    gradient the output node handed over, if any."""
+
+    @staticmethod
+    def forward(ctx, ps, i, a, anchor):
+        ps.bind()
+        ar = ps.rows(a, "the input of layer[%d].intermediate" % i)
+        gel, u = ps.eng._inter_fwd(ps.st, i, ar, ps.need_backward)
+        ctx.ps, ctx.i = ps, i
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(ar, u)
+        nseq, _, L, _ = ps.dims()
+        return gel.view(nseq, L, -1)
+
+    @staticmethod
+    def backward(ctx, dgel):
+        ps, i = ctx.ps, ctx.i
+        residual = ps.handover.pop(("ds2", i), None)
+        if dgel is None:
+            return None, None, (None if residual is None else ps.view(residual)), None
+        grads = _will_execute(ctx, 1)
+        ar, u = ctx.saved_tensors
+        du = (dgel.reshape(u.shape).float() * u.float()).to(torch.bfloat16)
+        with ps.eng._node_backward(ps.st, grads) as sq:
+            da = ps.eng._intermediate_backward(ps.st, i, dict(a=ar), du, sq, grads, residual)
+        return None, None, ps.view(da), None
+
+
+class _OutNode(torch.autograd.Function):
+    """layer[i].output: (intermediate_output, attention_output) -> layer_output = LN2(dropout(gel Wo^T + b) + attention_output).
+    The FFN-down dgrad runs without the gelu' multiply (the hooks see d intermediate_output); the residual's gradient goes to the
+    intermediate node under the same rule as _SelfOutputNode's."""
+
+    @staticmethod
+    def forward(ctx, ps, i, gel, a, anchor, partner):
+        ps.bind()
+        nseq, _, L, H = ps.dims()
+        n = ps.eng._lin["l%d.inter" % i].n
+        if tuple(gel.shape) != (nseq, L, n):
+            raise RuntimeError("ClipBertBaseModel: the input of layer[%d].output must be (%d, %d, %d), got %s" % (i, nseq, L, n, tuple(gel.shape)))
+        gr = gel.detach().to(torch.bfloat16).reshape(nseq * L, n).contiguous()
+        ar = ps.rows(a, "the attention output handed to layer[%d].output" % i)
+        s2, st2, y = ps.eng._out_fwd(ps.st, i, gr, ar)
+        ctx.ps, ctx.i, ctx.partner = ps, i, partner
+        ctx.save_for_backward(gr, s2, st2)
+        ps.fwd["y_rows"] = y
+        return ps.view(y)
+
+    @staticmethod
+    def backward(ctx, dy):
+        ps, i = ctx.ps, ctx.i
+        grads = _will_execute(ctx, 2)
+        ly = _ly(("gel", "s2", "st2"), ctx.saved_tensors, _layer_seed(ps, i))
+        with ps.eng._node_backward(ps.st, grads) as sq:
+            dgel, ds2 = ps.eng._output_backward(ps.st, i, ly, ps.dense(dy), sq, grads, fused=False)
+        nseq, _, L, H = ps.dims()
+        dgel = dgel.view(nseq, L, -1)
+        if ctx.partner is not None and _engine_executes(ctx.partner):
+            ps.handover[("ds2", i)] = ds2
+            return None, None, dgel, None, None, None
+        return None, None, dgel, ps.view(ds2), None, None
+
+
+class _PoolerModNode(torch.autograd.Function):
+    """bert.pooler: sequence_output -> pooled_output (tanh' applied on entry to the backward, as one product)."""
+
+    @staticmethod
+    def forward(ctx, ps, h, anchor):
+        ps.bind()
+        x = ps.rows(h, "the input of bert.pooler")
+        pooled = ps.eng._pooler_fwd(ps.st, x)
+        ctx.ps = ps
+        ctx.save_for_backward(x, pooled)
+        ps.fwd["seq_rows"] = x
+        return pooled
+
+    @staticmethod
+    def backward(ctx, dpooled):
+        ps = ctx.ps
+        x, pooled = ctx.saved_tensors
+        grads = _will_execute(ctx, 1)
+        nseq, _, L, H = ps.dims()
+        with ps.eng._node_backward(ps.st, grads):
+            dx = ps.eng._pooler_backward(_pooler_pre_grad(pooled, dpooled), x, nseq, L, H, grads)
+        return None, ps.view(dx), None
+
+
+class _HeadNode(torch.autograd.Function):
+    """A head's classifier / MLM / ITM part after a hooked pooler: (sequence_output, pooled_output) -> the head's outputs. Its
+    backward returns d pooled_output without tanh' (the pooler node applies it: one bf16 rounding more than the default path's
+    fused AUX_TANH_GRAD epilogue)."""
+
+    @staticmethod
+    def forward(ctx, ps, seq, pooled, anchor):
+        return _head_forward(ctx, ps, seq, pooled.detach().to(torch.bfloat16).contiguous())
+
+    @staticmethod
+    def backward(ctx, *douts):
+        ps = ctx.ps
+        grads = _will_execute(ctx, 2)
+        nseq, _, L, H = ps.dims()
+        st = ctx.st
+        with ps.eng._node_backward(st, grads):
+            dpooled = ps.eng._head_backward(st, _head_douts(ctx, douts), nseq, H, tanh=False, grads=grads)
+            extra = ps.eng._extra_sequence_grad(st)
+        return None, (None if extra is None else ps.view(extra)), dpooled, None
+
+
+class _HeadPoolerNode(torch.autograd.Function):
+    """A head's part together with the pooler's backward (pooler not hooked): sequence_output -> the head's outputs, tanh' fused
+    into the head's dgrad epilogue as on the default path."""
+
+    @staticmethod
+    def forward(ctx, ps, seq, pooled, anchor):
+        return _head_forward(ctx, ps, seq, pooled)
+
+    @staticmethod
+    def backward(ctx, *douts):
+        ps = ctx.ps
+        grads = _will_execute(ctx, 2)
+        nseq, _, L, H = ps.dims()
+        st = ctx.st
+        with ps.eng._node_backward(st, grads):
+            dpre = ps.eng._head_backward(st, _head_douts(ctx, douts), nseq, H, grads=grads)
+            dx = ps.eng._pooler_backward(dpre, st["x_last"], nseq, L, H, grads)
+            extra = ps.eng._extra_sequence_grad(st)
+            if extra is not None:
+                dx += extra
+        return None, ps.view(dx), None, None
+
+
+def _head_forward(ctx, ps, seq, pooled):
+    eng = ps.eng
+    ps.bind()
+    x = ps.fwd.pop("seq_rows", None)
+    if x is None or ps.fwd.get("seq") is not seq:
+        x = ps.rows(seq, "the sequence output handed to the head")
+    st = dict(ps.st, x_last=x, pooled=pooled)
+    nseq = ps.dims()[0]
+    outs = eng._head_forward(pooled, st, nseq, st["p_h"], st["seed"], ps.need_backward)
+    ctx.ps, ctx.st = ps, st
+    ctx.set_materialize_grads(False)
+    ctx.multi = isinstance(outs, tuple)
+    return outs
+
+
+def _head_douts(ctx, douts):
+    return douts if ctx.multi else douts[0]
+
+
 class _ClipBertHeadModel(nn.Module):
     """Shared engine: ClipBertBaseModel + an MLP head; subclasses set the head and the loss."""
 
@@ -608,6 +1432,9 @@ class _ClipBertHeadModel(nn.Module):
                 s2v = torch.tensor([i for i, r in enumerate(repeat_counts) for _ in range(r)], dtype=torch.int32)
                 starts = torch.tensor([0] + list(torch.tensor(repeat_counts).cumsum(0)), dtype=torch.int32)
                 repeat = (0, s2v.to(dev), starts.to(dev))
+        hooked = self._bert_hooked()
+        if hooked:
+            return self._run_modules(text_input_ids, visual_inputs, text_input_mask, repeat, hooked)
         grid = visual_inputs
         if grid.dtype != torch.bfloat16:
             grid = grid.to(torch.bfloat16)
@@ -673,6 +1500,73 @@ class _ClipBertHeadModel(nn.Module):
         st["layers"] = st["attn"] = None    # each layer's activations are saved tensors of its node(s) now, released with them
         return h, pooled, (hidden if flags[0] else []), (maps if flags[2] else attn)
 
+    # ---- module path: hooks on bert and the modules below it ---------------------------------------------------------------
+    def _bert_sites(self):
+        """([(name, module, the name of the module to hook instead or None when the module itself is hookable, whether it is one
+        of the head's own modules)], {module: its encoder layer}, the sites' hook dicts), computed once."""
+        sites = self.__dict__.get("_bert_site_cache")
+        if sites is None:
+            bert = self.bert
+            by_name = dict(bert.named_modules(prefix="bert"))
+            sites = []
+            for name, mod in by_name.items():
+                instead = None
+                if not isinstance(mod, _BERT_SITES):
+                    instead = name
+                    while not isinstance(by_name.get(instead), _BERT_SITES):
+                        instead = instead.rsplit(".", 1)[0]
+                sites.append((name, mod, instead, False))
+            inside = set(by_name.values())
+            sites += [(name, mod, None, True) for name, mod in self.named_modules() if mod is not self and mod not in inside]
+            index = {m: i for i, layer in enumerate(bert.encoder.layer) for m in layer.modules()}
+            # the hook registries of every site (torch adds hooks to these dicts in place): the no-hook check in one C loop
+            dicts = tuple(d for _, m, _, _ in sites for d in (m._forward_hooks, m._forward_pre_hooks, m._backward_hooks,
+                                                              m._backward_pre_hooks))
+            self.__dict__["_bert_site_cache"] = sites = (sites, index, dicts)
+        return sites
+
+    def _bert_site_index(self):
+        return self._bert_sites()[1]
+
+    def _bert_hooked(self):
+        """The set of bert's modules the forward must call because a hook is registered on them (all of them when a global module
+        hook exists); empty: the default path. Raises for hooks that cannot be honoured."""
+        glob = _global_hooks()
+        sites, _, hook_dicts = self._bert_sites()
+        if not glob and not any(map(len, hook_dicts)):
+            return set()
+        hooked = set()
+        for name, mod, instead, in_head in sites:
+            if not _has_hooks(mod):
+                if glob and instead is None and not in_head:
+                    hooked.add(mod)
+                continue
+            if in_head:
+                raise RuntimeError("%s: hooks on the head's own module %s are not supported: the head's layers run fused behind its "
+                                   "forward; hook the head itself or a module of its bert" % (type(self).__name__, name))
+            if instead is not None:
+                raise RuntimeError("ClipBertBaseModel: hooks on %s are not supported: it runs fused into a kernel of its parent and its "
+                                   "output never exists in memory; hook %s instead" % (name, instead))
+            hooked.add(mod)
+        if hooked and self._grad_ready_hook is not None:
+            raise RuntimeError("ClipBertBaseModel: hooks on the transformer's modules are for analysis, not data-parallel training: "
+                               "they cannot run while the overlapped gradient exchange (enable_overlapped_allreduce) is enabled")
+        return hooked
+
+    def _run_modules(self, ids, visual_inputs, mask, repeat, hooked):
+        """The head's forward with bert on the module path: bert(...) called as a module (torch's hooks on it and below it fire),
+        then the head's part as one node. With repeat counts, the (B', T, h, w, 768) rows of repeat_tensor_rows are materialised
+        for the hooks only when a hook on bert or bert.visual_embeddings can see them, and then as a detached copy: unless a hook
+        replaces them, the visual-embedding kernel still repeats the head's grid and sums its gradient, as on the default path."""
+        bert = self.bert
+        given = visual_inputs
+        if repeat[0] != 1 and (bert in hooked or bert.visual_embeddings in hooked):
+            g = visual_inputs.detach()
+            given = g.repeat_interleave(repeat[0], 0) if repeat[0] > 1 else g.index_select(0, repeat[1].to(torch.int64))
+        with _BertPass(self, hooked, repeat, (given, visual_inputs)) as ps:
+            out = bert(ids, given, mask)
+            return ps.run_head(out[0], out[1])
+
     @contextlib.contextmanager
     def _node_backward(self, st, grads):
         """Around the backward of one layerwise node: the pass's dropout word bound (its masks regenerated) and unbound on the way
@@ -711,26 +1605,66 @@ class _ClipBertHeadModel(nn.Module):
     def _forward_body(self, ids, grid, mask, repeat, need_backward, base=None):
         """base = None: the head's forward, returns its outputs. base = (want_hidden, want_attn): ClipBertBaseModel.forward,
         returns (sequence_output, pooled_output, hidden_states, attentions) without running the head."""
+        want_hidden, want_attn = base[:2] if base is not None else (False, False)
+        st = self._pass_state(ids, grid, mask, repeat, self.bert.training if base is not None else self.training)
+        nseq, nvid, T, gh, gw, lt, L = st["dims"]
+        H, M, seed, p_h = st["H"], nseq * L, st["seed"], st["p_h"]
+        # ---- embeddings: [text ; visual] written straight into one (B', L, 768) buffer ----
+        x = torch.empty(M, H, dtype=torch.bfloat16, device=ids.device)
+        self._text_fwd(st, ids, x)
+        self._visual_fwd(st, st["grid"], repeat, x)
+        cap = self._capture
+        if cap is not None:
+            cap["embeddings"] = x.view(nseq, L, H).clone()
+            cap.update(seed=seed, drop_word=st["drop_word"], stats_t=st["stats_t"], stats_v=st["stats_v"], grid=st["grid"],
+                       idx=None if st["sample"] is None else st["sample"][0], row_tab=st["row_tab"], col_tab=st["col_tab"])
+        # ---- encoder ----
+        hidden, attn = [], []
+        for i in range(len(self.bert.encoder.layer)):
+            if self._inject is not None and i in self._inject:      # test hook: layer-local parity (same input on both sides)
+                x = self._inject[i].to(device=ids.device, dtype=torch.bfloat16).reshape(M, H).contiguous()
+            if want_hidden:
+                hidden.append(x.view(nseq, L, H))
+            qkv, ctx, lse, probs = self._self_fwd(st, i, x, need_backward, want_attn)
+            if want_attn:
+                attn.append(probs)
+            s1, st1, a = self._attn_out_fwd(st, i, ctx, x)
+            gel, u = self._inter_fwd(st, i, a, need_backward)
+            s2, st2, y = self._out_fwd(st, i, gel, a)
+            ls = seed + 16 * (i + 1)
+            if need_backward:
+                st["layers"].append(dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2, seed=ls))
+            if cap is not None:
+                cap["l%d" % i] = dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, gel=gel, u=u, s2=s2, st2=st2)
+            x = y
+            if cap is not None:
+                cap["layer%d" % i] = x.view(nseq, L, H)
+        st["x_last"] = x
+        pooled = self._pooler_fwd(st, x)
+        st["pooled"] = pooled
+        if cap is not None:
+            cap["pooled"] = pooled
+        if base is not None:
+            if want_hidden:
+                hidden.append(x.view(nseq, L, H))
+            out = (x.view(nseq, L, H), pooled, hidden, attn)
+        else:
+            out = self._head_forward(pooled, st, nseq, p_h, seed, need_backward)
+        return out, (st if need_backward else None)
+
+    # ---- the forward's per-module pieces: the default path calls them in this order, the module path from the modules ------
+    def _pass_state(self, ids, grid, mask, repeat, train):
+        """The state one forward pass shares: its seed, dropout probabilities and word (drawn and bound here), dims, the visual
+        grid and position tables (a sampled subset in pre-training), the embedding stats, and the per-layer stash list."""
         dev = ids.device
         cfg = self.config
         H = _cfg(cfg, "hidden_size")
-        heads = _cfg(cfg, "num_attention_heads")
-        eps = float(_cfg(cfg, "layer_norm_eps"))
-        want_hidden, want_attn = base[:2] if base is not None else (False, False)
-        train = self.bert.training if base is not None else self.training
         p_h = float(_cfg(cfg, "hidden_dropout_prob")) if train else 0.0
         p_a = float(_cfg(cfg, "attention_probs_dropout_prob")) if train else 0.0
         seed = self._next_seed()
         nseq, lt = ids.shape
         nvid, T, gh, gw, _ = grid.shape
-        L = lt + gh * gw
-        M = nseq * L
-        bf16, f32 = torch.bfloat16, torch.float32
-        n_ex, s2v, starts = repeat
-
-        def new(*shape, dtype=bf16):
-            return torch.empty(*shape, dtype=dtype, device=dev)
-
+        f32 = torch.float32
         # ---- pre-training only, train mode only: keep a random subset of the visual tokens (modeling.py:80-88) ----
         # The kept positions are the same for every sequence of the batch, so the subset is presented to the embedding kernels
         # as a (n_keep x 1) grid whose "row" table is row[idx // w] + col[idx % w] (its "column" table is one zero row): index
@@ -745,86 +1679,93 @@ class _ClipBertHeadModel(nn.Module):
             col_tab = torch.zeros(1, H, dtype=f32, device=dev)
             sample = (idx, gh, gw, row_tab, col_tab)
             gh, gw = n_keep, 1
-            L = lt + n_keep
-            M = nseq * L
         drop_word = self._advance_dropout_stream(dev) if (p_h > 0 or p_a > 0) else None
         ops.dropout_offset_bind(drop_word)
-        st = dict(ids=ids, mask=mask, grid=grid, repeat=repeat, seed=seed, p_h=p_h, p_a=p_a, dims=(nseq, nvid, T, gh, gw, lt, L), layers=[],
-                  sample=sample, drop_word=drop_word)
-        # ---- embeddings: [text ; visual] written straight into one (B', L, 768) buffer ----
-        x = new(M, H)
-        st["stats_t"] = new(nseq * lt, 2, dtype=f32)
-        st["stats_v"] = new(nseq * gh * gw, 2, dtype=f32)
+        return dict(ids=ids, mask=mask, grid=grid, repeat=repeat, seed=seed, p_h=p_h, p_a=p_a, dims=(nseq, nvid, T, gh, gw, lt, lt + gh * gw),
+                    layers=[], sample=sample, drop_word=drop_word, row_tab=row_tab, col_tab=col_tab, H=H,
+                    heads=_cfg(cfg, "num_attention_heads"), eps=float(_cfg(cfg, "layer_norm_eps")),
+                    stats_t=torch.empty(nseq * lt, 2, dtype=f32, device=dev), stats_v=torch.empty(nseq * gh * gw, 2, dtype=f32, device=dev))
+
+    def _text_fwd(self, st, ids, x):
+        """BertEmbeddings: LN(word[ids] + pos + type[0]) and dropout into the text rows of x ([B' * L, H], row pitch L * H)."""
+        nseq, _, _, _, _, lt, L = st["dims"]
         g_t, b_t, _, _ = self._ln("emb.ln")
-        g_v, b_v, _, _ = self._ln("vis.ln")
         word, pos, typ = self._emb("emb.word")[0], self._emb("emb.pos")[0], self._emb("emb.type")[0]
-        ops.embed_text_fwd(ids, word, pos, typ, g_t, b_t, x, st["stats_t"], nseq, lt, L, eps, p_h, seed + 1)
-        ops.embed_visual_fwd(grid, s2v, n_ex, row_tab, col_tab, self._emb("vis.type")[0], g_v, b_v,
-                             x, st["stats_v"], nseq, T, gh, gw, lt, L, eps, p_h, seed + 2)
-        cap = self._capture
-        if cap is not None:
-            cap["embeddings"] = x.view(nseq, L, H).clone()
-            cap.update(seed=seed, drop_word=drop_word, stats_t=st["stats_t"], stats_v=st["stats_v"], grid=grid,
-                       idx=None if sample is None else sample[0], row_tab=row_tab, col_tab=col_tab)
-        # ---- encoder ----
-        hidden, attn = [], []
-        for i in range(len(self.bert.encoder.layer)):
-            ls = seed + 16 * (i + 1)
-            if self._inject is not None and i in self._inject:      # test hook: layer-local parity (same input on both sides)
-                x = self._inject[i].to(device=dev, dtype=bf16).reshape(M, H).contiguous()
-            if want_hidden:
-                hidden.append(x.view(nseq, L, H))
-            qkv_l, ao_l, in_l, out_l = (self._lin["l%d.%s" % (i, k)] for k in ("qkv", "ao", "inter", "out"))
-            g1, b1, _, _ = self._ln("l%d.ln1" % i)
-            g2, b2, _, _ = self._ln("l%d.ln2" % i)
-            qkv = new(M, 3 * H)
-            self._gemm_fwd(x, M, qkv_l, qkv)
-            ctx = new(M, H)
-            lse = new(nseq, heads, L, dtype=f32) if (need_backward or want_attn) else None
-            ops.attention_fwd(qkv, mask, ctx, lse, nseq, L, lt, heads, p_a, ls + 1)
-            if want_attn:       # same seed and bound word as the forward: the probabilities its context was made from
-                probs = new(nseq, heads, L, L, dtype=f32)
-                ops.attention_probs(qkv, mask, lse, probs, nseq, L, lt, heads, p_a, ls + 1)
-                attn.append(probs)
-            s1 = new(M, H)
-            self._gemm_fwd(ctx, M, ao_l, s1, residual=x, res_ld=H, dropout_p=p_h, dropout_seed=ls + 2)
-            a = new(M, H)
-            st1 = new(M, 2, dtype=f32)
-            ops.layernorm_fwd(s1, g1, b1, a, st1, eps)
-            u = new(M, in_l.n) if need_backward else None
-            gel = new(M, in_l.n)
-            if need_backward:
-                # u holds gelu'(pre-activation), not the pre-activation: the backward epilogue is then one multiply
-                self._gemm_fwd(a, M, in_l, gel, act=ops.ACT_GELU_STASH_GRAD, out2=u, out2_ld=in_l.n)
-            else:
-                self._gemm_fwd(a, M, in_l, gel, act=ops.ACT_GELU)
-            s2 = new(M, H)
-            self._gemm_fwd(gel, M, out_l, s2, residual=a, res_ld=H, dropout_p=p_h, dropout_seed=ls + 3)
-            y = new(M, H)
-            st2 = new(M, 2, dtype=f32)
-            ops.layernorm_fwd(s2, g2, b2, y, st2, eps)
-            if need_backward:
-                st["layers"].append(dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2, seed=ls))
-            if cap is not None:
-                cap["l%d" % i] = dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, gel=gel, u=u, s2=s2, st2=st2)
-            x = y
-            if cap is not None:
-                cap["layer%d" % i] = x.view(nseq, L, H)
-        st["x_last"] = x
-        # ---- pooler on the [CLS] rows (row pitch L*768, no gather) ----
-        pl = self._lin["pooler"]
-        pooled = new(nseq, H)
-        self._gemm_fwd(x, nseq, pl, pooled, a_ld=L * H, act=ops.ACT_TANH)
-        st["pooled"] = pooled
-        if cap is not None:
-            cap["pooled"] = pooled
-        if base is not None:
-            if want_hidden:
-                hidden.append(x.view(nseq, L, H))
-            out = (x.view(nseq, L, H), pooled, hidden, attn)
+        ops.embed_text_fwd(ids, word, pos, typ, g_t, b_t, x, st["stats_t"], nseq, lt, L, st["eps"], st["p_h"], st["seed"] + 1)
+
+    def _text_vectors_fwd(self, st, vec, x):
+        """BertEmbeddings from fp32 word vectors vec ([B' * Lt, H] rows, any row pitch): LN(vec + pos + type[0]) and dropout."""
+        nseq, _, _, _, _, lt, L = st["dims"]
+        g_t, b_t, _, _ = self._ln("emb.ln")
+        ops.embed_text_fwd_vectors(vec, self._emb("emb.pos")[0], self._emb("emb.type")[0], g_t, b_t, x, st["stats_t"], nseq, lt, L,
+                                   st["eps"], st["p_h"], st["seed"] + 1)
+
+    def _visual_fwd(self, st, grid, repeat, x):
+        """VisualInputEmbedding: frame mean, + row / col / type, LN and dropout into the visual rows of x."""
+        nseq, _, T, gh, gw, lt, L = st["dims"]
+        n_ex, s2v, _ = repeat
+        g_v, b_v, _, _ = self._ln("vis.ln")
+        ops.embed_visual_fwd(grid, s2v, n_ex, st["row_tab"], st["col_tab"], self._emb("vis.type")[0], g_v, b_v,
+                             x, st["stats_v"], nseq, T, gh, gw, lt, L, st["eps"], st["p_h"], st["seed"] + 2)
+
+    def _self_fwd(self, st, i, x, need_backward, want_attn):
+        """BertSelfAttention of layer i from its input rows x: (qkv, context, lse or None, post-dropout probabilities or None)."""
+        nseq, _, _, _, _, lt, L = st["dims"]
+        H, heads, M, dev = st["H"], st["heads"], nseq * L, x.device
+        ls = st["seed"] + 16 * (i + 1)
+        qkv = torch.empty(M, 3 * H, dtype=torch.bfloat16, device=dev)
+        self._gemm_fwd(x, M, self._lin["l%d.qkv" % i], qkv)
+        ctx = torch.empty(M, H, dtype=torch.bfloat16, device=dev)
+        lse = torch.empty(nseq, heads, L, dtype=torch.float32, device=dev) if (need_backward or want_attn) else None
+        ops.attention_fwd(qkv, st["mask"], ctx, lse, nseq, L, lt, heads, st["p_a"], ls + 1)
+        probs = None
+        if want_attn:       # same seed and bound word as the forward: the probabilities its context was made from
+            probs = torch.empty(nseq, heads, L, L, dtype=torch.float32, device=dev)
+            ops.attention_probs(qkv, st["mask"], lse, probs, nseq, L, lt, heads, st["p_a"], ls + 1)
+        return qkv, ctx, lse, probs
+
+    def _attn_out_fwd(self, st, i, ctx, x):
+        """BertSelfOutput: a = LN1(dropout(ctx Wao^T + b) + x); returns (s1, its LN stats, a)."""
+        M, H, dev = ctx.shape[0], st["H"], ctx.device
+        g1, b1, _, _ = self._ln("l%d.ln1" % i)
+        s1 = torch.empty(M, H, dtype=torch.bfloat16, device=dev)
+        self._gemm_fwd(ctx, M, self._lin["l%d.ao" % i], s1, residual=x, res_ld=H, dropout_p=st["p_h"], dropout_seed=st["seed"] + 16 * (i + 1) + 2)
+        a = torch.empty(M, H, dtype=torch.bfloat16, device=dev)
+        st1 = torch.empty(M, 2, dtype=torch.float32, device=dev)
+        ops.layernorm_fwd(s1, g1, b1, a, st1, st["eps"])
+        return s1, st1, a
+
+    def _inter_fwd(self, st, i, a, need_backward):
+        """BertIntermediate: (gel = GELU(a Win^T + b), u = gelu'(pre-activation) or None)."""
+        M, dev = a.shape[0], a.device
+        in_l = self._lin["l%d.inter" % i]
+        gel = torch.empty(M, in_l.n, dtype=torch.bfloat16, device=dev)
+        u = None
+        if need_backward:
+            # u holds gelu'(pre-activation), not the pre-activation: the backward epilogue is then one multiply
+            u = torch.empty(M, in_l.n, dtype=torch.bfloat16, device=dev)
+            self._gemm_fwd(a, M, in_l, gel, act=ops.ACT_GELU_STASH_GRAD, out2=u, out2_ld=in_l.n)
         else:
-            out = self._head_forward(pooled, st, nseq, p_h, seed, need_backward)
-        return out, (st if need_backward else None)
+            self._gemm_fwd(a, M, in_l, gel, act=ops.ACT_GELU)
+        return gel, u
+
+    def _out_fwd(self, st, i, gel, a):
+        """BertOutput: y = LN2(dropout(gel Wo^T + b) + a); returns (s2, its LN stats, y)."""
+        M, H, dev = gel.shape[0], st["H"], gel.device
+        g2, b2, _, _ = self._ln("l%d.ln2" % i)
+        s2 = torch.empty(M, H, dtype=torch.bfloat16, device=dev)
+        self._gemm_fwd(gel, M, self._lin["l%d.out" % i], s2, residual=a, res_ld=H, dropout_p=st["p_h"], dropout_seed=st["seed"] + 16 * (i + 1) + 3)
+        y = torch.empty(M, H, dtype=torch.bfloat16, device=dev)
+        st2 = torch.empty(M, 2, dtype=torch.float32, device=dev)
+        ops.layernorm_fwd(s2, g2, b2, y, st2, st["eps"])
+        return s2, st2, y
+
+    def _pooler_fwd(self, st, x):
+        """BertPooler on the [CLS] rows of x (row pitch L * H, no gather)."""
+        nseq, L = st["dims"][0], st["dims"][6]
+        pooled = torch.empty(nseq, st["H"], dtype=torch.bfloat16, device=x.device)
+        self._gemm_fwd(x, nseq, self._lin["pooler"], pooled, a_ld=L * st["H"], act=ops.ACT_TANH)
+        return pooled
 
     # generic 2-layer MLP head: dropout -> Linear -> ReLU -> Linear (modeling.py:534-539,552-553)
     def _mlp_head_forward(self, pooled, st, nseq, p_h, seed, num_out):
@@ -855,33 +1796,59 @@ class _ClipBertHeadModel(nn.Module):
     def _wgrad(self, li, dy, x, rows, x_ld=None):
         ops.gemm(**self._wgrad_kw(li, dy, x, rows, x_ld))
 
+    def _split_wgrad_kw(self, key, li, dy, x, rows):
+        """A weight gradient of a layer whose backward is split into nodes (the module path): one launch, pinned to the tile width
+        and K-split of the grouped launch _layer_backward issues for it (ops.group_wgrad: the layer's four, or its FFN and
+        attention pairs), so that each element is summed in the same order and observe-only hooks keep the bits."""
+        kw = self._wgrad_kw(li, dy, x, rows)
+        gmode = ops.group_wgrad
+        if gmode not in (1, 3, 4) or not dy.is_cuda:
+            return kw
+        cache = self.__dict__.setdefault("_wgrad_pins", {})
+        pins = cache.get((rows, gmode))
+        if pins is None:
+            lins = {k: self._lin["l0.%s" % k] for k in ("out", "inter", "ao", "qkv")}
+            pins = {}
+            for grp in ([("out", "inter"), ("ao", "qkv")] if gmode == 4 else [("out", "inter", "ao", "qkv")]):
+                # the plan query reads the descriptors' shapes only
+                plan = ops.gemm_wgrad_group_plan([self._wgrad_kw(lins[k], lins[k].gw, lins[k].gw, rows) for k in grp])
+                pins.update({k: plan for k in grp})
+            cache[(rows, gmode)] = pins
+        if pins[key] is None:
+            return kw
+        bn, split = pins[key]
+        return dict(kw, block_n=bn, split_k=split)
+
     def _dgrad(self, li, dy, rows, out, **kw):
         ops.gemm(mode=ops.CB_GEMM_NN, m=rows, n=li.k, k=li.n, a=dy, a_rows=rows, a_ld=li.n, b=li.w, b_rows=li.n, b_ld=li.k,
                  out=out, out_ld=kw.pop("out_ld", li.k), **kw)
 
-    def _mlp_head_backward(self, st, dlogits, nseq, H):
-        """Returns d(pooled) (bf16, [nseq, H])."""
+    def _mlp_head_backward(self, st, dlogits, nseq, H, tanh=True, grads=True):
+        """Returns d pooler pre-activation (bf16, [nseq, H]); tanh = False: d pooled_output. grads = False: no parameter gradient
+        is written."""
         dev = dlogits.device
         bf16 = torch.bfloat16
         c0, c2, pl = self._lin["cls0"], self._lin["cls2"], self._lin["pooler"]
         dl = torch.empty(nseq, c2.n, dtype=bf16, device=dev)
         ops.pad_cast(dlogits.float().contiguous() if dlogits.dtype != torch.float32 or not dlogits.is_contiguous() else dlogits, dl)
-        self._wgrad(c2, dl, st["c1"], nseq)
-        ops.colsum(dl, c2.gb, nseq, c2.n)
+        if grads:
+            self._wgrad(c2, dl, st["c1"], nseq)
+            ops.colsum(dl, c2.gb, nseq, c2.n)
         dc1 = torch.empty(nseq, c0.n, dtype=bf16, device=dev)
         self._dgrad(c2, dl, nseq, dc1, aux=st["c1"], aux_ld=c0.n, aux_mode=ops.AUX_RELU_MASK)
-        self._wgrad(c0, dc1, st["pd"], nseq)
-        ops.colsum(dc1, c0.gb, nseq, c0.n)
+        if grads:
+            self._wgrad(c0, dc1, st["pd"], nseq)
+            ops.colsum(dc1, c0.gb, nseq, c0.n)
         dpooled = torch.empty(nseq, H, dtype=bf16, device=dev)
         # d(pooler pre-activation) = (dc1 @ W0) * dropout_mask * tanh'(pooled)
-        self._dgrad(c0, dc1, nseq, dpooled, dropout_p=st["p_h"], dropout_seed=st["seed"] + 5, aux=st["pooled"], aux_ld=H,
-                    aux_mode=ops.AUX_TANH_GRAD)
+        tanh_kw = dict(aux=st["pooled"], aux_ld=H, aux_mode=ops.AUX_TANH_GRAD) if tanh else {}
+        self._dgrad(c0, dc1, nseq, dpooled, dropout_p=st["p_h"], dropout_seed=st["seed"] + 5, **tanh_kw)
         if self._capture is not None:
             self._capture.setdefault("bwd", {}).update(dl=dl, dc1=dc1)
         return dpooled
 
-    def _head_backward(self, st, dout, nseq, H):
-        return self._mlp_head_backward(st, dout, nseq, H)
+    def _head_backward(self, st, dout, nseq, H, tanh=True, grads=True):
+        return self._mlp_head_backward(st, dout, nseq, H, tanh, grads)
 
     def _backward_impl(self, st, dout, grid_needs_grad):
         try:
@@ -1069,21 +2036,128 @@ class _ClipBertHeadModel(nn.Module):
             self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
         return dxn
 
+    # ---- the backward's per-module pieces (the module path's split layers; the default path runs _layer_backward) --------
+    def _output_backward(self, st, i, ly, dy, sq, grads, fused):
+        """layer[i].output from the gradient dy at its output: (d intermediate_output, times gelu' when fused; ds2, the gradient
+        of its residual input attention_output)."""
+        M, H = dy.shape
+        p_h, ls = st["p_h"], ly["seed"]
+        in_l, out_l = self._lin["l%d.inter" % i], self._lin["l%d.out" % i]
+        g2, _, dg2, db2 = self._ln("l%d.ln2" % i)
+        dbo = out_l.gb
+        if not grads:
+            dg2 = db2 = dbo = None
+        ds2 = torch.empty(M, H, dtype=torch.bfloat16, device=dy.device)
+        ds2d = torch.empty_like(ds2) if p_h > 0 else None
+        ops.layernorm_bwd(dy, ly["s2"], ly["st2"], g2, ds2, ds2d, dg2, db2, dbo, p_h, ls + 3)
+        dd = ds2d if ds2d is not None else ds2
+        if grads:
+            kw = self._split_wgrad_kw("out", out_l, dd, ly["gel"], M)
+            sq.run(lambda: ops.gemm(**kw), dd, ly["gel"])
+        dgel = torch.empty(M, in_l.n, dtype=torch.bfloat16, device=dy.device)
+        if fused:
+            self._dgrad(out_l, dd, M, dgel, aux=ly["u"], aux_ld=in_l.n, aux_mode=ops.AUX_MUL)
+        else:
+            self._dgrad(out_l, dd, M, dgel)
+        return dgel, ds2
+
+    def _intermediate_backward(self, st, i, ly, du, sq, grads, residual):
+        """layer[i].intermediate from du, the gradient at its pre-activation: d attention_output, plus residual (ds2) in the
+        dgrad epilogue when given."""
+        M, H = du.shape[0], st["H"]
+        in_l = self._lin["l%d.inter" % i]
+        if grads:
+            kw = self._split_wgrad_kw("inter", in_l, du, ly["a"], M)
+            sq.run(lambda: (ops.gemm(**kw), ops.colsum(du, in_l.gb, M, in_l.n)), du, ly["a"])
+        da = torch.empty(M, H, dtype=torch.bfloat16, device=du.device)
+        if residual is None:
+            self._dgrad(in_l, du, M, da)
+        else:
+            self._dgrad(in_l, du, M, da, residual=residual, res_ld=H)
+        return da
+
+    def _self_output_backward(self, st, i, ly, da, sq, grads):
+        """layer[i].attention.output from the gradient da at its output: (d context, ds1 = the gradient of its residual input)."""
+        M, H = da.shape
+        p_h, ls = st["p_h"], ly["seed"]
+        ao_l = self._lin["l%d.ao" % i]
+        g1, _, dg1, db1 = self._ln("l%d.ln1" % i)
+        dbao = ao_l.gb
+        if not grads:
+            dg1 = db1 = dbao = None
+        ds1 = torch.empty(M, H, dtype=torch.bfloat16, device=da.device)
+        ds1d = torch.empty_like(ds1) if p_h > 0 else None
+        ops.layernorm_bwd(da, ly["s1"], ly["st1"], g1, ds1, ds1d, dg1, db1, dbao, p_h, ls + 2)
+        dd1 = ds1d if ds1d is not None else ds1
+        if grads:
+            kw = self._split_wgrad_kw("ao", ao_l, dd1, ly["ctx"], M)
+            sq.run(lambda: ops.gemm(**kw), dd1, ly["ctx"])
+        dctx = torch.empty(M, H, dtype=torch.bfloat16, device=da.device)
+        self._dgrad(ao_l, dd1, M, dctx)
+        return dctx, ds1
+
+    def _self_attention_backward(self, st, i, ly, dctx, dattn, sq, grads, residual):
+        """layer[i].attention.self from d context (the forward's own context O in the attention backward) and dattn, a gradient
+        of its map or None: the gradient at its input, plus residual (ds1) in the dgrad epilogue when given."""
+        nseq, _, _, _, _, lt, L = st["dims"]
+        H, heads = st["H"], st["heads"]
+        M = nseq * L
+        ls = ly["seed"]
+        qkv_l = self._lin["l%d.qkv" % i]
+        dqkv = torch.empty(M, 3 * H, dtype=torch.bfloat16, device=dctx.device)
+        ops.attention_bwd(ly["qkv"], st["mask"], ly["ctx"], dctx, ly["lse"], dqkv, nseq, L, lt, heads, st["p_a"], ls + 1)
+        if dattn is not None:
+            drow = torch.empty(nseq, heads, L, dtype=torch.float32, device=dctx.device)
+            ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn, drow, dqkv, nseq, L, lt, heads, st["p_a"], ls + 1)
+        if grads:
+            kw = self._split_wgrad_kw("qkv", qkv_l, dqkv, ly["x"], M)
+            sq.run(lambda: (ops.gemm(**kw), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
+        dxn = torch.empty(M, H, dtype=torch.bfloat16, device=dctx.device)
+        if residual is None:
+            self._dgrad(qkv_l, dqkv, M, dxn)
+        else:
+            self._dgrad(qkv_l, dqkv, M, dxn, residual=residual, res_ld=H)
+        return dxn
+
     def _embedding_backward(self, st, dx, grid_needs_grad, grads=True):
         """The text and visual embeddings from the gradient at their output dx; returns d visual_inputs (None unless
         grid_needs_grad). grads = False: no parameter gradient is written (the visual kernel's go to scratch)."""
+        if grads:
+            self._text_embedding_backward(st, st["ids"], dx)
+        return self._visual_embedding_backward(st, st["grid"], st["repeat"], dx, grid_needs_grad, grads)
+
+    def _text_embedding_backward(self, st, ids, dx):
+        """bert.embeddings' parameter gradients from the gradient at the encoder input dx (its text rows are read)."""
+        nseq, _, _, _, _, lt, L = st["dims"]
+        g_t, _, dg_t, db_t = self._ln("emb.ln")
+        (word, dword), (pos, dpos), (typ, dtyp) = self._emb("emb.word"), self._emb("emb.pos"), self._emb("emb.type")
+        ops.embed_text_bwd(dx, ids, word, pos, typ, g_t, st["stats_t"], dword, dpos, dtyp, dg_t, db_t, nseq, lt, L, st["p_h"],
+                           st["seed"] + 1)
+
+    def _text_vectors_backward(self, st, vec, dx, grads):
+        """bert.embeddings from the gradient at the encoder input dx when its word vectors came from word_embeddings: returns d vec
+        (fp32 [B' * Lt, H]); grads = False: the parameter gradients go to scratch."""
+        nseq, _, _, _, _, lt, L = st["dims"]
+        g_t, _, dg_t, db_t = self._ln("emb.ln")
+        (pos, dpos), (typ, dtyp) = self._emb("emb.pos"), self._emb("emb.type")
+        if not grads:
+            dpos, dtyp, dg_t, db_t = (torch.zeros_like(t) for t in (dpos, dtyp, dg_t, db_t))
+        dvec = torch.empty(nseq * lt, vec.shape[1], dtype=torch.float32, device=dx.device)
+        ops.embed_text_bwd_vectors(dx, vec, pos, typ, g_t, st["stats_t"], dvec, dpos, dtyp, dg_t, db_t, nseq, lt, L, st["p_h"],
+                                   st["seed"] + 1)
+        return dvec
+
+    def _visual_embedding_backward(self, st, grid, repeat, dx, grid_needs_grad, grads=True):
+        """bert.visual_embeddings from the gradient at the encoder input dx (its visual rows are read); returns d grid (None
+        unless grid_needs_grad)."""
         dev = dx.device
         H = _cfg(self.config, "hidden_size")
-        nseq, nvid, T, gh, gw, lt, L = st["dims"]
+        nseq, _, T, gh, gw, lt, L = st["dims"]
+        nvid = grid.shape[0]
         p_h = st["p_h"]
         bf16 = torch.bfloat16
-        n_ex, s2v, starts = st["repeat"]
-        g_t, _, dg_t, db_t = self._ln("emb.ln")
+        n_ex, s2v, starts = repeat
         g_v, _, dg_v, db_v = self._ln("vis.ln")
-        (word, dword), (pos, dpos), (typ, dtyp) = self._emb("emb.word"), self._emb("emb.pos"), self._emb("emb.type")
-        if grads:
-            ops.embed_text_bwd(dx, st["ids"], word, pos, typ, g_t, st["stats_t"], dword, dpos, dtyp, dg_t, db_t, nseq, lt, L, p_h,
-                               st["seed"] + 1)
         (row, drow), (col, dcol), (vtyp, dvtyp) = self._emb("vis.row"), self._emb("vis.col"), self._emb("vis.type")
         if not grads:
             if not grid_needs_grad:
@@ -1093,13 +2167,13 @@ class _ClipBertHeadModel(nn.Module):
         dgrid = torch.empty(nvid, T, gh, gw, H, dtype=bf16, device=dev) if grid_needs_grad else None
         sample = st.get("sample")
         if sample is None:
-            ops.embed_visual_bwd(dx, st["grid"], s2v, starts, n_ex, row, col, vtyp, g_v, st["stats_v"], dv_tmp, dgrid, drow, dcol, dvtyp,
+            ops.embed_visual_bwd(dx, grid, s2v, starts, n_ex, row, col, vtyp, g_v, st["stats_v"], dv_tmp, dgrid, drow, dcol, dvtyp,
                                  dg_v, db_v, nseq, nvid, T, gh, gw, lt, L, p_h, st["seed"] + 2)
         else:
             # sampled visual tokens (see _forward_impl): gradients of the (n_keep x 1) virtual grid, scattered back by index
             idx, gh0, gw0, row_s, col_s = sample
             drow_s, dcol_s = torch.zeros_like(row_s), torch.zeros_like(col_s)
-            ops.embed_visual_bwd(dx, st["grid"], s2v, starts, n_ex, row_s, col_s, vtyp, g_v, st["stats_v"], dv_tmp, dgrid, drow_s, dcol_s,
+            ops.embed_visual_bwd(dx, grid, s2v, starts, n_ex, row_s, col_s, vtyp, g_v, st["stats_v"], dv_tmp, dgrid, drow_s, dcol_s,
                                  dvtyp, dg_v, db_v, nseq, nvid, T, gh, gw, lt, L, p_h, st["seed"] + 2)
             if grads:
                 drow.index_add_(0, idx // gw0, drow_s)         # d(row[r] + col[c]) goes to both tables
@@ -1434,7 +2508,7 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
         v = _cfg(self.config, "vocab_size")
         return itm[:, :2], scores.view(nseq, lt, vp)[:, :, :v]
 
-    def _head_backward(self, st, douts, nseq, H):
+    def _head_backward(self, st, douts, nseq, H, tanh=True, grads=True):
         ditm, dscores = douts
         dev = st["x_last"].device
         bf16 = torch.bfloat16
@@ -1446,9 +2520,10 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
         if ditm is not None:
             dl = torch.empty(nseq, itm_l.n, dtype=bf16, device=dev)
             ops.pad_cast(ditm.float().contiguous(), dl)
-            self._wgrad(itm_l, dl, st["pooled"], nseq)
-            ops.colsum(dl, itm_l.gb, nseq, itm_l.n)
-            self._dgrad(itm_l, dl, nseq, dpre, aux=st["pooled"], aux_ld=H, aux_mode=ops.AUX_TANH_GRAD)
+            if grads:
+                self._wgrad(itm_l, dl, st["pooled"], nseq)
+                ops.colsum(dl, itm_l.gb, nseq, itm_l.n)
+            self._dgrad(itm_l, dl, nseq, dpre, **(dict(aux=st["pooled"], aux_ld=H, aux_mode=ops.AUX_TANH_GRAD) if tanh else {}))
             if cap is not None:
                 cap["dl"] = dl
         st["mlm_dx"] = None
@@ -1460,20 +2535,24 @@ class ClipBertForPreTraining(_ClipBertHeadModel):
             e = self._spec["emb.word"]
             gword = self._flat.grad[e["offset"]: e["offset"] + vp * H].view(vp, H)
             eb = self._spec["mlm_bias"]
-            ops.gemm(mode=ops.CB_GEMM_WGRAD, m=vp, n=H, k=R, a=ds, a_rows=R, a_ld=vp, b=st["mlm_t2"], b_rows=R, b_ld=H, out=gword,
-                     out_ld=H, out_fp32=1)
-            ops.colsum(ds, self._flat.grad[eb["offset"]: eb["offset"] + vp], R, vp)
+            if grads:
+                ops.gemm(mode=ops.CB_GEMM_WGRAD, m=vp, n=H, k=R, a=ds, a_rows=R, a_ld=vp, b=st["mlm_t2"], b_rows=R, b_ld=H, out=gword,
+                         out_ld=H, out_fp32=1)
+                ops.colsum(ds, self._flat.grad[eb["offset"]: eb["offset"] + vp], R, vp)
             dt2 = torch.empty(R, H, dtype=bf16, device=dev)
             ops.gemm(mode=ops.CB_GEMM_NN, m=R, n=H, k=vp, a=ds, a_rows=R, a_ld=vp, b=self._word_bf16, b_rows=vp, b_ld=H, out=dt2, out_ld=H)
             g, _, dg, db = self._ln("mlm_ln")
+            if not grads:
+                dg = db = None
             dt1 = torch.empty(R, H, dtype=bf16, device=dev)
             ops.layernorm_bwd(dt2, st["mlm_t1"], st["mlm_stats"], g, dt1, None, dg, db, None, 0.0, 0)
             # d(pre-GELU) = dt1 * gelu'(u): a dgrad-style epilogue needs a GEMM, so fold it into the dgrad of transform.dense
             # by first masking dt1 (relu_mask has no gelu form) -> use the NN GEMM of the *identity-free* path below
             du = torch.empty(R, H, dtype=bf16, device=dev)
             _gelu_bwd(dt1, st["mlm_u"], du)
-            self._wgrad(t_l, du, st["xt"], R)
-            ops.colsum(du, t_l.gb, R, H)
+            if grads:
+                self._wgrad(t_l, du, st["xt"], R)
+                ops.colsum(du, t_l.gb, R, H)
             dxt = torch.empty(R, H, dtype=bf16, device=dev)
             self._dgrad(t_l, du, R, dxt)
             st["mlm_dx"] = dxt

@@ -58,10 +58,14 @@ _SIGS = {
     "cb_maxpool2x2_relu_fwd": [_vp, _vp, _i, _i, _i, _i, _vp],
     "cb_maxpool2x2_relu_bwd": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "cb_relu_mask": [_vp, _vp, _vp, _i64, _vp],
+    "cb_embed_text_fwd_vectors": [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _u64, _vp],
+    "cb_embed_text_bwd_vectors": [_vp, _vp, _i64] + [_vp] * 9 + [_i, _i, _i, _i, _f, _u64, _vp],
+    "cb_embed_word_scatter": [_vp, _vp, _vp, _i, _i, _i, _vp],
     "cb_nhwc_intake": [_vp, _i, _i64, _i64, _i64, _i64, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp],
     # deterministic variants: the arguments of the plain entry point, then (scratch, scratch_bytes) before the stream
     "cb_layernorm_bwd_det": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _u64, _vp, _i64, _vp],
     "cb_embed_text_bwd_det": [_vp] * 12 + [_i, _i, _i, _i, _i, _f, _u64, _vp, _i64, _vp],
+    "cb_embed_text_bwd_vectors_det": [_vp, _vp, _i64] + [_vp] * 9 + [_i, _i, _i, _i, _f, _u64, _vp, _i64, _vp],
     "cb_embed_visual_bwd_det": [_vp, _vp, _vp, _vp, _i] + [_vp] * 12 + [_i, _i, _i, _i, _i, _i, _i, _i, _f, _u64, _vp, _i64, _vp],
     "cb_colsum_det": [_vp, _i64, _vp, _i, _i, _vp, _i64, _vp],
     "cb_clip_lse_loss_det": [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _i64, _vp],
@@ -70,6 +74,7 @@ _SIGS = {
     # scratch-size queries (int64 results)
     "cb_layernorm_bwd_scratch_bytes": [_i],
     "cb_embed_text_bwd_scratch_bytes": [_i, _i],
+    "cb_embed_text_bwd_vectors_scratch_bytes": [_i, _i],
     "cb_embed_visual_bwd_scratch_bytes": [_i, _i, _i],
     "cb_colsum_scratch_bytes": [_i, _i],
     "cb_clip_loss_scratch_bytes": [_i],
@@ -349,6 +354,15 @@ def gemm_workspace_bytes(kw):
     return int(L.lib().cb_gemm_workspace_bytes(_gemm_descs([kw])))
 
 
+def gemm_wgrad_group_plan(kws):
+    """cb_gemm_wgrad_group_plan: (tile width, K-split) cb_gemm_wgrad_group runs the problems with, or None when it runs them as
+    separate launches."""
+    bn, split = _c.c_int(0), _c.c_int(0)
+    if L.lib().cb_gemm_wgrad_group_plan(_gemm_descs(kws), len(kws), _c.byref(bn), _c.byref(split)) != 0:
+        raise RuntimeError("cb_gemm_wgrad_group_plan failed: %s" % L.lib().cb_last_error().decode())
+    return (bn.value, split.value) if bn.value else None
+
+
 def gemm_wgrad_group_workspace_bytes(kws):
     """cb_gemm_wgrad_group_workspace_bytes: the whole group's workspace (carried by the first descriptor)."""
     return int(L.lib().cb_gemm_wgrad_group_workspace_bytes(_gemm_descs(kws), len(kws)))
@@ -470,6 +484,28 @@ def embed_text_bwd_det(dh, ids, word, pos, type0, gamma, stats, dword, dpos, dty
     _call("cb_embed_text_bwd_det", _p(dh), _p(ids), _p(word), _p(pos), _p(type0), _p(gamma), _p(stats), _p(dword), _p(dpos),
           _p(dtype0), _p(dgamma), _p(dbeta), nseq, lt, l, word.shape[0], word.shape[1], p, seed, _p(scratch), scratch.numel() * 4,
           _s())
+
+
+def embed_text_fwd_vectors(vec, pos, type0, gamma, beta, out, stats, nseq, lt, l, eps, p, seed):
+    """cb_embed_text_fwd_vectors: the text embeddings from fp32 word vectors vec ([nseq * lt, 768] rows, any row pitch)."""
+    _call("cb_embed_text_fwd_vectors", _p(vec), vec.stride(0), _p(pos), _p(type0), _p(gamma), _p(beta), _p(out), _p(stats), nseq, lt,
+          l, vec.shape[1], eps, p, seed, _s())
+
+
+def embed_text_bwd_vectors(dh, vec, pos, type0, gamma, stats, dvec, dpos, dtype0, dgamma, dbeta, nseq, lt, l, p, seed):
+    """cb_embed_text_bwd_vectors (_det in deterministic mode): dvec[r] (fp32, contiguous) instead of a word-table scatter."""
+    if deterministic():
+        scratch = _scratch(int(_fn("cb_embed_text_bwd_vectors_scratch_bytes")(nseq, lt)), dh)
+        _call("cb_embed_text_bwd_vectors_det", _p(dh), _p(vec), vec.stride(0), _p(pos), _p(type0), _p(gamma), _p(stats), _p(dvec),
+              _p(dpos), _p(dtype0), _p(dgamma), _p(dbeta), nseq, lt, l, vec.shape[1], p, seed, _p(scratch), scratch.numel() * 4, _s())
+        return
+    _call("cb_embed_text_bwd_vectors", _p(dh), _p(vec), vec.stride(0), _p(pos), _p(type0), _p(gamma), _p(stats), _p(dvec), _p(dpos),
+          _p(dtype0), _p(dgamma), _p(dbeta), nseq, lt, l, vec.shape[1], p, seed, _s())
+
+
+def embed_word_scatter(ids, dvec, dword):
+    """cb_embed_word_scatter: dword[ids[r]] += dvec[r], one writer and one order per table row."""
+    _call("cb_embed_word_scatter", _p(ids), _p(dvec), _p(dword), ids.numel(), dword.shape[0], dword.shape[1], _s())
 
 
 def embed_visual_fwd(grid, seq2vid, n_ex, rowemb, colemb, type0, gamma, beta, out, stats, nseq, t, gh, gw, lt, l, eps, p,

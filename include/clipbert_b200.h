@@ -202,6 +202,10 @@ int cb_gemm(const cb_gemm_desc* desc, void* stream);
 int cb_gemm_tile_width(const cb_gemm_desc* desc);
 /* bytes of workspace a CB_GEMM_WGRAD descriptor needs in deterministic mode (0: one K-split, or not a weight gradient) */
 int64_t cb_gemm_workspace_bytes(const cb_gemm_desc* desc);
+/* the plan cb_gemm_wgrad_group runs n CB_GEMM_WGRAD problems with: *bn = tile width and *split = K-splits per problem, or 0 and 0
+ * when they run as separate cb_gemm launches. A single weight gradient with block_n = *bn and split_k = *split sums every output
+ * element in the group's order (ClipBertBaseModel's split layers, modeling.py); launches nothing */
+int cb_gemm_wgrad_group_plan(const cb_gemm_desc* descs, int n, int* bn, int* split);
 /* n independent CB_GEMM_WGRAD problems in ONE persistent launch: the weight gradients of the four Linear layers of a BertLayer
  * (autograd of transformers.py:238-301,363-381) or of the convs of one bottleneck block. The problems should share their
  * reduction length k (tokens / pixels); 1 <= n <= 8. One prologue and tail instead of n, no K-split when the group fills the SMs.
@@ -272,6 +276,25 @@ int cb_embed_text_bwd_det(const void* dh, const int64_t* ids, const float* word,
                           const float* gamma, const float* stats, float* dword, float* dpos, float* dtype0, float* dgamma,
                           float* dbeta, int nseq, int lt, int l, int vocab, int hidden, float dropout_p, uint64_t seed,
                           float* scratch, int64_t scratch_bytes, void* stream);
+/* BertEmbeddings from word vectors (transformers.py:172-199: inputs_embeds = word_embeddings(input_ids), then + position +
+ * token type, LayerNorm, dropout), for a hook on word_embeddings that sees or replaces word[ids]. vec: fp32 rows, row
+ * r = b * lt + t at vec + r * vec_ld (vec_ld >= 768, a multiple of 4; 16-byte aligned); otherwise as cb_embed_text_fwd / _bwd /
+ * _bwd_det, the same stats, dropout masks and parameter-gradient order. The backward writes dvec[r] (fp32, contiguous
+ * [nseq * lt, 768], one writer per element) instead of adding into a word table; cb_embed_word_scatter adds such rows into the
+ * table: every table row word[id] receives the sum of the rows carrying id, in row order, added once (one writer per table row,
+ * the same bits in both modes). Scratch of _det: cb_embed_text_bwd_vectors_scratch_bytes. */
+int cb_embed_text_fwd_vectors(const float* vec, int64_t vec_ld, const float* pos, const float* type0, const float* gamma,
+                              const float* beta, void* out, float* stats, int nseq, int lt, int l, int hidden, float eps,
+                              float dropout_p, uint64_t seed, void* stream);
+int cb_embed_text_bwd_vectors(const void* dh, const float* vec, int64_t vec_ld, const float* pos, const float* type0,
+                              const float* gamma, const float* stats, float* dvec, float* dpos, float* dtype0, float* dgamma,
+                              float* dbeta, int nseq, int lt, int l, int hidden, float dropout_p, uint64_t seed, void* stream);
+int64_t cb_embed_text_bwd_vectors_scratch_bytes(int nseq, int lt);
+int cb_embed_text_bwd_vectors_det(const void* dh, const float* vec, int64_t vec_ld, const float* pos, const float* type0,
+                                  const float* gamma, const float* stats, float* dvec, float* dpos, float* dtype0, float* dgamma,
+                                  float* dbeta, int nseq, int lt, int l, int hidden, float dropout_p, uint64_t seed, float* scratch,
+                                  int64_t scratch_bytes, void* stream);
+int cb_embed_word_scatter(const int64_t* ids, const float* dvec, float* dword, int rows, int vocab, int hidden, void* stream);
 int64_t cb_embed_visual_bwd_scratch_bytes(int nseq, int gh, int gw);
 int cb_embed_visual_bwd_det(const void* dh, const void* grid, const int32_t* seq2vid, const int32_t* vid_start, int n_ex,
                             const float* rowemb, const float* colemb, const float* type0, const float* gamma,
