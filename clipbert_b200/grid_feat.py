@@ -392,6 +392,15 @@ class _CnnFn(torch.autograd.Function):
 
 
 class GridFeatBackbone(nn.Module):
+    """``model.recompute_activations = True`` (default False) trades compute for activation memory, as wrapping each ResNet stage
+    in ``torch.utils.checkpoint`` does on the reference: a pass that records autograd keeps only each stage's input (the pooled
+    stem output for res2, the previous stage's output for the others) instead of every block's activations, and the backward
+    re-runs the stage's blocks from it, with the forward's launches, just before that stage's backward. One stage's activations
+    are alive at a time; the gradients are bit-identical to the switch off in deterministic mode. Refused together with hooks on
+    the CNN's modules (the module path keeps every block's activations as its nodes' saved tensors)."""
+
+    recompute_activations = False
+
     def __init__(self, detectron2_model_cfg=None, config=None, input_format="BGR", freeze_at=2):
         super().__init__()
         assert input_format == "BGR", "detectron 2 image input format should be BGR"
@@ -593,6 +602,10 @@ class GridFeatBackbone(nn.Module):
         _require_cuda(x)
         self._ensure_ready(x.device)
         if self._hooked():
+            if self.recompute_activations and torch.is_grad_enabled():
+                raise RuntimeError("GridFeatBackbone: recompute_activations cannot be combined with hooks on the CNN's modules: the "
+                                   "module path keeps every block's activations for its nodes' backward; remove the hooks or turn "
+                                   "the switch off")
             return self._module_forward(x)
         if not (torch.is_grad_enabled() and (x.requires_grad or self._any_trainable())):
             return self._forward_impl(x, need_backward=False)[0]
@@ -685,29 +698,33 @@ class GridFeatBackbone(nn.Module):
 
     def _forward_impl(self, images, need_backward, frames_grad=False):
         """``frames_grad``: the backward also computes the gradient with respect to the frames, so the stem output and every
-        block's activations (frozen blocks too) are kept."""
+        block's activations (frozen blocks too) are kept. With ``recompute_activations`` the stash keeps each such stage's input
+        instead of its blocks' activations (``stages``); _backward_impl re-runs the blocks."""
         bsz, n_frms, c, h, w = images.shape
         assert c == 3
         n = bsz * n_frms
         cur, frames, hh, ww = self._stem_forward(images.reshape(n, c, h, w), need_backward and frames_grad)
+        recompute = need_backward and self.recompute_activations
         # ---- res2..res5 ----
-        blocks = []
+        blocks, stages = [], []
         bb = self.feature.backbone
         stage_names = [s[0] for s in RESNET50_STAGES]
         for si, name in enumerate(stage_names):
             stage = getattr(bb, name)
             for bi, blk in enumerate(stage):
                 last = (si == len(stage_names) - 1) and (bi == len(stage) - 1)
-                if self._inject is not None and ("%s.%d" % (name, bi)) in self._inject:
-                    # test hook: this block starts from a given NHWC activation (layer-local parity: both implementations see the same input)
-                    cur = self._inject["%s.%d" % (name, bi)].to(device=cur.device, dtype=torch.bfloat16).reshape(n * hh * ww, -1).contiguous()
+                cur = self._injected(name, bi, cur, n, hh, ww)
+                if bi == 0:
+                    stage_in = dict(name=name, x=cur, h=hh, w=ww)
                 st = self._block_forward(blk, cur, n, hh, ww, last)
                 hh, ww = st["h"], st["w"]
                 keep = need_backward and (st["trainable"] or frames is not None)     # a frozen block's dgrad chain leads to the frames
-                if not keep:
+                if not keep or recompute:
                     self._pad_put(st["a_pad"], n, hh, ww)     # consumed by conv2 above; stream order makes the reuse safe
                 else:
                     blocks.append(st)
+                if keep and recompute and bi == 0:
+                    stages.append(stage_in)
                 cur = st["y"]
             if self._capture is not None:
                 self._capture[name] = (cur.view(n, hh + 2, ww + 2, -1)[:, 1:-1, 1:-1] if name == "res5" else cur.view(n, hh, ww, -1))
@@ -723,10 +740,32 @@ class GridFeatBackbone(nn.Module):
         if not need_backward:
             self._pad_put(cur, n, hh, ww)           # res5 output (padded), consumed by the grid_encoder conv
         if need_backward:
-            stash = dict(n=n, h=hh, w=ww, res5_pad=cur, gconv=gconv, blocks=blocks, frames=frames)
+            stash = dict(n=n, h=hh, w=ww, res5_pad=cur, gconv=gconv, blocks=blocks, stages=stages, frames=frames)
             if self._capture is not None:
                 self._capture["stash"] = stash
         return grid, stash
+
+    def _injected(self, name, bi, cur, n, h, w):
+        """The input of block name.bi: cur, or the NHWC activation a test injected there (layer-local parity: both implementations
+        see the same input)."""
+        key = "%s.%d" % (name, bi)
+        if self._inject is None or key not in self._inject:
+            return cur
+        return self._inject[key].to(device=cur.device, dtype=torch.bfloat16).reshape(n * h * w, -1).contiguous()
+
+    def _recompute_stage(self, sg, n):
+        """The activations of one stage's blocks as _block_forward returned them in the forward, re-run from the stage's kept
+        input with the same launches (recompute_activations). The last block's conv3 is not re-run: its output is the next stage's
+        kept input, or res5_pad, and no block backward reads a block's own output."""
+        blocks = []
+        cur, hh, ww = sg["x"], sg["h"], sg["w"]
+        stage = getattr(self.feature.backbone, sg["name"])
+        for bi, blk in enumerate(stage):
+            cur = self._injected(sg["name"], bi, cur, n, hh, ww)
+            st = self._block_forward(blk, cur, n, hh, ww, blk.block_name == RESNET50_LAST_BLOCK, need_y=bi < len(stage) - 1)
+            hh, ww, cur = st["h"], st["w"], st["y"]
+            blocks.append(st)
+        return blocks
 
     def _stem_forward(self, x, keep_frames):
         """x: (n, 3, h, w) frames. Returns (pooled stem output, compact [n*hh*ww, 64]; what the frame gradient needs when
@@ -794,9 +833,10 @@ class GridFeatBackbone(nn.Module):
             self._capture["stem"] = cur.view(n, hh, ww, 64)
         return cur, frames, hh, ww
 
-    def _block_forward(self, blk, x_in, n, h_in, w_in, last):
+    def _block_forward(self, blk, x_in, n, h_in, w_in, last, need_y=True):
         """One bottleneck block from x_in (compact [n*h_in*w_in, cin]). Its output y is compact, or zero-bordered for the last
-        block (the grid_encoder conv reads it). Returns the block's activations as its backward reads them."""
+        block (the grid_encoder conv reads it); need_y = False (a recompute whose output is kept elsewhere): no shortcut and
+        conv3 launches, y None. Returns the block's activations as its backward reads them."""
         dev, bf16 = x_in.device, torch.bfloat16
         hh, ww = h_in, w_in
         if blk.stride == 2:
@@ -806,10 +846,13 @@ class GridFeatBackbone(nn.Module):
         else:
             xs = x_in
         rows = n * hh * ww
-        sc = self._conv1x1(blk.shortcut, xs, rows, ops.ACT_NONE) if blk.has_shortcut else xs
+        sc = self._conv1x1(blk.shortcut, xs, rows, ops.ACT_NONE) if blk.has_shortcut and need_y else xs
         a_pad = self._pad_get(n, hh, ww, blk.mid, dev)
         self._conv1x1(blk.conv1, xs, rows, ops.ACT_RELU, rowmap=ops.ROWMAP_PAD, hw=(hh, ww), out=a_pad)
         b = self._conv3x3(blk.conv2, a_pad, n, hh, ww, ops.ACT_RELU)
+        if not need_y:
+            return dict(name=blk.block_name, blk=blk, x_in=x_in, xs=xs, a_pad=a_pad, b=b, y=None, h=hh, w=ww, h_in=h_in, w_in=w_in,
+                        trainable=blk.conv1.weight.requires_grad)
         if last:
             y = self._pad_get(n, hh, ww, blk.cout, dev)
             self._conv1x1(blk.conv3, b, rows, ops.ACT_RELU, residual=sc, rowmap=ops.ROWMAP_PAD, hw=(hh, ww), out=y)
@@ -876,23 +919,27 @@ class GridFeatBackbone(nn.Module):
         if cap is not None:
             cap["grid_encoder"] = dict(dg_pad=dg_pad)
         blocks = stash["blocks"]
+        stages = stash["stages"]
         frames = stash["frames"]
-        g = self._grid_conv_backward(dg_pad, res5_pad, n, h, w, sq, ge.weight.requires_grad, bool(blocks))
+        g = self._grid_conv_backward(dg_pad, res5_pad, n, h, w, sq, ge.weight.requires_grad, bool(blocks or stages))
         del dg_pad
-        for st in reversed(blocks):
-            lowest = st is blocks[0]
-            bucket = None
-            if st["trainable"] and last and self._bucket_hook is not None and st["name"] == "res5.0":
-                # every weight gradient of res5 + grid_encoder (78 % of the CNN's trainable parameters, the tail of the
-                # flat buffer) has been enqueued: its exchange can overlap the res4 / res3 backward
-                bucket = lambda blk=st["blk"]: self._bucket_hook(self._flat.grad, blk.shortcut._e["offset"], sq.side if sq.forked else None)  # noqa: E731
-            # d2 FREEZE_AT: no gradient below the lowest block, unless it leads to the frames
-            need_dx = not lowest or (st["blk"].has_shortcut and frames is not None)
-            gin = self._block_backward(st, g, n, sq, recycle, cap=cap, need_dx=need_dx, bucket=bucket)
-            recycle.append((st["a_pad"], n, st["h"], st["w"]))
-            if gin is None:
-                break
-            g = gin
+        if stages:
+            # recompute_activations: top-down, each stage's blocks re-run from its kept input, then its backward. The join makes
+            # the main stream wait for the stage's weight gradients, the last readers of its activations, before those are
+            # released; the next stage then recomputes into that memory. Of the stage's zero-bordered buffers (a_pad, db_pad of
+            # each block) the pool keeps one, the buffer the next forward reuses block by block; the others go back to the
+            # allocator, since no other stage has their geometry, and the next backward allocates them zeroed again
+            for sg in reversed(stages):
+                blocks = self._recompute_stage(sg, n)
+                stage_recycle = []
+                g = self._blocks_backward(blocks, g, n, sq, stage_recycle, cap, frames, last, lowest=sg is stages[0])
+                sq.join()
+                for t, tn, th, tw in stage_recycle:
+                    if not self._pad_pool.get((tn, th, tw, t.shape[1])):
+                        self._pad_put(t, tn, th, tw)
+                del blocks, stage_recycle
+        else:
+            g = self._blocks_backward(blocks, g, n, sq, recycle, cap, frames, last, lowest=True)
         dx = None
         if frames is not None:
             dx = self._stem_backward(g, frames, n, cap)
@@ -902,6 +949,24 @@ class GridFeatBackbone(nn.Module):
         if not self._optimizer_emits_packed and self._any_trainable():
             self._dirty = True   # an optimizer step normally follows: repack bf16 operands on the next forward
         return dx
+
+    def _blocks_backward(self, blocks, g, n, sq, recycle, cap, frames, last, lowest):
+        """The backward of consecutive blocks, top-down from g; returns the gradient below the first of them, or None when none
+        is needed. ``lowest``: blocks[0] is the lowest block that runs a backward."""
+        for st in reversed(blocks):
+            bucket = None
+            if st["trainable"] and last and self._bucket_hook is not None and st["name"] == "res5.0":
+                # every weight gradient of res5 + grid_encoder (78 % of the CNN's trainable parameters, the tail of the
+                # flat buffer) has been enqueued: its exchange can overlap the res4 / res3 backward
+                bucket = lambda blk=st["blk"]: self._bucket_hook(self._flat.grad, blk.shortcut._e["offset"], sq.side if sq.forked else None)  # noqa: E731
+            # d2 FREEZE_AT: no gradient below the lowest block, unless it leads to the frames
+            need_dx = not (lowest and st is blocks[0]) or (st["blk"].has_shortcut and frames is not None)
+            gin = self._block_backward(st, g, n, sq, recycle, cap=cap, need_dx=need_dx, bucket=bucket)
+            recycle.append((st["a_pad"], n, st["h"], st["w"]))
+            if gin is None:
+                return None
+            g = gin
+        return g
 
     def _grid_conv_backward(self, dg_pad, res5_pad, n, h, w, sq, wgrad, need_dx, mask=True):
         """grid_encoder conv from dg_pad (zero-bordered gradient at its output): its weight gradient on the side queue (wgrad) and

@@ -204,10 +204,18 @@ class ClipBertBaseModel(nn.Module):
     visual_embeddings, encoder, each layer's attention (self, output), intermediate and output, pooler - so torch's hooks on them
     fire, and a forward hook or pre-hook may replace what they return or receive. The backward is a chain of nodes split at the
     hooked modules. INTEGRATION.md lists what each module hands to its hooks and the hooks that are refused.
+
+    ``model.recompute_activations = True`` (default False; also on ``head.bert``) trades compute for activation memory, as
+    wrapping each BertLayer in ``torch.utils.checkpoint`` does on the reference: a pass that records autograd keeps only each
+    encoder layer's input hidden state, and the backward re-runs the layer's forward (same launches, seeds and dropout word, so
+    the same masks, under CUDA-graph replay too) just before that layer's backward. The gradients are bit-identical to the
+    switch off in deterministic mode. Refused together with ``differentiable_attentions``, ``layerwise_autograd`` and module
+    hooks, whose backward reads every layer's activations as saved tensors.
     """
 
     differentiable_attentions = False
     layerwise_autograd = False
+    recompute_activations = False
 
     def __init__(self, config, _engine=None):
         super().__init__()
@@ -1457,9 +1465,14 @@ class _ClipBertHeadModel(nn.Module):
         ids = text_input_ids.contiguous()
         mask = attention_mask.to(torch.int64).contiguous()
         flags = (bool(want_hidden), bool(want_attn), bool(want_attn and diff_attn))
-        if torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters())) and layerwise:
+        records = torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters()))
+        if records and self.bert.recompute_activations and (diff_attn or layerwise):
+            raise RuntimeError("ClipBertBaseModel: recompute_activations cannot be combined with %s: its backward reads every "
+                               "layer's activations; turn one of the switches off" %
+                               ("differentiable_attentions" if diff_attn else "layerwise_autograd"))
+        if records and layerwise:
             seq, pooled, hidden, attn = self._run_layerwise(ids, grid, mask, flags)
-        elif torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters())):
+        elif records:
             outs = _BaseModelFn.apply(self, grid, self.bert.pooler.dense.weight, ids, mask, flags)
             n_hidden = len(self.bert.encoder.layer) + 1 if flags[0] else 0
             seq, pooled, hidden, attn = outs[0], outs[1], outs[2:2 + n_hidden], outs[2 + n_hidden:]
@@ -1551,6 +1564,10 @@ class _ClipBertHeadModel(nn.Module):
         if hooked and self._grad_ready_hook is not None:
             raise RuntimeError("ClipBertBaseModel: hooks on the transformer's modules are for analysis, not data-parallel training: "
                                "they cannot run while the overlapped gradient exchange (enable_overlapped_allreduce) is enabled")
+        if hooked and self.bert.recompute_activations and torch.is_grad_enabled():
+            raise RuntimeError("ClipBertBaseModel: recompute_activations cannot be combined with hooks on the transformer's modules: "
+                               "the module path keeps every layer's activations for its nodes' backward; remove the hooks or turn "
+                               "the switch off")
         return hooked
 
     def _run_modules(self, ids, visual_inputs, mask, repeat, hooked):
@@ -1620,6 +1637,7 @@ class _ClipBertHeadModel(nn.Module):
                        idx=None if st["sample"] is None else st["sample"][0], row_tab=st["row_tab"], col_tab=st["col_tab"])
         # ---- encoder ----
         hidden, attn = [], []
+        recompute = need_backward and self.bert.recompute_activations
         for i in range(len(self.bert.encoder.layer)):
             if self._inject is not None and i in self._inject:      # test hook: layer-local parity (same input on both sides)
                 x = self._inject[i].to(device=ids.device, dtype=torch.bfloat16).reshape(M, H).contiguous()
@@ -1632,7 +1650,9 @@ class _ClipBertHeadModel(nn.Module):
             gel, u = self._inter_fwd(st, i, a, need_backward)
             s2, st2, y = self._out_fwd(st, i, gel, a)
             ls = seed + 16 * (i + 1)
-            if need_backward:
+            if need_backward and recompute:
+                st["layers"].append(dict(x=x, seed=ls, recompute=True))    # the rest is re-run before the layer's backward
+            elif need_backward:
                 st["layers"].append(dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2, seed=ls))
             if cap is not None:
                 cap["l%d" % i] = dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, gel=gel, u=u, s2=s2, st2=st2)
@@ -1885,9 +1905,16 @@ class _ClipBertHeadModel(nn.Module):
                 dx += dhidden[i + 1]
             if ret_hidden is not None:
                 _set_retained_hidden_grad(ret_hidden[i + 1], dx, nseq, L, H)
-            dx = self._layer_backward(st, i, st["layers"][i], dx, sq, cap, None if dattn is None else dattn[i],
+            ly = st["layers"][i]
+            if ly.get("recompute"):
+                # recompute_activations: the layer's forward re-run from its kept input under this pass's seeds and bound dropout
+                # word (the forward's masks), beside the weight gradients of the layer above; then the join makes the main
+                # stream wait for those, their activations' last readers, and drops them
+                ly = self._recompute_layer(st, i, ly)
+                sq.join()
+            dx = self._layer_backward(st, i, ly, dx, sq, cap, None if dattn is None else dattn[i],
                                       None if ret_attn is None else ret_attn[i])
-            st["layers"][i] = None     # free this layer's stash
+            st["layers"][i] = ly = None     # free this layer's stash
         if dhidden is not None and dhidden[0] is not None:                 # hidden_states[0] = the embedding output
             if cap is not None and len(st["layers"]):
                 cap["l0"]["dxn"] = dx.clone()
@@ -1901,6 +1928,16 @@ class _ClipBertHeadModel(nn.Module):
         if not self._optimizer_emits_packed:
             self._dirty = True
         return dgrid
+
+    def _recompute_layer(self, st, i, ly):
+        """Encoder layer i's stash as the forward kept it, from its kept input ly["x"]: the forward's launches, seeds and (bound by
+        the caller) dropout word, so every tensor is the forward's bit for bit. The layer output is not needed."""
+        x = ly["x"]
+        qkv, ctx, lse, _ = self._self_fwd(st, i, x, True, False)
+        s1, st1, a = self._attn_out_fwd(st, i, ctx, x)
+        gel, u = self._inter_fwd(st, i, a, True)
+        s2, st2, _ = self._out_fwd(st, i, gel, a)
+        return dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2, seed=ly["seed"])
 
     def _pooler_backward(self, dpre, x_last, nseq, L, H, grads=True):
         """d pooler pre-activation (None: no gradient) -> the gradient at the top of the encoder, [nseq * L, H] bf16 with the [CLS]
