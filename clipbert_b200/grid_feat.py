@@ -22,7 +22,7 @@ import torch
 from torch import nn
 
 from . import ops
-from .modeling import _will_execute
+from .modeling import _engine_runs
 from .params import FlatGroup
 
 RESNET50_STAGES = (("res2", 3, 64, 256, 1), ("res3", 4, 128, 512, 2), ("res4", 6, 256, 1024, 2), ("res5", 3, 512, 2048, 2))
@@ -197,7 +197,8 @@ class _BlockNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         ps, blk = ctx.ps, ctx.blk
-        need_dx, grads = _will_execute(ctx, 0), ctx.has_anchor and _will_execute(ctx, 1)
+        need_dx = _engine_runs(ctx.next_functions[0][0], False)
+        grads = ctx.has_anchor and _engine_runs(ctx.next_functions[1][0], False)
         if not (need_dx or grads):
             return None, None, None, None
         xs, a_pad, b, y = ctx.saved_tensors
@@ -223,7 +224,8 @@ class _GridConvNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dg):
         ps, (h, w) = ctx.ps, ctx.hw
-        need_dx, grads = _will_execute(ctx, 0), ctx.has_anchor and _will_execute(ctx, 1)
+        need_dx = _engine_runs(ctx.next_functions[0][0], False)
+        grads = ctx.has_anchor and _engine_runs(ctx.next_functions[1][0], False)
         if not (need_dx or grads):
             return None, None, None
         res5, = ctx.saved_tensors

@@ -5,8 +5,8 @@ Mirrors the reference classes in ``src/modeling/modeling.py`` / ``src/modeling/t
 ClipBertForMultipleChoice, ClipBertForPreTraining): same constructor (a BertConfig-like object),
 same forward signatures and return dicts, same state_dict keys (SURVEY.md App. B). The torch.nn
 modules below are parameter containers whose ``forward`` runs only on the module path: when a hook is registered on bert or a
-module below it, bert(...) and the heads call them (_BertPass), each running its part of the engine. All arithmetic
-is the hand-written sm_90a kernels behind libclipbert_sm90.so:
+module below it, bert(...) and the heads call them (_BertPass), each running its part of the engine; so does bert(...) with
+layerwise_autograd on. All arithmetic is the hand-written sm_90a kernels behind libclipbert_sm90.so:
 
   embeddings     cb_embed_text_fwd / cb_embed_visual_fwd (gather + sum + LN + dropout; the visual
                  kernel also fuses the frame mean, the row/col/type adds, repeat_tensor_rows and
@@ -189,10 +189,11 @@ class ClipBertBaseModel(nn.Module):
 
     By default the whole pass is one autograd node: a tensor hook on a map or hidden state fires before that node runs and sees
     only the loss's direct term, and ``torch.autograd.grad(score, attentions)`` (or hidden states) returns only that term.
-    ``model.layerwise_autograd = True`` (default False; also on ``head.bert``) makes a pass that records autograd a chain of
-    nodes - the embeddings, one node per encoder layer (two when the maps are differentiable: A_k, hidden_states[k] ->
-    attentions[k], and C_k, (hidden_states[k], attentions[k]) -> hidden_states[k + 1], the reference's dataflow) and the
-    pooler - with sequence_output the same tensor as hidden_states[12]. Tensor hooks, ``torch.autograd.grad``,
+    ``model.layerwise_autograd = True`` (default False; also on ``head.bert``) runs a pass that records autograd through the
+    modules, as a hook does (below), so that it is a chain of nodes - the embeddings, one node per encoder layer
+    (two when the maps are differentiable: A_k, hidden_states[k] -> attentions[k], and C_k, (hidden_states[k], attentions[k])
+    -> hidden_states[k + 1], the reference's dataflow) and the pooler - with sequence_output the same tensor as
+    hidden_states[12]. With a hook set as well, the hooks decide where the chain splits. Tensor hooks, ``torch.autograd.grad``,
     ``retain_grad()`` and ``backward(inputs=...)`` on any map or hidden state then follow torch's semantics, and a hook that
     rewrites a map's gradient changes every gradient below that layer. Parameter gradients too: a node writes them only when
     the backward accumulates into the parameters (``autograd.grad`` leaves the flat gradient buffer as it was), and
@@ -236,11 +237,11 @@ class ClipBertBaseModel(nn.Module):
         eng = self._engine
         ps = _BERT_PASSES[-1] if _BERT_PASSES and _BERT_PASSES[-1].awaits(eng) else None
         if ps is None:
-            hooked = eng._bert_hooked()
-            if not hooked:
+            ps, records = eng._base_pass(visual_inputs)
+            if ps is None:
                 return eng._run_base(text_input_ids, visual_inputs, attention_mask, self.output_hidden_states, self.output_attentions,
-                                     self.differentiable_attentions, self.layerwise_autograd)
-            with _BertPass(eng, hooked) as ps:
+                                     self.differentiable_attentions, records)
+            with ps:
                 return ps.base(text_input_ids, visual_inputs, attention_mask)
         return ps.base(text_input_ids, visual_inputs, attention_mask)
 
@@ -346,150 +347,6 @@ class _BaseModelFn(torch.autograd.Function):
 _LAYER_STASH = ("x", "qkv", "ctx", "lse", "s1", "st1", "a", "u", "gel", "s2", "st2")
 
 
-class _LayerwisePass:
-    """What the nodes of one layerwise bert(...) pass share: the engine, the pass's stash (its per-layer activations move into the
-    nodes' saved tensors) and the hand-over from C_k to A_k of a map-split layer (dqkv with its V block, ds1)."""
-
-    def __init__(self, module, st):
-        self.module, self.st, self.handover = module, st, {}
-
-    def dims(self):
-        nseq, _, _, _, _, _, L = self.st["dims"]
-        return nseq, L, _cfg(self.module.config, "hidden_size")
-
-    def dense(self, g):
-        """An upstream gradient of a hidden state as the engine's [nseq * L, H] contiguous bf16 operand."""
-        nseq, L, H = self.dims()
-        return g.reshape(nseq * L, H).to(torch.bfloat16).contiguous()
-
-    def hidden(self, i):
-        """hidden_states[i] as a fresh view: the input of layer i, or the top of the encoder."""
-        nseq, L, H = self.dims()
-        layers = self.st["layers"]
-        return (layers[i]["x"] if i < len(layers) else self.st["x_last"]).view(nseq, L, H)
-
-
-def _will_execute(ctx, k):
-    """Whether the engine runs, in the current backward, the node behind tensor input k of this node (False when that input
-    takes no gradient). For a parameter anchor: whether this backward accumulates into the parameters - backward() does;
-    torch.autograd.grad() and backward(inputs=...) without the parameter do not."""
-    node = ctx.next_functions[k][0]
-    if node is None:
-        return False
-    try:
-        return bool(torch._C._will_engine_execute_node(node))
-    except RuntimeError:        # autograd.grad() with the anchor parameter among its inputs: no accumulation into .grad
-        return False
-
-
-class _EmbeddingNode(torch.autograd.Function):
-    """(visual_inputs, anchor) -> hidden_states[0]."""
-
-    @staticmethod
-    def forward(ctx, ps, grid, anchor):
-        st = ps.st
-        ctx.ps = ps
-        ctx.save_for_backward(st.pop("ids"), st.pop("grid"), st.pop("stats_t"), st.pop("stats_v"))
-        return ps.hidden(0)
-
-    @staticmethod
-    def backward(ctx, dh):
-        ids, grid, stats_t, stats_v = ctx.saved_tensors
-        ps = ctx.ps
-        grads, need_grid = _will_execute(ctx, 1), _will_execute(ctx, 0)
-        if not (grads or need_grid):
-            return None, None, None
-        st = dict(ps.st, ids=ids, grid=grid, stats_t=stats_t, stats_v=stats_v)
-        with ps.module._node_backward(st, grads):
-            dgrid = ps.module._embedding_backward(st, ps.dense(dh), need_grid, grads)
-        return None, dgrid, None
-
-
-class _LayerNode(torch.autograd.Function):
-    """Encoder layer i, hidden_states[i] -> hidden_states[i + 1] (maps not differentiable)."""
-
-    @staticmethod
-    def forward(ctx, ps, i, h, anchor):
-        ly = ps.st["layers"][i]
-        ctx.ps, ctx.i, ctx.seed = ps, i, ly["seed"]
-        ctx.save_for_backward(*(ly[k] for k in _LAYER_STASH))
-        return ps.hidden(i + 1)
-
-    @staticmethod
-    def backward(ctx, dy):
-        ly = dict(zip(_LAYER_STASH, ctx.saved_tensors), seed=ctx.seed)
-        ps, grads = ctx.ps, _will_execute(ctx, 1)
-        with ps.module._node_backward(ps.st, grads) as sq:
-            dxn = ps.module._layer_backward(ps.st, ctx.i, ly, ps.dense(dy), sq, grads=grads)
-        return None, None, dxn.view(*ps.dims()), None
-
-
-class _MapNode(torch.autograd.Function):
-    """A_k: hidden_states[k] -> attentions[k]. Its backward receives the map's full gradient G (the direct term, C_k's dO V^T and
-    whatever hooks made of them) and finishes layer k: dQ / dK from G, the QKV weight gradient, the dgrad to hidden_states[k]."""
-
-    @staticmethod
-    def forward(ctx, ps, i, h, anchor):
-        ly = ps.st["layers"][i]
-        ctx.ps, ctx.i, ctx.seed = ps, i, ly["seed"]
-        ctx.save_for_backward(ly["x"], ly["qkv"], ly["lse"])
-        return ps.st["attn"][i]
-
-    @staticmethod
-    def backward(ctx, G):
-        x, qkv, lse = ctx.saved_tensors
-        ps, grads = ctx.ps, _will_execute(ctx, 1)
-        handover = ps.handover.pop(ctx.i, None)
-        with ps.module._node_backward(ps.st, grads) as sq:
-            dxn = ps.module._map_backward(ps.st, ctx.i, dict(x=x, qkv=qkv, lse=lse, seed=ctx.seed), G.to(torch.float32).contiguous(),
-                                          handover, sq, grads)
-        return None, None, dxn.view(*ps.dims()), None
-
-
-class _ContextNode(torch.autograd.Function):
-    """C_k: (hidden_states[k], attentions[k]) -> hidden_states[k + 1], the reference's dataflow past the map (ctx = A V, output
-    projection, LN1, FFN, LN2). Its backward returns d A = dO V^T for the map and nothing for hidden_states[k]: dV and the
-    residual ds1 are handed to A_k, which produces the whole gradient at hidden_states[k]."""
-
-    @staticmethod
-    def forward(ctx, ps, i, h, a, anchor):
-        ly = ps.st["layers"][i]
-        ctx.ps, ctx.i, ctx.seed = ps, i, ly["seed"]
-        ctx.save_for_backward(*(ly[k] for k in _LAYER_STASH))
-        return ps.hidden(i + 1)
-
-    @staticmethod
-    def backward(ctx, dy):
-        ly = dict(zip(_LAYER_STASH, ctx.saved_tensors), seed=ctx.seed)
-        ps, grads = ctx.ps, _will_execute(ctx, 2)
-        split = "with_map" if _will_execute(ctx, 1) else "map_only"       # A_k runs in this backward: hand dV and ds1 over
-        with ps.module._node_backward(ps.st, grads) as sq:
-            dmap, handover = ps.module._layer_backward(ps.st, ctx.i, ly, ps.dense(dy), sq, grads=grads, split=split)
-        if handover is not None:
-            ps.handover[ctx.i] = handover
-        return None, None, None, dmap, None
-
-
-class _PoolerNode(torch.autograd.Function):
-    """hidden_states[-1] (= sequence_output) -> pooled_output."""
-
-    @staticmethod
-    def forward(ctx, ps, h, anchor):
-        ctx.ps = ps
-        pooled = ps.st.pop("pooled")
-        ctx.save_for_backward(ps.st.pop("x_last"), pooled)
-        return pooled
-
-    @staticmethod
-    def backward(ctx, dpooled):
-        x_last, pooled = ctx.saved_tensors
-        ps, grads = ctx.ps, _will_execute(ctx, 1)
-        nseq, L, H = ps.dims()
-        with ps.module._node_backward(ps.st, grads):
-            dx = ps.module._pooler_backward(_pooler_pre_grad(pooled, dpooled), x_last, nseq, L, H, grads)
-        return None, dx.view(nseq, L, H), None
-
-
 # ----------------------------------------------------------------------------------------------------
 # module path: hooks on bert and the modules below it
 # ----------------------------------------------------------------------------------------------------
@@ -517,35 +374,30 @@ def _global_hooks():
                                              "_global_backward_pre_hooks"))
 
 
-def _input_needed(ctx, k):
-    """Whether tensor input k of this node (a data input, not a parameter anchor) takes a gradient in the current backward: as
-    _will_execute, but a leaf that torch.autograd.grad() was asked for does."""
-    node = ctx.next_functions[k][0]
+def _engine_runs(node, captured):
+    """Whether the autograd engine runs ``node`` (a grad_fn; None: no gradient flows there) in the current backward. torch raises
+    for a node that torch.autograd.grad() captures instead of running, and ``captured`` is the answer then: False for a parameter
+    anchor (autograd.grad() does not accumulate into .grad; neither does backward(inputs=...) without the parameter), True for a
+    data input whose gradient the call asks for."""
     if node is None:
         return False
     try:
         return bool(torch._C._will_engine_execute_node(node))
-    except RuntimeError:        # a captured input of autograd.grad()
-        return True
-
-
-def _engine_executes(node):
-    """Whether the engine runs ``node`` (a grad_fn) in the current backward."""
-    try:
-        return bool(torch._C._will_engine_execute_node(node))
     except RuntimeError:
-        return False
+        return captured
 
 
 class _BertPass:
-    """One bert(...) pass on the module path (a hook on bert or a module below it): each module the forward calls runs its part of
-    the engine here, from the tensor it was handed (the previous module's output, or what a hook replaced it with) to a view of
-    the bf16 buffer it writes. A pass that records autograd runs each part as a node whose activations are its saved tensors:
-    one node per encoder layer unless a sub-module of that layer is hooked, then the attention (or, with its self-attention or
-    output hooked, _SelfNode + _SelfOutputNode) and the FFN (or, with intermediate or output hooked, _InterNode + _OutNode)."""
+    """One bert(...) pass on the module path (a hook on bert or a module below it, or layerwise_autograd with no hook): each module
+    the forward calls runs its part of the engine here, from the tensor it was handed (the previous module's output, or what a
+    hook replaced it with) to a view of the bf16 buffer it writes. A pass that records autograd runs each part as a node whose
+    activations are its saved tensors: one node per encoder layer unless a sub-module of that layer is hooked, then the attention
+    (or, with its self-attention or output hooked, _SelfNode + _SelfOutputNode) and the FFN (or, with intermediate or output
+    hooked, _InterNode + _OutNode). split_maps (layerwise_autograd with differentiable maps): a layer with no hooked sub-module
+    is two nodes, _MapNode (A_k) and _ContextNode (C_k)."""
 
-    def __init__(self, eng, hooked, repeat=None, given=None):
-        self.eng, self.hooked = eng, hooked
+    def __init__(self, eng, hooked, repeat=None, given=None, split_maps=False):
+        self.eng, self.hooked, self.split_maps = eng, hooked, split_maps
         self.repeat = (1, None, None) if repeat is None else repeat
         self.head = repeat is not None          # a head's pass: bert(...) is called by the head and returns to it
         self.given = given                      # head: (the visual_inputs it hands to bert, the grid behind them)
@@ -637,9 +489,12 @@ class _BertPass:
         self.fwd["grid"], self.fwd["grid_src"] = visual_inputs, src
         nseq, lt, L, H = self.dims()
         self.x = torch.empty(nseq * L, H, dtype=torch.bfloat16, device=ids.device)
-        t = bert.embeddings(ids)
-        v = bert.visual_embeddings(visual_inputs)
-        x = self.give(_JoinNode.apply(self, t, v), self.fwd.pop("x_rows"))
+        if self.hooked:
+            t = bert.embeddings(ids)
+            v = bert.visual_embeddings(visual_inputs)
+            x = self.give(_JoinNode.apply(self, t, v), self.fwd.pop("x_rows"))
+        else:                                   # layerwise_autograd: both embeddings as one node, in the default path's order
+            x = self.give(_EmbeddingsNode.apply(self, src, bert.embeddings.word_embeddings.weight), self.x)
         ext = None
         enc_mods = [bert.encoder] + [m for ly in bert.encoder.layer for m in (ly, ly.attention, ly.attention.self)]
         if self.is_hooked(*enc_mods):         # the reference's extended additive mask, for the hooks that can see it
@@ -713,6 +568,10 @@ class _BertPass:
         i = self.layer_index(mod)
         att = mod.attention
         if not self.is_hooked(att, att.self, att.output, mod.intermediate, mod.output):
+            if self.split_maps:
+                probs = _MapNode.apply(self, i, h, att.self.query.weight)
+                y = _ContextNode.apply(self, i, h, probs, att.output.dense.weight)
+                return self.give(y, self.fwd.pop("y_rows")), probs
             y, probs = _LayerModNode.apply(self, i, h, att.self.query.weight)
             return self._maps((self.give(y, self.fwd.pop("y_rows")),), probs)
         ao = att(h, attention_mask, None)
@@ -812,7 +671,7 @@ class _TextNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dt):
         ps = ctx.ps
-        if dt is None or not _will_execute(ctx, 1):
+        if dt is None or not _engine_runs(ctx.next_functions[1][0], False):
             return None, None, None
         ids, = ctx.saved_tensors
         with ps.eng._node_backward(ps.st, True):
@@ -835,7 +694,7 @@ class _WordNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dvec):
         ps = ctx.ps
-        if dvec is None or not _will_execute(ctx, 1):
+        if dvec is None or not _engine_runs(ctx.next_functions[1][0], False):
             return None, None, None
         ids, = ctx.saved_tensors
         nseq, lt, _, H = ps.dims()
@@ -866,7 +725,7 @@ class _TextVectorsNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dt):
         ps = ctx.ps
-        need_vec, grads = _input_needed(ctx, 0), _will_execute(ctx, 1)
+        need_vec, grads = _engine_runs(ctx.next_functions[0][0], True), _engine_runs(ctx.next_functions[1][0], False)
         if dt is None or not (need_vec or grads):
             return None, None, None
         v, = ctx.saved_tensors
@@ -890,7 +749,7 @@ class _VisualNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dv):
         ps = ctx.ps
-        need_grid, grads = _input_needed(ctx, 0), _will_execute(ctx, 2)
+        need_grid, grads = _engine_runs(ctx.next_functions[0][0], True), _engine_runs(ctx.next_functions[2][0], False)
         if dv is None or not (need_grid or grads):
             return None, None, None, None, None
         g, = ctx.saved_tensors
@@ -899,6 +758,30 @@ class _VisualNode(torch.autograd.Function):
         if dgrid is not None:
             dgrid = dgrid.view(ctx.grid[0])
         return None, dgrid, None, None, None
+
+
+class _EmbeddingsNode(torch.autograd.Function):
+    """bert.embeddings, bert.visual_embeddings and their concat as one node, for a pass with no hook: visual_inputs -> the encoder
+    input (B', L, H). Its backward runs the text, then the visual embedding backward, as the default path does."""
+
+    @staticmethod
+    def forward(ctx, ps, grid, anchor):
+        st = ps.st
+        ps.bind()
+        ps.eng._text_fwd(st, st["ids"], ps.x)
+        ps.eng._visual_fwd(st, st["grid"], ps.repeat, ps.x)
+        ctx.ps, ctx.shape = ps, grid.shape
+        return ps.view(ps.x)
+
+    @staticmethod
+    def backward(ctx, dx):
+        ps = ctx.ps
+        need_grid, grads = _engine_runs(ctx.next_functions[0][0], True), _engine_runs(ctx.next_functions[1][0], False)
+        if not (need_grid or grads):
+            return None, None, None
+        with ps.eng._node_backward(ps.st, grads):
+            dgrid = ps.eng._embedding_backward(ps.st, ps.dense(dx), need_grid, grads)
+        return None, (None if dgrid is None else dgrid.view(ctx.shape)), None
 
 
 class _JoinNode(torch.autograd.Function):
@@ -966,20 +849,17 @@ class _LayerModNode(torch.autograd.Function):
         eng, st = ps.eng, ps.st
         ps.bind()
         x = ps.rows(h, "the input of encoder.layer[%d]" % i)
-        qkv, c, lse, probs = eng._self_fwd(st, i, x, ps.need_backward, ps.want_attn)
-        s1, st1, a = eng._attn_out_fwd(st, i, c, x)
-        gel, u = eng._inter_fwd(st, i, a, ps.need_backward)
-        s2, st2, y = eng._out_fwd(st, i, gel, a)
+        ly, y, probs = eng._layer_fwd(st, i, x, ps.need_backward, ps.want_attn)
         ctx.ps, ctx.i = ps, i
         ctx.set_materialize_grads(False)
-        ctx.save_for_backward(x, qkv, c, lse, s1, st1, a, u, gel, s2, st2)
+        ctx.save_for_backward(*(ly[k] for k in _LAYER_STASH))
         ps.fwd["y_rows"] = y
         return ps.view(y), _map_outputs(ctx, ps, probs)
 
     @staticmethod
     def backward(ctx, dy, dprobs):
         ps, i = ctx.ps, ctx.i
-        grads, need_dx = _will_execute(ctx, 1), _input_needed(ctx, 0)
+        grads, need_dx = _engine_runs(ctx.next_functions[1][0], False), _engine_runs(ctx.next_functions[0][0], True)
         dattn = _dmap(ps, dprobs)
         if not (grads or need_dx) or (dy is None and dattn is None):
             return None, None, None, None
@@ -988,6 +868,67 @@ class _LayerModNode(torch.autograd.Function):
         with ps.eng._node_backward(ps.st, grads) as sq:
             dxn = ps.eng._layer_backward(ps.st, i, ly, dy, sq, dattn=dattn, grads=grads)
         return None, None, ps.view(dxn), None
+
+
+class _MapNode(torch.autograd.Function):
+    """A_k, encoder.layer[k] split at its differentiable map (layerwise_autograd): hidden_states[k] -> attentions[k]. Its forward
+    runs the whole layer and leaves the stash to C_k. Its backward receives the map's full gradient G (the direct term, C_k's
+    dO V^T and whatever hooks made of them) and finishes layer k: dQ / dK from G, the QKV weight gradient, the dgrad to
+    hidden_states[k]."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, anchor):
+        ps.bind()
+        x = ps.rows(h, "the input of encoder.layer[%d]" % i)
+        ly, y, probs = ps.eng._layer_fwd(ps.st, i, x, ps.need_backward, True)
+        ctx.ps, ctx.i = ps, i
+        ctx.save_for_backward(x, ly["qkv"], ly["lse"])
+        ps.fwd["layer"], ps.fwd["y_rows"] = ly, y
+        return probs
+
+    @staticmethod
+    def backward(ctx, G):
+        ps, i = ctx.ps, ctx.i
+        grads = _engine_runs(ctx.next_functions[1][0], False)
+        ly = _ly(("x", "qkv", "lse"), ctx.saved_tensors, _layer_seed(ps, i))
+        handover = ps.handover.pop(i, None)
+        with ps.eng._node_backward(ps.st, grads) as sq:
+            dxn = ps.eng._map_backward(ps.st, i, ly, G.to(torch.float32).contiguous(), handover, sq, grads)
+        return None, None, ps.view(dxn), None
+
+
+class _ContextNode(torch.autograd.Function):
+    """C_k: (hidden_states[k], attentions[k]) -> hidden_states[k + 1], the reference's dataflow past the map (ctx = A V, output
+    projection, LN1, FFN, LN2). Its backward returns d A = dO V^T for the map and nothing for hidden_states[k]: dV and the
+    residual ds1 are handed to A_k, which produces the whole gradient at hidden_states[k]."""
+
+    @staticmethod
+    def forward(ctx, ps, i, h, a, anchor):
+        ly = ps.fwd.pop("layer")
+        ctx.ps, ctx.i = ps, i
+        ctx.save_for_backward(*(ly[k] for k in _LAYER_STASH))
+        return ps.view(ps.fwd["y_rows"])
+
+    @staticmethod
+    def backward(ctx, dy):
+        ps, i = ctx.ps, ctx.i
+        eng, st = ps.eng, ps.st
+        nseq, lt, L, H = ps.dims()
+        ly = _ly(_LAYER_STASH, ctx.saved_tensors, _layer_seed(ps, i))
+        grads = _engine_runs(ctx.next_functions[2][0], False)
+        with eng._node_backward(st, grads) as sq:
+            wg = eng._wgrad_list()
+            du, ds2 = eng._output_backward(st, i, ly, ps.dense(dy), sq, grads, fused=True, wg=wg)
+            da = eng._intermediate_backward(st, i, ly, du, sq, grads, ds2, wg=wg)
+            dctx, ds1 = eng._self_output_backward(st, i, ly, da, sq, grads, wg=wg)
+            eng._issue_wgrads(sq, wg)                       # the QKV weight gradient is A_k's
+            dmap = torch.empty(nseq, st["heads"], L, L, dtype=torch.float32, device=dy.device)
+            ops.attention_dprobs(ly["qkv"], dctx, dmap, False, nseq, L, st["heads"])
+            if _engine_runs(ctx.next_functions[1][0], False):      # A_k runs in this backward: hand dV and ds1 over
+                dqkv = torch.empty(nseq * L, 3 * H, dtype=torch.bfloat16, device=dy.device)
+                ops.attention_bwd_dv(ly["qkv"], st["mask"], ly["lse"], dctx, dqkv, nseq, L, lt, st["heads"], st["p_a"], ly["seed"] + 1)
+                ps.handover[i] = (dqkv, ds1)
+        return None, None, None, dmap, None
 
 
 class _AttentionNode(torch.autograd.Function):
@@ -1009,7 +950,7 @@ class _AttentionNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, da, dprobs):
         ps, i = ctx.ps, ctx.i
-        grads, need_dx = _will_execute(ctx, 1), _input_needed(ctx, 0)
+        grads, need_dx = _engine_runs(ctx.next_functions[1][0], False), _engine_runs(ctx.next_functions[0][0], True)
         dattn = _dmap(ps, dprobs)
         if not (grads or need_dx) or (da is None and dattn is None):
             return None, None, None, None
@@ -1040,7 +981,7 @@ class _FfnNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         ps, i = ctx.ps, ctx.i
-        grads, need_dx = _will_execute(ctx, 1), _input_needed(ctx, 0)
+        grads, need_dx = _engine_runs(ctx.next_functions[1][0], False), _engine_runs(ctx.next_functions[0][0], True)
         if not (grads or need_dx):
             return None, None, None, None
         ly = _ly(("a", "u", "gel", "s2", "st2"), ctx.saved_tensors, _layer_seed(ps, i))
@@ -1071,7 +1012,7 @@ class _SelfNode(torch.autograd.Function):
     def backward(ctx, dctx, dprobs):
         ps, i = ctx.ps, ctx.i
         residual = ps.handover.pop(("ds1", i), None)
-        grads = _will_execute(ctx, 1)
+        grads = _engine_runs(ctx.next_functions[1][0], False)
         dattn = _dmap(ps, dprobs)
         ly = _ly(("x", "qkv", "ctx", "lse"), ctx.saved_tensors, _layer_seed(ps, i))
         if dctx is None and dattn is None:
@@ -1101,11 +1042,11 @@ class _SelfOutputNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, da):
         ps, i = ctx.ps, ctx.i
-        grads = _will_execute(ctx, 2)
+        grads = _engine_runs(ctx.next_functions[2][0], False)
         ly = _ly(("ctx", "s1", "st1"), ctx.saved_tensors, _layer_seed(ps, i))
         with ps.eng._node_backward(ps.st, grads) as sq:
             dctx, ds1 = ps.eng._self_output_backward(ps.st, i, ly, ps.dense(da), sq, grads)
-        if ctx.partner is not None and _engine_executes(ctx.partner):
+        if _engine_runs(ctx.partner, False):
             ps.handover[("ds1", i)] = ds1
             return None, None, ps.view(dctx), None, None, None
         return None, None, ps.view(dctx), ps.view(ds1), None, None
@@ -1133,7 +1074,7 @@ class _InterNode(torch.autograd.Function):
         residual = ps.handover.pop(("ds2", i), None)
         if dgel is None:
             return None, None, (None if residual is None else ps.view(residual)), None
-        grads = _will_execute(ctx, 1)
+        grads = _engine_runs(ctx.next_functions[1][0], False)
         ar, u = ctx.saved_tensors
         du = (dgel.reshape(u.shape).float() * u.float()).to(torch.bfloat16)
         with ps.eng._node_backward(ps.st, grads) as sq:
@@ -1164,13 +1105,13 @@ class _OutNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         ps, i = ctx.ps, ctx.i
-        grads = _will_execute(ctx, 2)
+        grads = _engine_runs(ctx.next_functions[2][0], False)
         ly = _ly(("gel", "s2", "st2"), ctx.saved_tensors, _layer_seed(ps, i))
         with ps.eng._node_backward(ps.st, grads) as sq:
             dgel, ds2 = ps.eng._output_backward(ps.st, i, ly, ps.dense(dy), sq, grads, fused=False)
         nseq, _, L, H = ps.dims()
         dgel = dgel.view(nseq, L, -1)
-        if ctx.partner is not None and _engine_executes(ctx.partner):
+        if _engine_runs(ctx.partner, False):
             ps.handover[("ds2", i)] = ds2
             return None, None, dgel, None, None, None
         return None, None, dgel, ps.view(ds2), None, None
@@ -1193,7 +1134,7 @@ class _PoolerModNode(torch.autograd.Function):
     def backward(ctx, dpooled):
         ps = ctx.ps
         x, pooled = ctx.saved_tensors
-        grads = _will_execute(ctx, 1)
+        grads = _engine_runs(ctx.next_functions[1][0], False)
         nseq, _, L, H = ps.dims()
         with ps.eng._node_backward(ps.st, grads):
             dx = ps.eng._pooler_backward(_pooler_pre_grad(pooled, dpooled), x, nseq, L, H, grads)
@@ -1212,7 +1153,7 @@ class _HeadNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *douts):
         ps = ctx.ps
-        grads = _will_execute(ctx, 2)
+        grads = _engine_runs(ctx.next_functions[2][0], False)
         nseq, _, L, H = ps.dims()
         st = ctx.st
         with ps.eng._node_backward(st, grads):
@@ -1232,7 +1173,7 @@ class _HeadPoolerNode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *douts):
         ps = ctx.ps
-        grads = _will_execute(ctx, 2)
+        grads = _engine_runs(ctx.next_functions[2][0], False)
         nseq, _, L, H = ps.dims()
         st = ctx.st
         with ps.eng._node_backward(st, grads):
@@ -1455,8 +1396,9 @@ class _ClipBertHeadModel(nn.Module):
             return _TransformerFn.apply(self, grid, anchor, ids, mask, repeat)
         return self._forward_impl(ids, grid, mask, repeat, need_backward=False)[0]
 
-    def _run_base(self, text_input_ids, visual_inputs, attention_mask, want_hidden, want_attn, diff_attn=False, layerwise=False):
-        """ClipBertBaseModel.forward on this engine (the head itself is not run). visual_inputs: (B', T, h, w, 768)."""
+    def _run_base(self, text_input_ids, visual_inputs, attention_mask, want_hidden, want_attn, diff_attn, records):
+        """ClipBertBaseModel.forward on this engine's default path (the head itself is not run), one autograd node when the pass
+        records autograd (_base_pass). visual_inputs: (B', T, h, w, 768)."""
         _require_cuda(text_input_ids)
         self._ensure_ready(text_input_ids.device)
         assert visual_inputs.shape[0] == text_input_ids.shape[0], "visual_inputs must have one row per text example"
@@ -1465,14 +1407,7 @@ class _ClipBertHeadModel(nn.Module):
         ids = text_input_ids.contiguous()
         mask = attention_mask.to(torch.int64).contiguous()
         flags = (bool(want_hidden), bool(want_attn), bool(want_attn and diff_attn))
-        records = torch.is_grad_enabled() and (grid.requires_grad or any(p.requires_grad for p in self.bert.parameters()))
-        if records and self.bert.recompute_activations and (diff_attn or layerwise):
-            raise RuntimeError("ClipBertBaseModel: recompute_activations cannot be combined with %s: its backward reads every "
-                               "layer's activations; turn one of the switches off" %
-                               ("differentiable_attentions" if diff_attn else "layerwise_autograd"))
-        if records and layerwise:
-            seq, pooled, hidden, attn = self._run_layerwise(ids, grid, mask, flags)
-        elif records:
+        if records:
             outs = _BaseModelFn.apply(self, grid, self.bert.pooler.dense.weight, ids, mask, flags)
             n_hidden = len(self.bert.encoder.layer) + 1 if flags[0] else 0
             seq, pooled, hidden, attn = outs[0], outs[1], outs[2:2 + n_hidden], outs[2 + n_hidden:]
@@ -1485,33 +1420,27 @@ class _ClipBertHeadModel(nn.Module):
             out = out + (tuple(attn),)
         return out
 
-    def _run_layerwise(self, ids, grid, mask, flags):
-        """ClipBertBaseModel.forward with layerwise_autograd: the pass runs as _forward_impl runs it (same launches, same bits),
-        then its outputs are handed out through a chain of autograd nodes - the embeddings, one node per encoder layer (two, A_k
-        and C_k, when the maps are differentiable) and the pooler - so that tensor hooks, torch.autograd.grad and
-        backward(inputs=...) on any hidden state or map follow torch's own semantics. Returns (sequence_output, pooled_output,
-        hidden_states, attentions) as _forward_impl does."""
+    def _base_pass(self, visual_inputs):
+        """Which path a bert(...) call takes: (the module-path pass to run it in, or None for the default path; whether the pass
+        records autograd). The module path serves a hook on bert or a module below it, and layerwise_autograd on a pass that
+        records autograd (the maps split when differentiable_attentions is on). Raises for the combinations that are refused."""
+        hooked = self._bert_hooked()
+        if hooked:
+            return _BertPass(self, hooked), None
+        bert = self.bert
+        records = torch.is_grad_enabled() and (visual_inputs.requires_grad or any(p.requires_grad for p in bert.parameters()))
+        if not records:
+            return None, False
+        if bert.recompute_activations and (bert.differentiable_attentions or bert.layerwise_autograd):
+            raise RuntimeError("ClipBertBaseModel: recompute_activations cannot be combined with %s: its backward reads every "
+                               "layer's activations; turn one of the switches off" %
+                               ("differentiable_attentions" if bert.differentiable_attentions else "layerwise_autograd"))
+        if not bert.layerwise_autograd:
+            return None, True
         if self._grad_ready_hook is not None:
             raise RuntimeError("ClipBertBaseModel.layerwise_autograd is for analysis, not data-parallel training: it cannot run while "
                                "the overlapped gradient exchange (enable_overlapped_allreduce) is enabled")
-        with torch.no_grad():
-            (_, _, _, attn), st = self._forward_impl(ids, grid, mask, (1, None, None), need_backward=True, base=flags)
-        st["attn"] = attn
-        ps = _LayerwisePass(self, st)
-        bert = self.bert
-        h = _EmbeddingNode.apply(ps, grid, bert.embeddings.word_embeddings.weight)
-        hidden, maps = [h], []
-        for i, layer in enumerate(bert.encoder.layer):
-            if flags[2]:
-                a = _MapNode.apply(ps, i, h, layer.attention.self.query.weight)
-                h = _ContextNode.apply(ps, i, h, a, layer.attention.output.dense.weight)
-                maps.append(a)
-            else:
-                h = _LayerNode.apply(ps, i, h, layer.attention.self.query.weight)
-            hidden.append(h)
-        pooled = _PoolerNode.apply(ps, h, bert.pooler.dense.weight)
-        st["layers"] = st["attn"] = None    # each layer's activations are saved tensors of its node(s) now, released with them
-        return h, pooled, (hidden if flags[0] else []), (maps if flags[2] else attn)
+        return _BertPass(self, set(), split_maps=bert.output_attentions and bert.differentiable_attentions), True
 
     # ---- module path: hooks on bert and the modules below it ---------------------------------------------------------------
     def _bert_sites(self):
@@ -1586,7 +1515,7 @@ class _ClipBertHeadModel(nn.Module):
 
     @contextlib.contextmanager
     def _node_backward(self, st, grads):
-        """Around the backward of one layerwise node: the pass's dropout word bound (its masks regenerated) and unbound on the way
+        """Around the backward of one module-path node: the pass's dropout word bound (its masks regenerated) and unbound on the way
         out, the node's side-queue weight gradients joined before it returns (a partial backward may run no later node), and,
         when it writes parameter gradients, the flat buffer attached and the bf16 operands due a repack."""
         ops.dropout_offset_bind(st["drop_word"])
@@ -1643,19 +1572,16 @@ class _ClipBertHeadModel(nn.Module):
                 x = self._inject[i].to(device=ids.device, dtype=torch.bfloat16).reshape(M, H).contiguous()
             if want_hidden:
                 hidden.append(x.view(nseq, L, H))
-            qkv, ctx, lse, probs = self._self_fwd(st, i, x, need_backward, want_attn)
+            ly, y, probs = self._layer_fwd(st, i, x, need_backward, want_attn)
             if want_attn:
                 attn.append(probs)
-            s1, st1, a = self._attn_out_fwd(st, i, ctx, x)
-            gel, u = self._inter_fwd(st, i, a, need_backward)
-            s2, st2, y = self._out_fwd(st, i, gel, a)
             ls = seed + 16 * (i + 1)
             if need_backward and recompute:
                 st["layers"].append(dict(x=x, seed=ls, recompute=True))    # the rest is re-run before the layer's backward
             elif need_backward:
-                st["layers"].append(dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2, seed=ls))
+                st["layers"].append(dict(ly, seed=ls))
             if cap is not None:
-                cap["l%d" % i] = dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, gel=gel, u=u, s2=s2, st2=st2)
+                cap["l%d" % i] = ly
             x = y
             if cap is not None:
                 cap["layer%d" % i] = x.view(nseq, L, H)
@@ -1780,6 +1706,15 @@ class _ClipBertHeadModel(nn.Module):
         ops.layernorm_fwd(s2, g2, b2, y, st2, st["eps"])
         return s2, st2, y
 
+    def _layer_fwd(self, st, i, x, need_backward, want_attn):
+        """BertLayer i from its input rows x: (its stash {x, qkv, ctx, lse, s1, st1, a, u, gel, s2, st2}, the output rows, the
+        post-dropout probabilities or None)."""
+        qkv, ctx, lse, probs = self._self_fwd(st, i, x, need_backward, want_attn)
+        s1, st1, a = self._attn_out_fwd(st, i, ctx, x)
+        gel, u = self._inter_fwd(st, i, a, need_backward)
+        s2, st2, y = self._out_fwd(st, i, gel, a)
+        return dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2), y, probs
+
     def _pooler_fwd(self, st, x):
         """BertPooler on the [CLS] rows of x (row pitch L * H, no gather)."""
         nseq, L = st["dims"][0], st["dims"][6]
@@ -1817,9 +1752,9 @@ class _ClipBertHeadModel(nn.Module):
         ops.gemm(**self._wgrad_kw(li, dy, x, rows, x_ld))
 
     def _split_wgrad_kw(self, key, li, dy, x, rows):
-        """A weight gradient of a layer whose backward is split into nodes (the module path): one launch, pinned to the tile width
-        and K-split of the grouped launch _layer_backward issues for it (ops.group_wgrad: the layer's four, or its FFN and
-        attention pairs), so that each element is summed in the same order and observe-only hooks keep the bits."""
+        """A weight gradient of an encoder layer launched on its own: one launch, pinned to the tile width and K-split of the
+        grouped launch _layer_backward issues for it (ops.group_wgrad: the layer's four, or its FFN and attention pairs), so that
+        each element is summed in the same order and observe-only hooks keep the bits."""
         kw = self._wgrad_kw(li, dy, x, rows)
         gmode = ops.group_wgrad
         if gmode not in (1, 3, 4) or not dy.is_cuda:
@@ -1838,6 +1773,37 @@ class _ClipBertHeadModel(nn.Module):
             return kw
         bn, split = pins[key]
         return dict(kw, block_n=bn, split_k=split)
+
+    def _wgrad_list(self):
+        """How a whole layer's backward (_layer_backward, _ContextNode) launches its weight gradients: [] to gather them into grouped
+        launches (ops.group_wgrad 1 and 3: the layer's four in one; 4: the FFN pair, then the attention pair), None for singles."""
+        return [] if ops.group_wgrad in (1, 3, 4) else None
+
+    def _layer_wgrad(self, sq, wg, i, key, dy, x, bias=False):
+        """The weight gradient of layer i's linear key (out, inter, ao or qkv) from dy and its input x, on the side queue sq, with
+        the bias column sum of dy when bias. wg None: launched now, pinned (_split_wgrad_kw). wg a list (_wgrad_list): the
+        descriptor joins it and the bias sum runs now; the list goes out as one grouped launch at the layer's last weight
+        gradient (QKV) and, in ops.group_wgrad 4, at the FFN's last (inter)."""
+        li = self._lin["l%d.%s" % (i, key)]
+        M = dy.shape[0]
+        colsum = (lambda: ops.colsum(dy, li.gb, M, li.n)) if bias else None
+        if wg is None:
+            kw = self._split_wgrad_kw(key, li, dy, x, M)
+            sq.run(lambda: (ops.gemm(**kw), colsum and colsum()), dy, x)
+            return
+        wg.append((self._wgrad_kw(li, dy, x, M), (dy, x)))
+        if key == "qkv" or (key == "inter" and ops.group_wgrad == 4):
+            self._issue_wgrads(sq, wg, colsum)
+        elif colsum is not None:
+            sq.run(colsum, dy)
+
+    def _issue_wgrads(self, sq, wg, then=None):
+        """The weight gradients gathered in wg (None: none) as one grouped launch on the side queue (a plain launch for one),
+        followed by then(); wg is emptied."""
+        if wg:
+            kws = [kw for kw, _ in wg]
+            sq.run(lambda: (ops.gemm_wgrad_group(kws), then and then()), *(t for _, keep in wg for t in keep))
+            wg.clear()
 
     def _dgrad(self, li, dy, rows, out, **kw):
         ops.gemm(mode=ops.CB_GEMM_NN, m=rows, n=li.k, k=li.n, a=dy, a_rows=rows, a_ld=li.n, b=li.w, b_rows=li.n, b_ld=li.k,
@@ -1932,12 +1898,8 @@ class _ClipBertHeadModel(nn.Module):
     def _recompute_layer(self, st, i, ly):
         """Encoder layer i's stash as the forward kept it, from its kept input ly["x"]: the forward's launches, seeds and (bound by
         the caller) dropout word, so every tensor is the forward's bit for bit. The layer output is not needed."""
-        x = ly["x"]
-        qkv, ctx, lse, _ = self._self_fwd(st, i, x, True, False)
-        s1, st1, a = self._attn_out_fwd(st, i, ctx, x)
-        gel, u = self._inter_fwd(st, i, a, True)
-        s2, st2, _ = self._out_fwd(st, i, gel, a)
-        return dict(x=x, qkv=qkv, ctx=ctx, lse=lse, s1=s1, st1=st1, a=a, u=u, gel=gel, s2=s2, st2=st2, seed=ly["seed"])
+        stash, _, _ = self._layer_fwd(st, i, ly["x"], True, False)
+        return dict(stash, seed=ly["seed"])
 
     def _pooler_backward(self, dpre, x_last, nseq, L, H, grads=True):
         """d pooler pre-activation (None: no gradient) -> the gradient at the top of the encoder, [nseq * L, H] bf16 with the [CLS]
@@ -1951,130 +1913,41 @@ class _ClipBertHeadModel(nn.Module):
             self._dgrad(pl, dpre, nseq, dx, out_ld=L * H)  # scatters into the [CLS] rows
         return dx
 
-    def _layer_backward(self, st, i, ly, dx, sq, cap=None, dattn=None, ret_attn=None, grads=True, split=None):
+    def _layer_backward(self, st, i, ly, dx, sq, cap=None, dattn=None, ret_attn=None, grads=True):
         """Encoder layer i from the gradient at its output dx ([nseq * L, H] bf16, not written) to the gradient at its input, with
-        the layer's stash ly; weight gradients on the side queue sq. dattn: a loss term on the layer's returned attention map,
-        ret_attn: the map when retained. grads = False: no parameter gradient is written (a backward that does not accumulate
-        into the parameters). split (the backward split at a differentiable map, ClipBertBaseModel.layerwise_autograd): stop at
-        the attention and return (d map = dO V^T, hand-over) - the hand-over (dqkv with its V block written, ds1) when split is
-        "with_map" (the map's node runs next and finishes the layer in _map_backward), None when it is "map_only"."""
-        dev = dx.device
-        H = _cfg(self.config, "hidden_size")
-        heads = _cfg(self.config, "num_attention_heads")
-        nseq, nvid, T, gh, gw, lt, L = st["dims"]
-        M = nseq * L
-        p_h, p_a = st["p_h"], st["p_a"]
-        bf16, f32 = torch.bfloat16, torch.float32
-
-        def new(*shape, dtype=bf16):
-            return torch.empty(*shape, dtype=dtype, device=dev)
-
-        ls = ly["seed"]
-        qkv_l, ao_l, in_l, out_l = (self._lin["l%d.%s" % (i, k)] for k in ("qkv", "ao", "inter", "out"))
-        g1, _, dg1, db1 = self._ln("l%d.ln1" % i)
-        g2, _, dg2, db2 = self._ln("l%d.ln2" % i)
-        dbo, dbao = out_l.gb, ao_l.gb
-        if not grads:
-            dg1 = db1 = dg2 = db2 = dbo = dbao = None
-        # y = LN2(s2), s2 = dropout(gel @ Wo^T + bo) + a
-        ds2 = new(M, H)
-        ds2d = new(M, H) if p_h > 0 else None
-        ops.layernorm_bwd(dx, ly["s2"], ly["st2"], g2, ds2, ds2d, dg2, db2, dbo, p_h, ls + 3)
-        dd = ds2d if ds2d is not None else ds2
-        gmode = ops.group_wgrad      # the layer's four weight gradients as ONE launch (issued when the last dY, dqkv, exists) or two pairs
-        group = gmode in (1, 3, 4)
-        pairs = gmode == 4
-        wg = [self._wgrad_kw(out_l, dd, ly["gel"], M)]
-        if grads and not group:
-            sq.run(lambda: ops.gemm(**wg[0]), dd, ly["gel"])
-        du = new(M, in_l.n)
-        self._dgrad(out_l, dd, M, du, aux=ly["u"], aux_ld=in_l.n, aux_mode=ops.AUX_MUL)
-        wg.append(self._wgrad_kw(in_l, du, ly["a"], M))
-        if not grads:
-            pass
-        elif pairs:
-            wg_ffn, wg = wg, []
-            sq.run(lambda: (ops.gemm_wgrad_group(wg_ffn), ops.colsum(du, in_l.gb, M, in_l.n)), dd, ly["gel"], du, ly["a"])
-        elif group:
-            sq.run(lambda: ops.colsum(du, in_l.gb, M, in_l.n), du)
-        else:
-            sq.run(lambda: (ops.gemm(**wg[1]), ops.colsum(du, in_l.gb, M, in_l.n)), du, ly["a"])
-        da = new(M, H)
-        self._dgrad(in_l, du, M, da, residual=ds2, res_ld=H)
-        # a = LN1(s1), s1 = dropout(ctx @ Wao^T + b) + x
-        ds1 = new(M, H)
-        ds1d = new(M, H) if p_h > 0 else None
-        ops.layernorm_bwd(da, ly["s1"], ly["st1"], g1, ds1, ds1d, dg1, db1, dbao, p_h, ls + 2)
-        dd1 = ds1d if ds1d is not None else ds1
-        wg.append(self._wgrad_kw(ao_l, dd1, ly["ctx"], M))
-        if grads and not group:
-            sq.run(lambda: ops.gemm(**wg[2]), dd1, ly["ctx"])
-        dctx = new(M, H)
-        self._dgrad(ao_l, dd1, M, dctx)
-        if split is not None:
-            if grads and group and wg:           # the weight gradients still pending here; the map's node issues the QKV one
-                sq.run(lambda: ops.gemm_wgrad_group(wg), dd, ly["gel"], du, ly["a"], dd1, ly["ctx"])
-            dmap = new(nseq, heads, L, L, dtype=f32)
-            ops.attention_dprobs(ly["qkv"], dctx, dmap, False, nseq, L, heads)
-            if split != "with_map":
-                return dmap, None
-            dqkv = new(M, 3 * H)
-            ops.attention_bwd_dv(ly["qkv"], st["mask"], ly["lse"], dctx, dqkv, nseq, L, lt, heads, p_a, ls + 1)
-            return dmap, (dqkv, ds1)
-        dqkv = new(M, 3 * H)
-        ops.attention_bwd(ly["qkv"], st["mask"], ly["ctx"], dctx, ly["lse"], dqkv, nseq, L, lt, heads, p_a, ls + 1)
-        if dattn is not None:      # a loss on attentions[i]: its dQ / dK added into dqkv
-            drow = new(nseq, heads, L, dtype=f32)
-            if cap is not None:
-                cap.setdefault("l%d" % i, {})["dqkv_attn"] = dqkv.clone()
-            ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn, drow, dqkv, nseq, L, lt, heads, p_a, ls + 1)
-        if ret_attn is not None:
-            _add_retained_attention_grad(ret_attn, ly["qkv"], dctx, nseq, L, heads)
-        wg.append(self._wgrad_kw(qkv_l, dqkv, ly["x"], M))
-        if not grads:
-            pass
-        elif group:
-            sq.run(lambda: (ops.gemm_wgrad_group(wg), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dd, ly["gel"], du, ly["a"], dd1, ly["ctx"], dqkv, ly["x"])
-        else:
-            sq.run(lambda: (ops.gemm(**wg[3]), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
-        dxn = new(M, H)
-        self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
-        if cap is not None:
-            c = cap.setdefault("l%d" % i, {})
-            c.update(dx=dx, ds2=ds2, ds2d=ds2d, du=du, da=da, ds1=ds1, ds1d=ds1d, dctx=dctx, dqkv=dqkv)
+        the layer's stash ly: the four per-module pieces in order, their weight gradients on the side queue sq as _wgrad_list
+        says. dattn: a loss term on the layer's returned attention map, ret_attn: the map when retained. grads = False: no
+        parameter gradient is written (a backward that does not accumulate into the parameters)."""
+        c = None if cap is None else cap.setdefault("l%d" % i, {})
+        wg = self._wgrad_list()
+        du, ds2 = self._output_backward(st, i, ly, dx, sq, grads, fused=True, wg=wg, cap=c)
+        da = self._intermediate_backward(st, i, ly, du, sq, grads, ds2, wg=wg)
+        dctx, ds1 = self._self_output_backward(st, i, ly, da, sq, grads, wg=wg, cap=c)
+        dxn = self._self_attention_backward(st, i, ly, dctx, dattn, sq, grads, ds1, wg=wg, cap=c, ret_attn=ret_attn)
+        if c is not None:
+            c.update(dx=dx, ds2=ds2, du=du, da=da, ds1=ds1, dctx=dctx)
             c.setdefault("dxn", dxn)
         return dxn
 
     def _map_backward(self, st, i, ly, G, handover, sq, grads=True):
         """The rest of encoder layer i's backward from G, the full gradient of its attention map (fp32 [nseq, heads, L, L]), when
-        the backward is split at the map: dQ / dK written from G (cb_attention_probs_bwd_store), then the QKV weight gradient and
-        the dgrad to the layer input with the residual ds1. handover = (dqkv with its V block, ds1) from _layer_backward, or None
-        when the layer's output got no gradient (dV = 0, no residual)."""
-        H = _cfg(self.config, "hidden_size")
-        heads = _cfg(self.config, "num_attention_heads")
-        nseq, nvid, T, gh, gw, lt, L = st["dims"]
-        M = nseq * L
-        dev = G.device
-        qkv_l = self._lin["l%d.qkv" % i]
+        the backward is split at the map (_MapNode): dQ / dK written from G (cb_attention_probs_bwd_store), then the QKV tail.
+        handover = (dqkv with its V block, ds1) from _ContextNode, or None when the layer's output got no gradient (dV = 0, no
+        residual)."""
+        nseq, _, _, _, _, lt, L = st["dims"]
+        H, heads = st["H"], st["heads"]
         if handover is None:
-            dqkv, ds1 = torch.empty(M, 3 * H, dtype=torch.bfloat16, device=dev), None
+            dqkv, ds1 = torch.empty(nseq * L, 3 * H, dtype=torch.bfloat16, device=G.device), None
             dqkv[:, 2 * H:].zero_()
         else:
             dqkv, ds1 = handover
-        drow = torch.empty(nseq, heads, L, dtype=torch.float32, device=dev)
+        drow = torch.empty(nseq, heads, L, dtype=torch.float32, device=G.device)
         ops.attention_probs_bwd_store(ly["qkv"], st["mask"], ly["lse"], G, drow, dqkv, nseq, L, lt, heads, st["p_a"], ly["seed"] + 1)
-        if grads:
-            kw = self._wgrad_kw(qkv_l, dqkv, ly["x"], M)
-            sq.run(lambda: (ops.gemm(**kw), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
-        dxn = torch.empty(M, H, dtype=torch.bfloat16, device=dev)
-        if ds1 is None:
-            self._dgrad(qkv_l, dqkv, M, dxn)
-        else:
-            self._dgrad(qkv_l, dqkv, M, dxn, residual=ds1, res_ld=H)
-        return dxn
+        return self._qkv_backward(st, i, ly, dqkv, sq, grads, ds1, wg=[])
 
-    # ---- the backward's per-module pieces (the module path's split layers; the default path runs _layer_backward) --------
-    def _output_backward(self, st, i, ly, dy, sq, grads, fused):
+    # ---- the backward's per-module pieces: _layer_backward calls them in this order, the module path's split layers one by one -
+    # wg: the layer's weight gradients, as _layer_wgrad takes them; cap: the layer's dict of captured gradients, or None
+    def _output_backward(self, st, i, ly, dy, sq, grads, fused, wg=None, cap=None):
         """layer[i].output from the gradient dy at its output: (d intermediate_output, times gelu' when fused; ds2, the gradient
         of its residual input attention_output)."""
         M, H = dy.shape
@@ -2089,23 +1962,23 @@ class _ClipBertHeadModel(nn.Module):
         ops.layernorm_bwd(dy, ly["s2"], ly["st2"], g2, ds2, ds2d, dg2, db2, dbo, p_h, ls + 3)
         dd = ds2d if ds2d is not None else ds2
         if grads:
-            kw = self._split_wgrad_kw("out", out_l, dd, ly["gel"], M)
-            sq.run(lambda: ops.gemm(**kw), dd, ly["gel"])
+            self._layer_wgrad(sq, wg, i, "out", dd, ly["gel"])
         dgel = torch.empty(M, in_l.n, dtype=torch.bfloat16, device=dy.device)
         if fused:
             self._dgrad(out_l, dd, M, dgel, aux=ly["u"], aux_ld=in_l.n, aux_mode=ops.AUX_MUL)
         else:
             self._dgrad(out_l, dd, M, dgel)
+        if cap is not None:
+            cap["ds2d"] = ds2d
         return dgel, ds2
 
-    def _intermediate_backward(self, st, i, ly, du, sq, grads, residual):
+    def _intermediate_backward(self, st, i, ly, du, sq, grads, residual, wg=None):
         """layer[i].intermediate from du, the gradient at its pre-activation: d attention_output, plus residual (ds2) in the
         dgrad epilogue when given."""
         M, H = du.shape[0], st["H"]
         in_l = self._lin["l%d.inter" % i]
         if grads:
-            kw = self._split_wgrad_kw("inter", in_l, du, ly["a"], M)
-            sq.run(lambda: (ops.gemm(**kw), ops.colsum(du, in_l.gb, M, in_l.n)), du, ly["a"])
+            self._layer_wgrad(sq, wg, i, "inter", du, ly["a"], bias=True)
         da = torch.empty(M, H, dtype=torch.bfloat16, device=du.device)
         if residual is None:
             self._dgrad(in_l, du, M, da)
@@ -2113,7 +1986,7 @@ class _ClipBertHeadModel(nn.Module):
             self._dgrad(in_l, du, M, da, residual=residual, res_ld=H)
         return da
 
-    def _self_output_backward(self, st, i, ly, da, sq, grads):
+    def _self_output_backward(self, st, i, ly, da, sq, grads, wg=None, cap=None):
         """layer[i].attention.output from the gradient da at its output: (d context, ds1 = the gradient of its residual input)."""
         M, H = da.shape
         p_h, ls = st["p_h"], ly["seed"]
@@ -2127,29 +2000,41 @@ class _ClipBertHeadModel(nn.Module):
         ops.layernorm_bwd(da, ly["s1"], ly["st1"], g1, ds1, ds1d, dg1, db1, dbao, p_h, ls + 2)
         dd1 = ds1d if ds1d is not None else ds1
         if grads:
-            kw = self._split_wgrad_kw("ao", ao_l, dd1, ly["ctx"], M)
-            sq.run(lambda: ops.gemm(**kw), dd1, ly["ctx"])
+            self._layer_wgrad(sq, wg, i, "ao", dd1, ly["ctx"])
         dctx = torch.empty(M, H, dtype=torch.bfloat16, device=da.device)
         self._dgrad(ao_l, dd1, M, dctx)
+        if cap is not None:
+            cap["ds1d"] = ds1d
         return dctx, ds1
 
-    def _self_attention_backward(self, st, i, ly, dctx, dattn, sq, grads, residual):
+    def _self_attention_backward(self, st, i, ly, dctx, dattn, sq, grads, residual, wg=None, cap=None, ret_attn=None):
         """layer[i].attention.self from d context (the forward's own context O in the attention backward) and dattn, a gradient
-        of its map or None: the gradient at its input, plus residual (ds1) in the dgrad epilogue when given."""
+        of its map or None: the gradient at its input, plus residual (ds1) in the dgrad epilogue when given. ret_attn: the
+        returned map when retained (its .grad gets dO V^T)."""
         nseq, _, _, _, _, lt, L = st["dims"]
         H, heads = st["H"], st["heads"]
-        M = nseq * L
         ls = ly["seed"]
-        qkv_l = self._lin["l%d.qkv" % i]
-        dqkv = torch.empty(M, 3 * H, dtype=torch.bfloat16, device=dctx.device)
+        dqkv = torch.empty(nseq * L, 3 * H, dtype=torch.bfloat16, device=dctx.device)
         ops.attention_bwd(ly["qkv"], st["mask"], ly["ctx"], dctx, ly["lse"], dqkv, nseq, L, lt, heads, st["p_a"], ls + 1)
-        if dattn is not None:
+        if dattn is not None:      # a loss on attentions[i]: its dQ / dK added into dqkv
             drow = torch.empty(nseq, heads, L, dtype=torch.float32, device=dctx.device)
+            if cap is not None:
+                cap["dqkv_attn"] = dqkv.clone()
             ops.attention_probs_bwd(ly["qkv"], st["mask"], ly["lse"], dattn, drow, dqkv, nseq, L, lt, heads, st["p_a"], ls + 1)
+        if ret_attn is not None:
+            _add_retained_attention_grad(ret_attn, ly["qkv"], dctx, nseq, L, heads)
+        if cap is not None:
+            cap["dqkv"] = dqkv
+        return self._qkv_backward(st, i, ly, dqkv, sq, grads, residual, wg)
+
+    def _qkv_backward(self, st, i, ly, dqkv, sq, grads, residual, wg=None):
+        """The QKV linear of layer[i].attention.self from dqkv: its weight gradient, the last of the layer, and the gradient at
+        the layer input, plus residual (ds1) in the dgrad epilogue when given."""
+        M, H = dqkv.shape[0], st["H"]
+        qkv_l = self._lin["l%d.qkv" % i]
         if grads:
-            kw = self._split_wgrad_kw("qkv", qkv_l, dqkv, ly["x"], M)
-            sq.run(lambda: (ops.gemm(**kw), ops.colsum(dqkv, qkv_l.gb, M, 3 * H)), dqkv, ly["x"])
-        dxn = torch.empty(M, H, dtype=torch.bfloat16, device=dctx.device)
+            self._layer_wgrad(sq, wg, i, "qkv", dqkv, ly["x"], bias=True)
+        dxn = torch.empty(M, H, dtype=torch.bfloat16, device=dqkv.device)
         if residual is None:
             self._dgrad(qkv_l, dqkv, M, dxn)
         else:

@@ -111,10 +111,14 @@ def test_refusals_on_emulated_ops(weights):
 
 
 # ------------------------------------------------------------------------------------------------ planted faults
-def test_fault_residual_summed_by_autograd_breaks_the_bits(weights, monkeypatch):
+def test_fault_residual_owner_seen_as_not_running_breaks_the_bits(weights, monkeypatch):
     """The residual's two bf16 contributions summed by autograd (rounded twice) instead of handed over."""
     from clipbert_b200 import modeling
-    monkeypatch.setattr(modeling, "_engine_executes", lambda node: False)
+    runs = modeling._engine_runs
+
+    def partner_never_runs(node, captured):      # the residual's owner (_SelfNode, _InterNode) seen as not running
+        return runs(node, captured) and type(node).__name__ not in ("_SelfNodeBackward", "_InterNodeBackward")
+    monkeypatch.setattr(modeling, "_engine_runs", partner_never_runs)
     with emulated():
         with pytest.raises(AssertionError):
             TH.run_bits_observe_only(CPU, weights, "cpu", "bert")
@@ -150,14 +154,14 @@ def test_fault_wrong_dropout_seed_fails_the_oracle(weights, monkeypatch):
             TH.run_sites_against_oracle(CPU, weights, "cpu")
 
 
-def test_fault_replaced_context_in_the_attention_backward_fails_the_oracle(weights, monkeypatch):
+def test_fault_replaced_context_in_the_self_attention_piece_fails_the_oracle(weights, monkeypatch):
     """The attention backward fed the context a hook replaced instead of the forward's own O (its D = rowsum(dO o O) term)."""
     from clipbert_b200 import modeling
     orig = modeling._ClipBertHeadModel._self_attention_backward
 
-    def wrong(self, st, i, ly, dctx, dattn, sq, grads, residual):
+    def wrong(self, st, i, ly, *args, **kw):
         ly = dict(ly, ctx=ly["ctx"] * TH._head_scale().to(ly["ctx"].dtype)) if i == 5 else ly
-        return orig(self, st, i, ly, dctx, dattn, sq, grads, residual)
+        return orig(self, st, i, ly, *args, **kw)
     monkeypatch.setattr(modeling._ClipBertHeadModel, "_self_attention_backward", wrong)
     with emulated():
         with pytest.raises(AssertionError):
