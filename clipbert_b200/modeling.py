@@ -1668,6 +1668,8 @@ class _ClipBertHeadModel(nn.Module):
         if want_attn:       # same seed and bound word as the forward: the probabilities its context was made from
             probs = torch.empty(nseq, heads, L, L, dtype=torch.float32, device=dev)
             ops.attention_probs(qkv, st["mask"], lse, probs, nseq, L, lt, heads, st["p_a"], ls + 1)
+        if self._capture is not None:      # test hook: what layer i's maps are made from, on the default and the module path
+            self._capture["attn%d" % i] = dict(qkv=qkv, lse=lse, seed=ls + 1, word=st["drop_word"])
         return qkv, ctx, lse, probs
 
     def _attn_out_fwd(self, st, i, ctx, x):

@@ -21,7 +21,7 @@ def attention_probs(qkv, text_mask, lse, probs, nseq, l, lt, heads, p, seed):
     emulator's restated masks, with the bound device word folded into the seed)."""
     hd = qkv.shape[1] // (3 * heads)
     q, k = (x.double().reshape(nseq, l, heads, hd).permute(0, 2, 1, 3) for x in qkv.view(nseq, l, 3, heads * hd).unbind(2)[:2])
-    madd = torch.cat([(text_mask == 0).double() * -10000.0, torch.zeros(nseq, l - lt, dtype=torch.float64)], dim=1)
+    madd = torch.cat([(text_mask[:, :lt] == 0).double() * -10000.0, torch.zeros(nseq, l - lt, dtype=torch.float64)], dim=1)
     pr = torch.exp(q @ k.transpose(-1, -2) / math.sqrt(hd) + madd[:, None, None, :] - lse.double()[..., None])
     mult = ops_emulator._drop_mult(p, seed, D.attention_index(nseq, heads, l))
     if mult is not None:

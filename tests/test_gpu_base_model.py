@@ -1,19 +1,16 @@
-"""ClipBertBaseModel.forward (src/modeling/modeling.py:201-238) on the H100 path, and cb_attention_probs, the kernel behind its
-output_attentions.
+"""ClipBertBaseModel.forward (src/modeling/modeling.py:201-238) on the H100 path, and the argument checks of cb_attention_probs,
+the kernel behind its output_attentions (its results are checked element by element in test_gpu_attention_probs_elementwise.py).
 
-Kernel: against a float64 restatement from the same bf16 Q / K and the forward's own lse, at every sequence-length regime
-(one tile, the 48-row kernels, the multi-tile flash forward, 521 tokens), with and without padded captions and dropout; the
-dropped elements against tests/dropout_ref.py bit for bit; guard bands around the output. Module: outputs, hidden states and
-attentions against the reference-generated golden vectors and the oracle, gradients of every transformer parameter and of
-visual_inputs against fp32 autograd, dropout pattern of train-mode attentions, CUDA-graph replay, and the heads unchanged by
-the two flags. The test bodies take the device as an argument: tests/test_base_model_emulated.py replays them on CPU.
+Module: outputs, hidden states and attentions against the reference-generated golden vectors and the oracle, gradients of
+every transformer parameter and of visual_inputs against fp32 autograd, dropout pattern of train-mode attentions, CUDA-graph
+replay, and the heads unchanged by the two flags. The test bodies take the device as an argument: tests/test_base_model_emulated.py replays them on CPU.
 """
 
 import pytest
 import torch
 
 import dropout_ref as D
-from util import TOL_BF16_OP, TOL_FP32_E2E, TOL_GRAD, TOL_LOGITS, TOL_MATCHED, TOL_MATCHED_DEEP, cosine, make_cfg, relerr
+from util import TOL_FP32_E2E, TOL_GRAD, TOL_LOGITS, TOL_MATCHED, TOL_MATCHED_DEEP, cosine, make_cfg, relerr
 
 pytestmark = pytest.mark.gpu
 
@@ -35,48 +32,6 @@ def _qkv_case(L, padded, seed, nseq=2, dev="cpu"):
         mask[0, lt // 2:] = 0            # the [CLS] key stays live: a row never sees only masked keys
         mask[1, lt - 1] = 0
     return qkv.to(dev), mask.to(dev), lt
-
-
-def _ref_probs(qkv, mask, lse, nseq, L, lt):
-    q, k = (x.double().reshape(nseq, L, HEADS, 64).permute(0, 2, 1, 3) for x in qkv.cpu().view(nseq, L, 3, HEADS * 64).unbind(2)[:2])
-    madd = torch.cat([(mask.cpu() == 0).double() * -10000.0, torch.zeros(nseq, L - lt, dtype=torch.float64)], dim=1)
-    return torch.exp(q @ k.transpose(-1, -2) / 8.0 + madd[:, None, None, :] - lse.cpu().double()[..., None])
-
-
-GUARD = 16          # floats on either side of the output (64 bytes: the output stays 16-byte aligned)
-
-
-@pytest.mark.parametrize("p", [0.0, 0.1])
-@pytest.mark.parametrize("padded", [False, True])
-@pytest.mark.parametrize("L", [1, 17, 41, 48, 64, 65, 69, 128, 169, 521])
-def test_attention_probs_kernel(cuda, L, padded, p):
-    from clipbert_b200 import ops
-    nseq, seed = 2, 1234 + L
-    qkv, mask, lt = _qkv_case(L, padded, L, nseq, cuda)
-    ctx = torch.empty(nseq * L, HEADS * 64, dtype=torch.bfloat16, device=cuda)
-    lse = torch.empty(nseq, HEADS, L, dtype=torch.float32, device=cuda)
-    ops.dropout_offset_bind(None)
-    ops.attention_fwd(qkv, mask, ctx, lse, nseq, L, lt, HEADS, p, seed)
-    n = nseq * HEADS * L * L
-    buf = torch.full((n + 2 * GUARD,), -7.25, dtype=torch.float32, device=cuda)
-    probs = buf[GUARD: GUARD + n].view(nseq, HEADS, L, L)
-    ops.attention_probs(qkv, mask, lse, probs, nseq, L, lt, HEADS, p, seed)
-    buf = buf.cpu()
-    assert bool((buf[:GUARD] == -7.25).all()) and bool((buf[GUARD + n:] == -7.25).all()), "a write left the output"
-    got = probs.cpu().double()
-    ref = _ref_probs(qkv, mask, lse, nseq, L, lt)
-    if p > 0:
-        keep = torch.from_numpy(D.multipliers(D.effective_seed(seed, None), D.attention_index(nseq, HEADS, L), p)).double()
-        live = ref > 0
-        assert torch.equal(got[live] == 0, keep[live] == 0), "dropped elements differ from the restated mask"
-        ref = ref * keep
-    else:
-        assert float((got.sum(-1) - 1).abs().max()) < 2e-5          # rows of a softmax
-    assert float((got - ref).abs().max()) < 2e-5 + 2e-4 * float(ref.abs().max()), float((got - ref).abs().max())
-    # P @ V is the forward's context (which multiplies V by P rounded to bf16)
-    v = qkv.cpu().view(nseq, L, 3, HEADS, 64)[:, :, 2].double().permute(0, 2, 1, 3)
-    pv = (got @ v).permute(0, 2, 1, 3).reshape(nseq * L, HEADS * 64)
-    assert relerr(pv, ctx.float()) < 2 * TOL_BF16_OP, relerr(pv, ctx.float())
 
 
 def test_attention_probs_rejects_bad_arguments(cuda):
